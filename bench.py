@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — meshlet visibility pipeline on B200 (BASELINE.json metric: meshlets culled/s + tris rasterised/s,
+"""bench.py — meshlet visibility pipeline on H100 (BASELINE.json metric: meshlets culled/s + tris rasterised/s,
 % of HBM roofline) with the CPU reference arm beside it.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one frame of the hot path over the synthetic scene of BASELINE.json configs[1]
 ("1M meshlet instances, 1 camera, two-pass Hi-Z occlusion cull"): clear attachments -> cull_meshes ->
@@ -55,7 +55,12 @@ def parse_args():
     ap.add_argument("--unique-meshes", type=int, default=256,
                     help="256 = the contract scene (bounds L2-resident); 65536 makes bounds / vertex data stream from HBM")
     ap.add_argument("--parity-frames", type=int, default=3, help="N>1: frames of the pre-timing check N GPUs == 1 GPU (0 = skip)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (rank 0)")
+    args = ap.parse_args()
+    if args.impl == "reference" and args.dump_outputs:
+        ap.error("--dump-outputs writes the outputs of the CUDA path; it does not apply to --impl reference")
+    return args
 
 
 def measured_peak_hbm():
@@ -65,7 +70,7 @@ def measured_peak_hbm():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "nominal (H100 SXM data sheet, HBM3)"
 
 
 class ClockSampler:
@@ -116,6 +121,48 @@ class ClockSampler:
                     reasons.add(n)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": mx, "reasons": sorted(reasons),
                 "samples": len(sm)}
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes {name: array} as out_dir/<name>.npy (float32 / float64 only).  When the whole exceeds DUMP_LIMIT_BYTES, every
+    array of 1 MiB or more keeps a fixed, seeded sample of its flattened elements (same indices for the same shape), all of
+    them in the same proportion; smaller arrays are written whole."""
+    os.makedirs(out_dir, exist_ok=True)
+    big = sum(a.nbytes for a in arrays.values() if a.nbytes >= 1 << 20)
+    small = sum(a.nbytes for a in arrays.values()) - big
+    budget = DUMP_LIMIT_BYTES - small - (1 << 16)  # headroom for the .npy headers
+    for name, a in arrays.items():
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        if small + big > DUMP_LIMIT_BYTES and a.nbytes >= 1 << 20:
+            keep = int(a.size * budget // big)
+            if keep < a.size:
+                idx = np.sort(np.random.default_rng(0).choice(a.size, size=keep, replace=False))
+                a = a.ravel()[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a))
+
+
+def frame_outputs(pipe, vis64, multi, slot, triangles):
+    """What a caller of the timed frame receives: the vis-buffer image as depth + id (the two halves of each packed 64-bit
+    texel), the sorted survivor ids (their order is atomics order), the counters (meshlet instances, early and late
+    survivors, triangles rasterised; whole job), this rank's visibility mask and the Hi-Z pyramid."""
+    v = vis64.cpu().numpy().view(np.uint64)
+    if multi:
+        cnt_g, ids_g = pipe.ctx.mgpu_gathered(slot)
+        ids = np.concatenate(ids_g)
+        counters = np.append(cnt_g[:, :3].sum(axis=0), triangles)
+    else:
+        c = pipe.counters()
+        ids = pipe.ctx.visible_indices(c["early"] + c["late"])
+        counters = np.array([c["total"], c["early"], c["late"], triangles])
+    return {"vis_depth": (v >> np.uint64(32)).astype(np.uint32).view(np.float32),
+            "vis_id": (v & np.uint64(0xFFFFFFFF)).astype(np.float64),
+            "survivor_ids": np.sort(ids).astype(np.float64),
+            "counters": counters.astype(np.float64),
+            "visibility_mask": pipe.ctx.mask().astype(np.float64),
+            "hiz": np.concatenate([l.ravel() for l in pipe.ctx.hiz_levels()]).astype(np.float32)}
 
 
 def load_oracle():
@@ -203,15 +250,14 @@ def run_reference(args):
 
     cores = os.cpu_count() or 1
     scene = make_bench_scene(args, max(1, args.gpus))
-    # bounded sample: every step is one full frame of the same scene on all host threads
-    for _ in range(max(0, min(args.warmup, 1))):
+    # every step is one full frame of the same scene on all host threads
+    for _ in range(max(0, args.warmup)):
         cpu_frames(scene, 1, cores)
-    n = max(1, min(args.steps, 4))
+    n = max(1, args.steps)
     sec, last = cpu_frames(scene, n, cores)
     value = scene.max_meshlet_instance_count / sec
     line = {
-        "impl": "reference", "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": args.gpus, "steps": n, "warmup": min(args.warmup, 1),
-        "steps_requested": args.steps, "steps_note": "the CPU arm is capped at 4 timed frames / 1 warm-up frame (~0.1 s per frame)",
+        "impl": "reference", "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": args.gpus, "steps": n, "warmup": max(0, args.warmup),
         "ms_per_step": sec * 1e3, "higher_is_better": True, "scaling": "strong" if args.total_meshlets else "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": workload_config(args, scene),
         "cpu_baseline": {"value": value, "unit": UNIT, "cores": cores, "kind": "port",
@@ -474,6 +520,12 @@ def main():
     cnt = pipe.counters()
     if multi:
         pipe.ctx.check_status()  # survivor-gather overflow / peer time-out are errors, not footnotes
+    if args.dump_outputs:  # the last timed step's outputs: no frame has run since
+        tris = torch.tensor([float(cnt["triangles"])], dtype=torch.float64)
+        if multi:
+            dist.all_reduce(tris, op=dist.ReduceOp.SUM)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, frame_outputs(pipe, pipe.vis64_bufs[(K - 1) & 1], multi, (K - 1) & 1, float(tris.item())))
 
     dbg("timed region done", ms_per_step)
     # ---------------- per-kernel durations (same steps, eager launches, one CUDA event after every stage) ----------------
@@ -553,18 +605,8 @@ def main():
     algo_kernel = N_local * 16 + ((N_local + 31) // 32) * 8 + 2 * 4 * ((M_bits + 31) // 32) + 4 * S_late + I_local * 272
     t_late = stages_ms["cull_late"] * 1e-3
     achieved = algo_kernel / t_late / 1e9 if t_late > 0 else 0.0
-    traffic, traffic_src = None, None
-    prof = os.path.join(ROOT, "profiles", "ncu_cull_late_summary.json")
-    if os.path.exists(prof):
-        try:
-            pj = json.load(open(prof))
-            traffic, traffic_src = pj.get("dram_bytes_per_launch"), pj.get("source", "profiles/ncu_cull_late_summary.json")
-        except Exception:
-            traffic = None
     roofline = {"bound": "hbm", "kernel": "k_cull_meshlets<HIZ,OCC,LATE> (late pass)", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": traffic,
-                "traffic_note": f"constant from a committed ncu --set full capture ({traffic_src}), not measured in this run" if traffic else None,
-                "peak_source": peak_src,
+                "frac": achieved / peak, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": algo_kernel, "kernel_ms": stages_ms["cull_late"],
                 "frac_survey_8d_formula": (algo_survey / t_late / 1e9 / peak) if t_late > 0 else None,
                 "algorithmic_bytes_survey_8d_formula": algo_survey,

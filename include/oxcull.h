@@ -1,5 +1,5 @@
 /*
- * oxcull.h — C ABI of liboxcull.so: the B200-native meshlet visibility pipeline.
+ * oxcull.h — C ABI of liboxcull.so: the H100-native meshlet visibility pipeline.
  *
  * Drop-in boundary for the ONE hot path of oxylusengine/Oxylus that SURVEY.md §8 scopes:
  *   RendererInstance::cull_geometry      Oxylus/src/Render/Passes/CullGeometry.cpp:61-404

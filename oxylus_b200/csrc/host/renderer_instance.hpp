@@ -107,9 +107,9 @@ private:
     bool in_flight = false;
   } slots_[2];
   // Device->host copies of the last submitted frame, not yet enqueued.  They are issued from inside the NEXT frame,
-  // right after its early cull has been launched (or by wait(), whichever comes first): measured on B200, a copy-engine
-  // transfer running while the many short kernels at the head of a frame are being launched doubles their latency
-  // (+85 us / frame), whereas it is free next to the one long early-raster kernel (OXR_TRACE=1 shows the timeline).
+  // right after its early cull has been launched (or by wait(), whichever comes first): a copy-engine transfer running
+  // while the many short kernels at the head of a frame are being launched lengthens their latency, whereas it is free next
+  // to the one long early-raster kernel (OXR_TRACE=1 shows the timeline).
   struct PendingCopy {
     bool active = false;
     int slot = 0;

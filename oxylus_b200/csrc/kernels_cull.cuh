@@ -15,7 +15,7 @@ constexpr int CULL_THREADS = 256;
 #define OXC_CULL_ITEMS 2
 #endif
 #ifndef OXC_CULL_MIN_BLOCKS
-#define OXC_CULL_MIN_BLOCKS 4
+#define OXC_CULL_MIN_BLOCKS 3
 #endif
 constexpr int CULL_ITEMS = OXC_CULL_ITEMS;               // meshlet instances per thread per tile
 constexpr int CULL_TILE = CULL_THREADS * CULL_ITEMS;   // 512 per CTA iteration -> one atomic per 512
@@ -300,7 +300,7 @@ __global__ void __launch_bounds__(1024) k_scan_block_sums(uint32_t* block_sums, 
 // cull_meshes.slang:74-84 — expansion.  Deterministic: ascending mesh instance, ascending meshlet.
 // One warp per mesh instance writes its run with coalesced 64-bit stores.  EXPAND_SPLIT CTAs share one 256-instance block of
 // the scan (each redoes the block's cheap scan and expands 256 / EXPAND_SPLIT of its instances): with one CTA per block the
-// 8 MB of a 1 M scene were written by 25 CTAs in 14 us (ncu, round 2).
+// 8 MB of a 1 M scene would be written by only ~25 CTAs.
 constexpr int EXPAND_SPLIT = 8;
 __global__ void __launch_bounds__(CULL_MESHES_THREADS) k_expand_meshlet_instances(const uint32_t* __restrict__ counts,
                                                                                  const uint32_t* __restrict__ block_offsets,
@@ -348,8 +348,8 @@ __global__ void __launch_bounds__(CULL_MESHES_THREADS) k_expand_meshlet_instance
 //   ZERO = the pyramid is known to be the per-frame cleared image (early pass, SURVEY §8a quirk 1)
 //
 // Round-2 design: a three-stage pipeline with WARP-PRIVATE shared-memory queues, so every expensive stage runs on 32 live
-// lanes whatever fraction of the input reaches it (round 1 ran each stage on the lanes of a fixed tile: ncu showed the
-// occlusion stage executing 362 warp instructions per 32 input meshlets for ~16 live entries).
+// lanes whatever fraction of the input reaches it (running each stage on the lanes of a fixed tile leaves most lanes of the
+// expensive occlusion stage idle).
 //
 //   stage 0  one lane per meshlet-instance INDEX, 32 consecutive indices ("slab") per warp.  The (mesh instance, meshlet)
 //            pair is recovered from the slab table (8 B per 32 meshlets, written by the expansion) plus the per-instance
@@ -582,8 +582,7 @@ struct CullWarp {
   // The index -> (mesh instance, meshlet) -> {mask word, bounds} resolution is a chain of three dependent loads; a warp
   // owns only a handful of slabs, so the chain of slab k+1.. is issued while slab k is being tested:
   //     iteration k:   issue  slab-table entry of k+3,  InstCull tail of k+2,  mask word + bounds of k+1;   test k
-  // (round 1 staged the 8 B/meshlet id stream with the bulk-copy engine and still paid the dependent InstCull -> mask ->
-  // bounds chain per tile; the first cut of this kernel without the pipeline was latency-bound at 40 us per 1 M.)
+  // (without the pipeline the kernel waits on the dependent InstCull -> mask -> bounds chain of every slab: latency-bound.)
   struct Resolved { // slab whose mask word / bounds are in flight
     uint4 bounds;
     uint32_t maskw, inst, idx, vi;
@@ -632,9 +631,8 @@ struct CullWarp {
       // engine (TMA, cp.async.bulk -> SASS UBLKCP) and the warp picks the records up from shared memory a slab later —
       // north_star's "meshlet bounds ... staged through TMA into shared memory".  A slab that straddles instances falls back
       // to one 128-bit load per lane.
-      // OPT-IN build flag OXC_CULL_TMA_BOUNDS: verified bit-identical on B200 (all 50 GPU tests) but measured SLOWER than the
-      // plain loads — late cull 42.2 -> 47.6 us at 1 M: a warp-wide LDG.128 of 512 contiguous bytes is already four full
-      // 128-byte lines in one instruction, issued a slab ahead; the bulk copy adds two votes, an mbarrier round trip and a
+      // OPT-IN build flag OXC_CULL_TMA_BOUNDS: bit-identical, but a warp-wide LDG.128 of 512 contiguous bytes is already four
+      // full 128-byte lines in one instruction, issued a slab ahead; the bulk copy adds two votes, an mbarrier round trip and a
       // shared-memory read per slab and saves nothing.  Default: off.
 #ifdef OXC_CULL_TMA_BOUNDS
       const uint32_t nv = __popc(__ballot_sync(0xffffffffu, r.valid)); // validity is a prefix of the lanes
@@ -718,13 +716,10 @@ struct CullWarp {
   }
 };
 
-#ifndef OXC_CULL_MIN_BLOCKS_EARLY
-#define OXC_CULL_MIN_BLOCKS_EARLY 3
-#endif
-// launch bounds per variant (measured on B200, round 2): the early pass (queue 0 -> stage A on compacted items) runs 21.6 us at
-// 3 CTAs / SM (85 registers) vs 26.6 us at 4; the late pass is indifferent (42 us) and keeps 4 CTAs / SM for the latency it hides
+// launch bounds: OXC_CULL_MIN_BLOCKS = 3 CTAs / SM for every variant.  At 4 (64 registers) the sm_90a build of the late pass
+// spills; at 3 (80 registers) it does not, and its time on H100 SXM stays within run-to-run spread (BASELINE.md 5.2)
 template <bool HIZ, bool OCC, bool LATE, bool ZERO>
-__global__ void __launch_bounds__(CULL_THREADS, (OCC && !LATE) ? OXC_CULL_MIN_BLOCKS_EARLY : OXC_CULL_MIN_BLOCKS) k_cull_meshlets(const __grid_constant__ CullParams p) {
+__global__ void __launch_bounds__(CULL_THREADS, OXC_CULL_MIN_BLOCKS) k_cull_meshlets(const __grid_constant__ CullParams p) {
   extern __shared__ __align__(16) unsigned char cull_smem_raw[];
   using Shared = CullShared<OCC && !LATE>;
   Shared& sh = *reinterpret_cast<Shared*>(cull_smem_raw);

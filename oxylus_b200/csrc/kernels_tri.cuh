@@ -156,8 +156,10 @@ __global__ void __launch_bounds__(TRI_THREADS) k_cull_triangles(const __grid_con
   }
 }
 
+// 3 CTAs / SM (80 registers) rather than 4 (64 registers, more spills in the pixel loop): on H100 SXM at 1 M meshlet
+// instances / 1080p the early raster takes 400-405 instead of 434-440 us, the late one 71-72 instead of 77 us (BASELINE.md 5.2)
 #ifndef OXC_RASTER_MIN_BLOCKS
-#define OXC_RASTER_MIN_BLOCKS 4
+#define OXC_RASTER_MIN_BLOCKS 3
 #endif
 #ifndef OXC_RASTER_BIG_PIXELS
 #define OXC_RASTER_BIG_PIXELS 32
@@ -283,8 +285,8 @@ OXC_DI bool big_push_warp(const TriParams& p, const TriSetup& s, uint32_t data, 
 }
 
 // One warp per queued chunk; the chunk is covered in 8x4-pixel tiles (raster spec steps 5-6).  Chunks are dealt to the warps
-// of the grid round-robin: round 1 took them from a counter, and ncu showed the kernel spending 12-22 us at 4-11 % issue
-// utilisation on ~9500 same-address atomics — every warp paid one just to learn that the queue was empty.
+// of the grid round-robin: taking them from a counter costs every warp one same-address atomic, even just to learn that the
+// queue is empty.
 __global__ void __launch_bounds__(256) k_raster_big(const __grid_constant__ TriParams p) {
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t total = min(p.big_counters[0], p.big_capacity);
@@ -312,16 +314,16 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
 #ifdef OXC_RASTER_SMEM_MICRO
   // the meshlet's micro-index run (<= 192 B, scene.slang:336-342) staged in shared memory: 49 words cover it plus the byte skew
   // of its start.  Two coalesced loads per warp, issued before the vertex transform, replace three dependent L1 loads + shifts
-  // per triangle (7.4 % of the kernel's stall samples): early raster 306 -> 294 us.  (The same staging through the bulk-copy
-  // engine, OXC_RASTER_TMA_MICRO below, is slower: its mbarrier state spills at the 64-register cap.)
+  // per triangle.  (The same staging through the bulk-copy engine, OXC_RASTER_TMA_MICRO below, adds live mbarrier state to a
+  // kernel that already spills at its register bound; not timed on H100.)
   __shared__ uint32_t micro_w[TRI_WARPS][52];
 #endif
 #ifdef OXC_RASTER_TMA_MICRO
   // OPT-IN (north_star: "micro-index data staged through TMA into shared memory"): the meshlet's micro-index run (<= 192 B,
   // scene.slang:336-342) is staged by the bulk-copy engine (cp.async.bulk -> SASS UBLKCP) while the vertices are transformed, and
-  // the 3 byte fetches per triangle become shared-memory byte loads.  Bit-identical output (all 50 GPU tests), but measured
-  // SLOWER on B200 at the 64-register cap this kernel runs at: early raster 306 -> 330 us, late 61 -> 67 us (the three extra live
-  // values push 150 more bytes of spills into the hot loop; the L1-resident LDG it replaces was never the bottleneck).  Default off.
+  // the 3 byte fetches per triangle become shared-memory byte loads.  Bit-identical output, but the three extra live values
+  // add spills to a hot loop that already spills at the kernel's register bound (80 at 3 CTAs / SM), and the L1-resident LDG
+  // it replaces is not the bottleneck.  Not timed on H100.  Default off.
   __shared__ __align__(16) uint8_t micro_all[TRI_WARPS][MICRO_STAGE_BYTES];
   __shared__ __align__(8) uint64_t micro_bar[TRI_WARPS];
   if (lane == 0) { mbar_init(&micro_bar[warp], 1); mbar_fence_init(); }
@@ -342,17 +344,15 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
   // 0..nb-1 each chase one meshlet header, so nb pointer chases are in flight together.
   // Guided self-scheduling: the grab size shrinks with the work that is left (remaining / (2 x warps in the grid), between 1
   // and RASTER_BATCH), so the kernel ends with single-meshlet grabs.
-  // Measured in round 2 (per-warp %globaltimer stamps, tools/raster_stats.py): a grab costs ~3.8 us in the early and ~7 us in
-  // the late pass (thousands of warps on one L2 atomic address).  Dealing the list onto 32 interleaved sequences with one
-  // counter each cut the late pass (119 -> 97 us) but cost the early pass more (365 -> 388..421 us: the extra scheduler
-  // state spills at the 64-register cap), so the single counter stays.
+  // A grab is slow (thousands of warps on one L2 atomic address; tools/raster_stats.py times it per warp).  Dealing the list
+  // onto 32 interleaved sequences with one counter each would shorten the late pass, but the extra scheduler state is more
+  // live registers in a kernel that already spills at its bound, so the single counter stays (not re-timed on H100).
   const uint32_t n_warps2 = gridDim.x * TRI_WARPS * 2u;
   // PREFETCH_GRAB (late pass): the grab for the NEXT batch is issued before the current batch is processed, so the atomic's
-  // round trip (measured ~7 us in the late pass: every warp of the GPU on one address, few meshlets per warp) overlaps a batch
-  // of rasterisation.  A/B on B200: late pass 114 -> 98 us; the early pass (55 meshlets per warp, 12 grabs) loses more balance
-  // from the batch each warp holds in reserve than it gains (375 -> 400 us; issuing the grab only when the last meshlet of the
-  // batch starts: 432 us; 3 CTAs / SM with 80 registers and no spills: 400 us), so it keeps the plain grab at 4 CTAs / SM: its
-  // waiting warps cost nothing while 31 others have instructions to issue.
+  // round trip (long in the late pass: every warp of the GPU on one address, few meshlets per warp) overlaps a batch of
+  // rasterisation.  The early pass (many meshlets per warp, few grabs) loses more balance from the batch each warp holds in
+  // reserve than it gains, so it keeps the plain grab: its waiting warps cost nothing while the others have instructions to
+  // issue.
   uint32_t g_next = 0, batch_next = 1;
   if (PREFETCH_GRAB && lane == 0) {
     batch_next = min((uint32_t)RASTER_BATCH, max(1u, count / n_warps2));
@@ -506,8 +506,7 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
         bool big = draw && (bw * bh > RASTER_BIG_PIXELS);
         if (draw && !big) raster_small(s, data, p.visbuf, p.width);
         // a triangle of a few chunks is pushed by its own lane; one of many chunks (a screen-filling triangle is ~1000) is
-        // pushed by the whole warp below — per-warp timestamps showed single lanes spending 30-80 us writing chunk entries,
-        // the tail of both raster launches
+        // pushed by the whole warp below — a single lane writing them all becomes the tail of the raster launch
         const bool few = big && big_chunk_count(s) <= BIG_PUSH_ALONE;
         if (few && p.big_queue && big_push(p, s, data)) big = false; // deferred to k_raster_big
         uint32_t big_mask = __ballot_sync(0xffffffffu, big);
@@ -548,6 +547,8 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
     unsigned long long* rec = reinterpret_cast<unsigned long long*>(p.big_queue) + (size_t)p.big_capacity * 8 + 128 +
                               ((size_t)(p.late ? gridDim.x * TRI_WARPS : 0) + blockIdx.x * TRI_WARPS + warp) * 6;
     rec[0] = t_entry; rec[1] = t_exit; rec[2] = t_chase; rec[3] = t_proc; rec[4] = n_done; rec[5] = n_grabs;
+    if (blockIdx.x == 0 && warp == 0) // statistics slot 45: the grid the records are laid out by (tools/raster_stats.py)
+      reinterpret_cast<unsigned long long*>(p.big_queue)[(size_t)p.big_capacity * 8 + (p.late ? 64 : 0) + 45] = gridDim.x;
   }
 #endif
 #pragma unroll

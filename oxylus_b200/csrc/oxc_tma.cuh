@@ -1,4 +1,4 @@
-// oxc_tma.cuh — the Blackwell / Hopper bulk asynchronous copy engine (TMA) in its 1-D form: cp.async.bulk global -> shared with
+// oxc_tma.cuh — the Hopper bulk asynchronous copy engine (TMA) in its 1-D form: cp.async.bulk global -> shared with
 // completion on an mbarrier (SASS: UBLKCP + SYNCS), plus an L1 prefetch hint.  Used by the raster (micro-index runs) and
 // available to the cull kernels.
 #pragma once

@@ -1,4 +1,4 @@
-// oxc_types.cuh — device-side records of the B200 meshlet visibility pipeline.
+// oxc_types.cuh — device-side records of the H100 meshlet visibility pipeline.
 //
 // HBM layout (DESIGN.md §layout):
 //   meshlet_instances  N x 8 B   (SceneGPU.hpp:106-109)      streamed, coalesced 64-bit loads

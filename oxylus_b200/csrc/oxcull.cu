@@ -1,5 +1,5 @@
 // oxcull.cu — liboxcull.so: context management and the C ABI of include/oxcull.h.
-// Every entry point enqueues hand-written sm_100a kernels (kernels_*.cuh) on the caller's stream.
+// Every entry point enqueues hand-written sm_90a kernels (kernels_*.cuh) on the caller's stream.
 // There is no CPU fallback: without a CUDA device oxc_create fails with OXC_E_NO_DEVICE.
 #include <cuda_runtime.h>
 
@@ -242,7 +242,7 @@ extern "C" {
 
 const char* oxc_last_error(void) { return g_err; }
 uint64_t oxc_kernel_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
-const char* oxc_version(void) { return "oxcull 0.1 (sm_100a)"; }
+const char* oxc_version(void) { return "oxcull 0.1 (sm_90a)"; }
 
 int oxc_create(int device, const OxcCreateInfo* info, OxcContext** out_ctx) {
   if (!info || !out_ctx) return fail(OXC_E_INVALID, "null argument");

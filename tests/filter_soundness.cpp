@@ -3,7 +3,7 @@
 // The kernel takes a decision with cheap arithmetic (fma chains, MUFU rcp / rsqrt) whenever an error bound proves that the
 // canonical evaluation — the one the CPU oracle restates and every GPU parity test compares against — must agree, and falls
 // back to the canonical path otherwise.  "Bit-identical for EVERY input" therefore rests on those bounds.  The GPU tests only
-// ever see what one B200's MUFU returns; this program compiles the very same device headers for the host (tests/host_shim/:
+// ever see what one GPU's MUFU returns; this program compiles the very same device headers for the host (tests/host_shim/:
 // each __f*_rn intrinsic is one IEEE binary32 operation under -ffp-contract=off, fmaf is exact) and replaces the two
 // approximate units by an ADVERSARY that returns any float the PTX ISA's accuracy statement allows (rcp.approx: 2^-23
 // relative, rsqrt.approx: 2^-22.4 relative, subnormal results flushed): always the lowest, always the highest, the nearest,

@@ -300,7 +300,7 @@ static inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {
   memset(p, 0, sizeof *p);
   snprintf(p->name, sizeof p->name, "SIMT emulator (host)");
-  p->multiProcessorCount = 2; p->major = 10; p->minor = 0; p->totalGlobalMem = (size_t)8 << 30; p->sharedMemPerBlockOptin = 227 * 1024;
+  p->multiProcessorCount = 2; p->major = 9; p->minor = 0; p->totalGlobalMem = (size_t)8 << 30; p->sharedMemPerBlockOptin = 227 * 1024;
   return cudaSuccess;
 }
 static inline cudaError_t cudaDeviceSynchronize() { return cudaSuccess; }

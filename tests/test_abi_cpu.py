@@ -100,7 +100,7 @@ def test_product_never_imports_oracle():
 
 def test_product_never_uses_the_test_emulator():
     """tests/host_shim/ (host stand-ins for the CUDA headers, the SIMT emulator) is test infrastructure: nothing under oxylus_b200/
-    includes it, builds it or loads an emulated library, and the shipped liboxcull.so is the nvcc build (it holds sm_100a device
+    includes it, builds it or loads an emulated library, and the shipped liboxcull.so is the nvcc build (it holds sm_90a device
     code and none of the emulator's symbols).  The only trace in the product sources is the OXC_HOST_SOUNDNESS_HARNESS guard around
     inline PTX, which no product build defines."""
     pkg = os.path.join(ROOT, "oxylus_b200")
@@ -115,7 +115,7 @@ def test_product_never_uses_the_test_emulator():
     assert "simt::" not in syms
     if shutil.which("cuobjdump"):
         elf = subprocess.run(["cuobjdump", "-lelf", capi.lib_path()], capture_output=True, text=True).stdout
-        assert "sm_100a" in elf, elf[:300]
+        assert "sm_90a" in elf, elf[:300]
 
 
 def _build_host_min(tmp_path):

@@ -1421,8 +1421,8 @@ def test_plain_c_host_runs(capi, tmp_path):
     assert "768 of 3072 pixels" in res.stdout
 
 
-# ---- written after the round's last GPU second was spent (DESIGN.md §4.3): these ran on the SIMT-emulated library only (plain, ASan,
-#      UBSan builds); they sit at the end of the file so that the B200-validated tests above are counted first ----
+# ---- alpha-tested discard: mip chains, golden fixture, random triangles, overdraw counter, clip-pass interaction, plain-C host
+#      (DESIGN.md §4.3); also run on the SIMT-emulated library (plain, ASan, UBSan builds) ----
 
 
 def test_alpha_discard_mipmapped_parity(capi, orc):
@@ -1553,7 +1553,7 @@ def test_alpha_discard_random_triangles(capi, orc):
 
     import os
 
-    n_seeds = int(os.environ.get("OXC_ALPHA_FUZZ_SEEDS", "6"))  # profiles/r2_emulated_alpha_fuzz.log: 400 seeds on the emulated library
+    n_seeds = int(os.environ.get("OXC_ALPHA_FUZZ_SEEDS", "6"))  # more seeds: OXC_ALPHA_FUZZ_SEEDS=400 on the emulated library
     discarding = 0
     for seed in range(n_seeds):
         rng = np.random.default_rng(100 + seed)

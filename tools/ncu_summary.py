@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Summarise an ncu report (--set full) into a small JSON for profiles/:  python tools/ncu_summary.py <report.ncu-rep> <out.json> [note]"""
+"""Summarise an ncu report (--set full) into a small JSON:  python tools/ncu_summary.py <report.ncu-rep> <out.json> [note]"""
 import csv
 import io
 import json

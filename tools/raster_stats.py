@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Instrumentation run (variant library built with -DOXC_RASTER_STATS): per round of 32 triangles, how long is the longest
-per-lane pixel loop?  Usage on the GPU box:  OXC_LIB_PATH=$PWD/oxylus_b200/liboxcull_stats.so python tools/raster_stats.py"""
+per-lane pixel loop?  Usage:  OXC_LIB_PATH=$PWD/oxylus_b200/liboxcull_stats.so python tools/raster_stats.py"""
 import os
 import sys
 
@@ -37,7 +37,10 @@ for name, o in (("early", 0), ("late", 64)):
           f"{st[o + 40] / 32 / frames:.0f}")
 
 # ---- per-warp timeline of the last frame's two raster launches (stats build only) ----
-nw = 148 * 4 * 8
+# the grid each launch used (statistics slot 45 of its half) x 8 warps per CTA; late records follow the early launch's
+grids = pipe.ctx.download(pipe.ctx.debug_stats_ptr(), np.uint64, n)[[45, 64 + 45]].astype(np.int64)
+assert grids[0] == grids[1] > 0, grids
+nw = int(grids[0]) * 8
 rec = pipe.ctx.download(pipe.ctx.debug_stats_ptr() + 128 * 8, np.uint64, 2 * nw * 6).reshape(2, nw, 6).astype(np.int64)
 for name, r in (("early", rec[0]), ("late", rec[1])):
     r = r[r[:, 0] > 0]

@@ -1,16 +1,10 @@
-// pipes.cu — issue-rate micro-benchmark for the instruction kinds the cull / raster kernels are made of (sm_100a).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a --fmad=false -O3 -o pipes pipes.cu ; run on the GPU box.
+// pipes.cu — issue-rate micro-benchmark for the instruction kinds the cull / raster kernels are made of (sm_90a).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a --fmad=false -O3 -o pipes pipes.cu ; run on an H100.
 // Prints warp-instructions / clk / SM for each kind with 8 independent chains per thread (ILP) and 32 warps / SM.
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdint>
-typedef unsigned long long u64;
 #define DI __device__ __forceinline__
-DI u64 pk(float a, float b) { u64 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-DI u64 add2(u64 a, u64 b) { u64 c; asm volatile("add.rn.f32x2 %0, %1, %2;" : "=l"(c) : "l"(a), "l"(b)); return c; }
-DI u64 mul2(u64 a, u64 b) { u64 c; asm volatile("mul.rn.f32x2 %0, %1, %2;" : "=l"(c) : "l"(a), "l"(b)); return c; }
-DI u64 fma2(u64 a, u64 b, u64 d) { u64 c; asm volatile("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(c) : "l"(a), "l"(b), "l"(d)); return c; }
-DI float min3(float a, float b, float c) { float r; asm volatile("min.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c)); return r; }
 DI float rcpa(float a) { float r; asm volatile("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(a)); return r; }
 
 constexpr int ITERS = 4096;
@@ -19,11 +13,9 @@ constexpr int CH = 8;
 template <int KIND>
 __global__ void __launch_bounds__(256) k(float* out, float seed, long long* clk) {
   float x[CH], y = seed * 1.0001f, z = seed * 0.5f;
-  u64 p[CH];
   uint32_t n[CH];
 #pragma unroll
-  for (int i = 0; i < CH; i++) { x[i] = seed + i + threadIdx.x; p[i] = pk(x[i], x[i] + 1.f); n[i] = threadIdx.x + i; }
-  const u64 py = pk(y, y), pz = pk(z, z);
+  for (int i = 0; i < CH; i++) { x[i] = seed + i + threadIdx.x; n[i] = threadIdx.x + i; }
   long long t0 = clock64();
 #pragma unroll 1
   for (int it = 0; it < ITERS; it++) {
@@ -32,16 +24,11 @@ __global__ void __launch_bounds__(256) k(float* out, float seed, long long* clk)
       if (KIND == 0) x[i] = __fadd_rn(x[i], y);
       if (KIND == 1) x[i] = __fmul_rn(x[i], y);
       if (KIND == 2) x[i] = __fmaf_rn(x[i], y, z);
-      if (KIND == 3) p[i] = add2(p[i], py);
-      if (KIND == 4) p[i] = mul2(p[i], py);
-      if (KIND == 5) p[i] = fma2(p[i], py, pz);
       if (KIND == 6) x[i] = fminf(x[i], y);
-      if (KIND == 7) x[i] = min3(x[i], y, z);
       if (KIND == 8) x[i] = rcpa(x[i]);
       if (KIND == 9) n[i] = (n[i] ^ (n[i] >> 3)) + 0x9E3779B9u;           // LOP3/SHF + IADD
       if (KIND == 10) { x[i] = __fadd_rn(x[i], y); n[i] = n[i] * 3u + 7u; } // FADD + IMAD
       if (KIND == 11) { x[i] = __fadd_rn(x[i], y); n[i] = (n[i] + 77u) ^ 5u; } // FADD + IADD/LOP (alu)
-      if (KIND == 12) { p[i] = add2(p[i], py); n[i] = (n[i] + 77u) ^ 5u; }    // FADD2 + alu
       if (KIND == 13) x[i] = __fdiv_rn(x[i], y);
       if (KIND == 14) x[i] = __fsqrt_rn(x[i]);
     }
@@ -49,7 +36,7 @@ __global__ void __launch_bounds__(256) k(float* out, float seed, long long* clk)
   long long t1 = clock64();
   float acc = 0.f;
 #pragma unroll
-  for (int i = 0; i < CH; i++) { acc += x[i] + __uint_as_float((uint32_t)p[i]) + __uint_as_float((uint32_t)(p[i] >> 32)) + (float)n[i]; }
+  for (int i = 0; i < CH; i++) { acc += x[i] + (float)n[i]; }
   out[blockIdx.x * blockDim.x + threadIdx.x] = acc;
   if (threadIdx.x == 0 && blockIdx.x == 0) *clk = t1 - t0;
 }
@@ -70,9 +57,9 @@ void run(const char* name, float ops_per_iter) {
 }
 
 int main() {
-  run<0>("FADD", 1); run<1>("FMUL", 1); run<2>("FFMA", 1); run<3>("FADD2", 1); run<4>("FMUL2", 1); run<5>("FFMA2", 1);
-  run<6>("FMNMX", 1); run<7>("FMNMX3", 1); run<8>("MUFU.RCP", 1); run<9>("LOP/SHF+IADD (2 ops)", 2);
-  run<10>("FADD+IMAD (2 ops)", 2); run<11>("FADD+IADD+LOP (3 ops)", 3); run<12>("FADD2+IADD+LOP (3 ops)", 3);
+  run<0>("FADD", 1); run<1>("FMUL", 1); run<2>("FFMA", 1);
+  run<6>("FMNMX", 1); run<8>("MUFU.RCP", 1); run<9>("LOP/SHF+IADD (2 ops)", 2);
+  run<10>("FADD+IMAD (2 ops)", 2); run<11>("FADD+IADD+LOP (3 ops)", 3);
   run<13>("fdiv_rn (1 call)", 1); run<14>("fsqrt_rn (1 call)", 1);
   return 0;
 }
