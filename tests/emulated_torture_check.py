@@ -4,7 +4,10 @@
 column, at the camera, far away.  No mesh builder produces such records, but the reference's shaders — and therefore the oracle —
 are defined for them, and "bit-identical to the canonical evaluation for every input" has to hold for them too (this is the
 scenario that found the cone filter turning a NaN radius into 0 and the frustum filter assuming h >= 0).
-Run by tests/test_emulated_library_cpu.py against the SIMT-emulated library; works unchanged on a GPU.
+Runs against whichever library capi loads: tests/test_emulated_library_cpu.py runs main() on the SIMT-emulated library, and
+tests/test_gpu_variants.py::test_hostile_frames runs every case of cases() on the GPU, where rcp.approx.ftz / rsqrt.approx.ftz
+give the hardware's flush-to-zero results that the emulator's IEEE stand-ins do not.  (tests/conftest.py imports mutate() under
+this module's name.)
 
     python tests/emulated_torture_check.py [seeds]"""
 import copy
@@ -147,29 +150,40 @@ def frames_equal(sc, frames=2, cams=None, occluder_depth=None, alpha=False):
     return ok
 
 
-def main():
-    seeds = int(sys.argv[1]) if len(sys.argv) > 1 else 2
-    base = synth.make_scene(8000, config_index=2, width=320, height=180, n_unique_meshes=24, max_lods=2, ragged=True)
-    bad = []
-    for seed in range(seeds):
-        for mode in ("bounds", "cones", "vertices", "transforms", "all"):
-            if not frames_equal(mutate(base, np.random.default_rng(seed * 10 + 1), mode)):
-                bad.append((seed, mode))
-    if not frames_equal(base, cams=hostile_cameras(base)):
-        bad.append("cameras")
-    # the same hostility with a material table set: NaN / Inf uv, positions and cameras reach the interpolation, the level selection
-    # and the texel addressing of the alpha test
-    for seed in range(seeds):
-        if not frames_equal(mutate(base, np.random.default_rng(seed * 10 + 1), "all"), alpha=True):
-            bad.append((seed, "all + alpha"))
-    if not frames_equal(base, cams=hostile_cameras(base), alpha=True):
-        bad.append("cameras + alpha")
+def base_scene():
+    return synth.make_scene(8000, config_index=2, width=320, height=180, n_unique_meshes=24, max_lods=2, ragged=True)
+
+
+def hostile_depth(base):
+    """the scene's occluder depth with 1 % of its pixels NaN, +-Inf, out of [0, 1], denormal or -0"""
     depth = base.occluder_depth.copy()
     rng = np.random.default_rng(3)
     sel = rng.random(depth.shape) < 0.01
     depth[sel] = rng.choice(np.array([np.nan, np.inf, -np.inf, -1.0, 2.0, 1e-45, -0.0], dtype=np.float32), int(sel.sum()))
-    if not frames_equal(base, occluder_depth=depth):
-        bad.append("external depth")
+    return depth
+
+
+def cases(seeds=2):
+    """(label, mutation mode or None, seed, hostile cameras, material table, hostile external depth) of every check main() runs.
+    With a material table the same hostility reaches the alpha test's interpolation, level selection and texel addressing."""
+    out = [(f"{mode} seed {seed}", mode, seed, False, False, False) for seed in range(seeds)
+           for mode in ("bounds", "cones", "vertices", "transforms", "all")]
+    out.append(("cameras", None, 0, True, False, False))
+    out += [(f"all + alpha seed {seed}", "all", seed, False, True, False) for seed in range(seeds)]
+    out += [("cameras + alpha", None, 0, True, True, False), ("external depth", None, 0, False, False, True)]
+    return out
+
+
+def run_case(base, case):
+    _, mode, seed, cams, alpha, depth = case
+    sc = base if mode is None else mutate(base, np.random.default_rng(seed * 10 + 1), mode)
+    return frames_equal(sc, cams=hostile_cameras(base) if cams else None, occluder_depth=hostile_depth(base) if depth else None, alpha=alpha)
+
+
+def main():
+    seeds = int(sys.argv[1]) if len(sys.argv) > 1 else 2
+    base = base_scene()
+    bad = [case[0] for case in cases(seeds) if not run_case(base, case)]
     print(f"{seeds * 5} hostile scenes x 2 frames, 10 hostile cameras, {seeds} hostile scenes + 10 hostile cameras with a material table, hostile external depth: "
           f"{'ok' if not bad else 'MISMATCH ' + repr(bad)}")
     sys.exit(1 if bad else 0)

@@ -87,6 +87,16 @@ def test_hostile_inputs_on_the_simt_emulator(emulated):
     assert res.returncode == 0 and res.stdout.strip().endswith("ok"), res.stdout[-2000:] + res.stderr[-2000:]
 
 
+def test_gpu_variants_on_the_simt_emulator(emulated):
+    """tests/test_gpu_variants.py: all nine k_cull_meshlets instantiations over three pyramid states, every flag subset and a second
+    camera, the occlusion toggle across frames, the mesh-level flags and the automatic shard id base, mixed cameras through the
+    raster and the triangle cull.  Its hostile frames are the torture script's, which test_hostile_inputs_on_the_simt_emulator runs."""
+    res = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", "test_gpu_variants.py"), "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider",
+                          "-k", "not hostile_frames"], cwd=ROOT, env=emulated, capture_output=True, text=True, timeout=900)
+    m = re.search(r"(\d+) passed", res.stdout)
+    assert res.returncode == 0 and m and int(m.group(1)) >= 18 and "skipped" not in res.stdout, res.stdout[-3000:] + res.stderr[-2000:]
+
+
 def test_gpu_parity_suite_with_hostile_scenes_on_the_simt_emulator(emulated):
     """the same suite once more with OXC_TEST_HOSTILE_SCENES set (tests/conftest.py): every synthetic scene the tests build gets
     the hostile record contents above, vertex positions included — hpb / multiview / plain culls, triangle cull, clip and chunk
