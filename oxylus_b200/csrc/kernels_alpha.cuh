@@ -97,8 +97,11 @@ OXC_DI void raster_box_alpha(const TriSetup& s, const AlphaMaterial& m, const Al
 }
 
 constexpr int ALPHA_THREADS = 128, ALPHA_WARPS = ALPHA_THREADS / 32;
+// bbox area above which the whole warp rasterises the triangle together.  Kept at 32 when the vis-buffer raster's threshold
+// rose to 128: every pixel here also samples the alpha texture, and this kernel has not been timed on H100.
+constexpr int ALPHA_BIG_PIXELS = 32;
 
-// one triangle's set-up handed from its lane to the whole warp (triangles of more than RASTER_BIG_PIXELS pixels)
+// one triangle's set-up handed from its lane to the whole warp (triangles of more than ALPHA_BIG_PIXELS pixels)
 struct AlphaBigRecord {
   TriSetup s;
   AlphaTri t;
@@ -173,7 +176,7 @@ __global__ void __launch_bounds__(ALPHA_THREADS) k_raster_alpha(const __grid_con
             const int why = tri_setup(to_screen(c0, p.f_width, p.f_height), to_screen(c1, p.f_width, p.f_height),
                                       to_screen(c2, p.f_width, p.f_height), p.width, p.height, s);
             if (why == TRI_DRAW) {
-              big = (s.px1 - s.px0 + 1) * (s.py1 - s.py0 + 1) > RASTER_BIG_PIXELS;
+              big = (s.px1 - s.px0 + 1) * (s.py1 - s.py0 + 1) > ALPHA_BIG_PIXELS;
               if (!big) raster_box_alpha<OVERDRAW>(s, m, at, data, p.visbuf, a.overdraw, p.width);
             } else if (why == TRI_INVALID_VERTEX) { // a vertex at w <= 0 / beyond the snap range: clipped like the plain raster does,
               ClipVertUV poly[2][12];                // with uv carried through the cuts (alpha spec step 3)
@@ -194,7 +197,7 @@ __global__ void __launch_bounds__(ALPHA_THREADS) k_raster_alpha(const __grid_con
           }
         } // else: malformed meshlet, the triangle is skipped like in the plain raster
       }
-      // triangles above RASTER_BIG_PIXELS pixels: the whole warp covers the bounding box in 8x4-pixel tiles
+      // triangles above ALPHA_BIG_PIXELS pixels: the whole warp covers the bounding box in 8x4-pixel tiles
       uint32_t big_mask = __ballot_sync(0xffffffffu, big);
       while (big_mask) {
         const uint32_t src = (uint32_t)__ffs(big_mask) - 1u;
