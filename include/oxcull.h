@@ -617,6 +617,78 @@ int oxc_mark_visible_pages(OxcContext* ctx, const float inv_projection_view[16] 
                            uint32_t* page_occupancy_dev, uint32_t* request_count_dev, int32_t* requests_dev /* int3 per request */,
                            uint32_t request_capacity, void* stream);
 
+/* ---- VSM page bookkeeping (SURVEY §8f.4): the passes of Shadowmaps.cpp:100-430 between the depth image and the shadow raster ----
+ * One frame is, on one stream (oxr_vsm_update_pages runs exactly this):
+ *   oxc_vsm_begin_frame         vuk::clear_image on sun_moved (:143-148), rmvsm_reset_page_visibility (:150-163), zero-filled
+ *                               page_occupancy (:224-232) and request count
+ *   oxc_vsm_invalidate_pages    rmvsm_invalidate_pages (:167-222), only when !sun_moved and there are dirty mesh instances
+ *   oxc_mark_visible_pages      rmvsm_mark_visible_pages (:234-275), request_count_dev = &allocator->active_request_count
+ *   oxc_vsm_allocate_pages      rmvsm_free_invisible_pages, rmvsm_build_free_page_list, rmvsm_allocate_pages (:277-329) and
+ *                               rmvsm_mark_dirty_pages (:373-406)
+ *   oxc_build_hpb               rmvsm_downsample_hpb (:331-371)
+ *   oxc_vsm_clear_dirty_pages   rmvsm_clear_dirty_pages (:408-431)
+ * then oxc_cull_meshlets_hpb_dirty_dev culls the shadow casters against the new bitmap.  Everything stays on the device: no call
+ * reads a count back, so the sequence can be captured into a CUDA graph.
+ * Page table entries: rmvsm.slang:16-34 (Visible 1, Dirty 2, Backed 4, Invalidated 8, AllocationFailed 16; physical page index in
+ * bits 16-31).  The physical atlas is an R32F image of physical_page_table_size^2 texels, row-major; physical page p sits at page
+ * coordinates (p % n, p / n), n = physical_page_table_size / page_size.
+ * Where the reference's outcome depends on the atomics order of the marking or the wave order of the allocation, the library
+ * commits to one admissible outcome (specification: oracle/oxc_oracle_vsm.c orc_vsm_*):
+ *   - free list: physical pages with occupancy 0 in ascending order
+ *   - allocation: the first min(active_request_count, request_capacity) requests are read; one naming an entry outside the table
+ *     is skipped (the reference would store out of bounds).  Requests are ranked by the linear address (layer * size + y) * size + x
+ *     of their entry; d requests for one entry take d consecutive free-list slots and the entry gets the highest of them below
+ *     free_page_count.  An entry whose first slot is past the free count is left unchanged: the reference sets AllocationFailed
+ *     on a local copy and returns without storing it.  alloc_cursor = slots handed out
+ *   - dirty list: ascending page table address; clipmap_dirty_flags[l] is 0 or 1 for every l < clipmap_count
+ *   - invalidation, deviation: every page a box covers is invalidated.  The reference visits the pages of 8 x 8 page sections
+ *     with section index < DIRECTIONAL_PAGE_TABLE_SIZE (64 per clipmap): the whole table at its size 64, but for other sizes it
+ *     misses the pages beyond 8 * floor(size / 8) and every section past the 64th
+ *   - arithmetic as everywhere: IEEE binary32, no contraction, project_aabb of cull.slang:12-47.
+ * Every entry point returns OXC_E_INVALID for a null pointer, clipmap_count outside 1..10, page_table_size < 1, a page_size that
+ * does not divide physical_page_table_size, more than 65536 physical pages (the 16-bit address) or a physical_page_count other
+ * than (physical_page_table_size / page_size)^2. */
+typedef struct OxcVsmAllocator { /* rmvsm.slang:228-236 VSMPageAllocator, scalar layout, 40 B (device memory) */
+  uint32_t active_request_count;          /* written by oxc_mark_visible_pages, zeroed by oxc_vsm_begin_frame */
+  uint32_t dirty_physical_page_count;     /* entries of dirty_physical_page_coords (the clear dispatch's z) */
+  uint32_t free_page_count;
+  uint32_t alloc_cursor;
+  int32_t* requests;                      /* int3 {x, y, layer} per request */
+  uint32_t* dirty_physical_page_coords;   /* u32x2 per dirty physical page */
+  uint32_t* free_page_list;
+} OxcVsmAllocator;
+OXC_STATIC_ASSERT(sizeof(OxcVsmAllocator) == 40, "VSMPageAllocator");
+/* page_tables_dev[clipmap][size][size]: cleared when sun_moved, else Visible, Dirty and Invalidated cleared (Backed,
+ * AllocationFailed, the address and the other bits stay); occupancy_dev[0, physical_page_count) = 0; *request_count_dev = 0. */
+int oxc_vsm_begin_frame(OxcContext* ctx, const OxcVsmContext* vsm, int sun_moved, uint32_t* page_tables_dev, uint32_t* occupancy_dev,
+                        uint32_t physical_page_count, uint32_t* request_count_dev, void* stream);
+/* rmvsm_invalidate_pages.slang:19-111: for every dirty mesh instance (indices into the scene's mesh instances, device) and
+ * clipmap, the mesh's bounds (OxcMesh::bounds) under the previous (previous_transforms_dev[transform_index], device) and the
+ * current world matrix: project_aabb(clipmap.projection_view_mat * world, z_near), a failed projection invalidates nothing;
+ * the clamped uv box covers pages floor(uv_min * size) .. ceil(uv_max * size) - 1, wrapped by the clipmap's page offset; every
+ * Backed entry there becomes exactly Invalidated (8).  A dirty index outside the mesh instance table is skipped.  Needs
+ * oxc_set_scene; invalidates whenever it is called (the frame sequence skips it on sun_moved). */
+int oxc_vsm_invalidate_pages(OxcContext* ctx, const OxcVsmContext* vsm, const OxcVirtualClipmap* clipmaps /* host */,
+                             const uint32_t* dirty_mesh_instances_dev, uint32_t dirty_count, const OxcTransformWorld* previous_transforms_dev,
+                             uint32_t* page_tables_dev, void* stream);
+/* Free invisible pages, free list, allocation and dirty list in one launch (one CTA: the tables are small and a single block
+ * makes every scan run in address order).  Writes the allocator's counters and its three pointers (requests_dev, dirty_coords_dev,
+ * free_list_dev).  free_list_dev holds physical_page_count entries; dirty_coords_dev holds clipmap_count * size^2 u32x2 entries
+ * (any entry may be dirty) and is the kernel's scratch for the per-entry request counts; clipmap_dirty_flags_dev holds
+ * clipmap_count u32. */
+int oxc_vsm_allocate_pages(OxcContext* ctx, const OxcVsmContext* vsm, uint32_t* page_tables_dev, const uint32_t* occupancy_dev,
+                           uint32_t physical_page_count, const int32_t* requests_dev, uint32_t request_capacity, OxcVsmAllocator* allocator_dev,
+                           uint32_t* free_list_dev, uint32_t* dirty_coords_dev, uint32_t* clipmap_dirty_flags_dev, void* stream);
+/* rmvsm_clear_dirty_pages.slang:12-25: every texel of each of the allocator's dirty pages = 1.0f (the count is read on the
+ * device).  A page whose coordinates lie outside the atlas is not written (the image store would be discarded). */
+int oxc_vsm_clear_dirty_pages(OxcContext* ctx, const OxcVsmContext* vsm, const OxcVsmAllocator* allocator_dev, const uint32_t* dirty_coords_dev,
+                              float* physical_atlas_dev, void* stream);
+/* oxc_cull_meshlets_hpb with the clipmap dirty flags read from DEVICE memory (clipmap_count u32, e.g. the flags
+ * oxc_vsm_allocate_pages wrote), as the reference binds them (CullGeometry.cpp:214-259): no read-back mid-frame. */
+int oxc_cull_meshlets_hpb_dirty_dev(OxcContext* ctx, const OxcCullCamera* camera, const OxcVirtualClipmap* clipmaps /* host */,
+                                    const uint32_t* clipmap_dirty_flags_dev, uint32_t clipmap_count, const uint8_t* hpb_dev,
+                                    uint32_t hpb_size, uint32_t hpb_levels, void* stream);
+
 int oxc_get_outputs(OxcContext* ctx, OxcOutputs* out);
 /* Instrumentation hook: 128 u64 counters that builds with -DOXC_RASTER_STATS fill (tools/raster_stats.py); zero otherwise. */
 void* oxc_debug_stats_ptr(OxcContext* ctx);
@@ -679,6 +751,36 @@ int oxr_render(OxrRenderer* r, const OxcCullCamera* camera, const float* occlude
 int oxr_submit(OxrRenderer* r, const OxcCullCamera* camera, uint32_t* vis32_host, float* depth_host,
                uint32_t* visible_indices_host, uint32_t visible_indices_capacity, int* ticket);
 int oxr_wait(OxrRenderer* r, int ticket, OxrFrameResult* result);
+
+/* RendererInstance::draw_virtual_shadowmap page loop (Shadowmaps.cpp:100-430, steps up to the shadow raster): the renderer owns the
+ * virtual page table, the HPB, occupancy, requests, the allocator and its lists, the clipmap dirty flags and the physical atlas
+ * (allocated by the first call, re-allocated when the shape changes: the table then starts cleared and the atlas zeroed), and runs
+ * the sequence of oxc_vsm_begin_frame on its stream from the depth of the frame oxr_render / oxr_wait completed last.  Previous
+ * transforms (invalidation) are the values each transform had before the oxr_update_transforms that last changed it.  Synchronous. */
+typedef struct OxrVsmPageContext {
+  OxcVsmContext vsm;                       /* page_size, page_table_size, physical_page_table_size, clipmap_count, ... */
+  OxcVirtualClipmap clipmaps[10];          /* clipmap_count used */
+  float inv_projection_view[16];           /* Camera::inv_projection_view of the frame */
+  float resolution[2];
+  uint32_t sun_moved;
+  uint32_t dirty_mesh_instance_count;
+  const uint32_t* dirty_mesh_instances;    /* host, dirty_mesh_instance_count indices (Scene.cpp dirty_mesh_instance_indices) */
+  uint32_t hpb_levels;                     /* 1..16 */
+} OxrVsmPageContext;
+typedef struct OxrVsmPages {               /* device pointers, valid until the next oxr_vsm_update_pages with another shape */
+  uint32_t* page_tables;                   /* [clipmap][size][size] */
+  uint8_t* hpb;                            /* oxc_build_hpb layout */
+  uint32_t* page_occupancy;
+  int32_t* requests;                       /* request_capacity int3 */
+  OxcVsmAllocator* allocator;
+  uint32_t* free_page_list;
+  uint32_t* dirty_physical_page_coords;
+  uint32_t* clipmap_dirty_flags;
+  float* physical_atlas;
+  uint32_t page_table_size, clipmap_count, physical_page_count, physical_atlas_size, hpb_levels, request_capacity;
+} OxrVsmPages;
+int oxr_vsm_update_pages(OxrRenderer* r, const OxrVsmPageContext* context);
+int oxr_vsm_pages(OxrRenderer* r, OxrVsmPages* out);
 
 /* ------------------------------------------------------------------------------------------------
  * oxb_* — mesh builder (SURVEY §8f.2): host-side producer of the blob layout above, mirroring build_gltf_mesh

@@ -171,6 +171,9 @@ class MaterialTable(C.Structure):
 VSM_PAGE_VISIBLE = 1
 VSM_PAGE_DIRTY = 2
 VSM_PAGE_BACKED = 4
+VSM_PAGE_INVALIDATED = 8
+VSM_PAGE_ALLOCATION_FAILED = 16
+VSM_MAX_CLIPMAPS = 10
 
 
 class SceneDesc(C.Structure):
@@ -235,6 +238,40 @@ VSM_CONTEXT_DT = np.dtype([("page_size", "<i4"), ("page_table_size", "<i4"), ("p
                            ("clipmap_selection_bias", "<f4"), ("virtual_extent", "<f4"), ("z_length", "<f4"),
                            ("directional_light_dir", "<f4", (3,))])
 assert VSM_CONTEXT_DT.itemsize == 56
+# rmvsm.slang:228-236 VSMPageAllocator (OxcVsmAllocator): counters, then device pointers of the three lists
+VSM_ALLOCATOR_DT = np.dtype([("active_request_count", "<u4"), ("dirty_physical_page_count", "<u4"), ("free_page_count", "<u4"),
+                             ("alloc_cursor", "<u4"), ("requests", "<u8"), ("dirty_physical_page_coords", "<u8"), ("free_page_list", "<u8")])
+assert VSM_ALLOCATOR_DT.itemsize == 40
+
+
+class VsmPageContext(C.Structure):
+    """OxrVsmPageContext (oxr_vsm_update_pages)"""
+
+    _fields_ = [
+        ("vsm", C.c_uint8 * VSM_CONTEXT_DT.itemsize),
+        ("clipmaps", C.c_uint8 * (CLIPMAP_DT.itemsize * VSM_MAX_CLIPMAPS)),
+        ("inv_projection_view", C.c_float * 16),
+        ("resolution", C.c_float * 2),
+        ("sun_moved", C.c_uint32),
+        ("dirty_mesh_instance_count", C.c_uint32),
+        ("dirty_mesh_instances", C.c_void_p),
+        ("hpb_levels", C.c_uint32),
+    ]
+
+
+class VsmPages(C.Structure):
+    """OxrVsmPages: device pointers of the renderer's virtual shadow map state"""
+
+    _fields_ = [
+        ("page_tables", C.c_void_p), ("hpb", C.c_void_p), ("page_occupancy", C.c_void_p), ("requests", C.c_void_p), ("allocator", C.c_void_p),
+        ("free_page_list", C.c_void_p), ("dirty_physical_page_coords", C.c_void_p), ("clipmap_dirty_flags", C.c_void_p),
+        ("physical_atlas", C.c_void_p),
+        ("page_table_size", C.c_uint32), ("clipmap_count", C.c_uint32), ("physical_page_count", C.c_uint32), ("physical_atlas_size", C.c_uint32),
+        ("hpb_levels", C.c_uint32), ("request_capacity", C.c_uint32),
+    ]
+
+
+assert C.sizeof(VsmPageContext) == 912 and C.sizeof(VsmPages) == 96
 
 
 class MgpuInfo(C.Structure):

@@ -20,11 +20,13 @@ SYMBOLS = [
     "oxc_cull_meshlets", "oxc_build_hiz", "oxc_build_hiz_packed", "oxc_build_hiz_mip0_packed", "oxc_build_hiz_from_mip0", "oxc_cull_triangles", "oxc_cull_triangles_small_primitive", "oxc_clear_visbuffer",
     "oxc_raster_visbuffer", "oxc_raster_visbuffer_clip_pass", "oxc_set_materials", "oxc_raster_overdraw", "oxc_clear_overdraw", "oxc_resolve_visbuffer", "oxc_merge_depth", "oxc_clear_visbuffer_with_depth", "oxc_cull_meshlets_multiview", "oxc_cull_meshlets_hpb", "oxc_cull_terrain",
     "oxc_decode_visbuffer", "oxc_build_hpb", "oxc_mark_visible_pages",
+    "oxc_vsm_begin_frame", "oxc_vsm_invalidate_pages", "oxc_vsm_allocate_pages", "oxc_vsm_clear_dirty_pages", "oxc_cull_meshlets_hpb_dirty_dev",
     "oxc_get_outputs", "oxc_check_status", "oxc_mark_hiz_dirty", "oxc_bind_camera_buffer", "oxc_load_camera", "oxc_debug_stats_ptr",
     "oxc_mgpu_get_unique_id", "oxc_mgpu_init", "oxc_mgpu_init_with_comm", "oxc_mgpu_shutdown", "oxc_mgpu_info", "oxc_mgpu_exchange_hiz",
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
     "oxb_last_error", "oxb_build_mesh", "oxb_mesh_blob_size", "oxb_mesh_lod0_meshlet_count", "oxb_mesh_emit", "oxb_mesh_free", "oxb_simplify",
     "oxr_create", "oxr_destroy", "oxr_context", "oxr_update", "oxr_update_transforms", "oxr_set_external_depth", "oxr_set_materials", "oxr_overdraw", "oxr_render", "oxr_submit", "oxr_wait",
+    "oxr_vsm_update_pages", "oxr_vsm_pages",
 ]
 
 
@@ -83,6 +85,11 @@ def load(build_if_missing=True):
     lib.oxc_decode_visbuffer.argtypes = [vp, vp, vp, vp, u32, u32, C.POINTER(abi.DecodeTargets), vp]
     lib.oxc_build_hpb.argtypes = [vp, vp, u32, u32, vp, u32, vp]
     lib.oxc_mark_visible_pages.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, u32, vp]
+    lib.oxc_vsm_begin_frame.argtypes = [vp, vp, i32, vp, vp, u32, vp, vp]
+    lib.oxc_vsm_invalidate_pages.argtypes = [vp, vp, vp, vp, u32, vp, vp, vp]
+    lib.oxc_vsm_allocate_pages.argtypes = [vp, vp, vp, vp, u32, vp, u32, vp, vp, vp, vp, vp]
+    lib.oxc_vsm_clear_dirty_pages.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.oxc_cull_meshlets_hpb_dirty_dev.argtypes = [vp, vp, vp, vp, u32, vp, u32, u32, vp]
     lib.oxc_get_outputs.argtypes = [vp, C.POINTER(abi.Outputs)]
     lib.oxc_check_status.argtypes = [vp, vp, C.POINTER(C.c_uint32)]
     lib.oxc_mark_hiz_dirty.argtypes = [vp]
@@ -127,6 +134,8 @@ def load(build_if_missing=True):
     lib.oxr_submit.argtypes = [vp, vp, vp, vp, vp, u32, C.POINTER(C.c_int)]
     lib.oxr_wait.argtypes = [vp, i32, C.POINTER(abi.FrameResult)]
     lib.oxr_render.argtypes = [vp, vp, vp, vp, vp, vp, u32, C.POINTER(abi.FrameResult)]
+    lib.oxr_vsm_update_pages.argtypes = [vp, C.POINTER(abi.VsmPageContext)]
+    lib.oxr_vsm_pages.argtypes = [vp, C.POINTER(abi.VsmPages)]
     _LIB = lib
     return lib
 
@@ -410,6 +419,34 @@ class Context:
                                                _ptr(occupancy_dev), _ptr(request_count_dev), _ptr(requests_dev), request_capacity, self.stream),
                "oxc_mark_visible_pages")
 
+    # ---- virtual shadow map page bookkeeping (oxc_vsm_*); `vsm` is an abi.VSM_CONTEXT_DT record, pointers are device pointers ----
+    def vsm_begin_frame(self, vsm, sun_moved, page_tables_dev, occupancy_dev, physical_page_count, request_count_dev):
+        vc = np.ascontiguousarray(vsm)
+        _check(self.lib.oxc_vsm_begin_frame(self.h, _ptr(vc), int(bool(sun_moved)), _ptr(page_tables_dev), _ptr(occupancy_dev), physical_page_count,
+                                            _ptr(request_count_dev), self.stream), "oxc_vsm_begin_frame")
+
+    def vsm_invalidate_pages(self, vsm, clipmaps, dirty_dev, dirty_count, previous_transforms_dev, page_tables_dev):
+        vc, cm = np.ascontiguousarray(vsm), np.ascontiguousarray(clipmaps)
+        _check(self.lib.oxc_vsm_invalidate_pages(self.h, _ptr(vc), _ptr(cm), _ptr(dirty_dev), dirty_count, _ptr(previous_transforms_dev),
+                                                 _ptr(page_tables_dev), self.stream), "oxc_vsm_invalidate_pages")
+
+    def vsm_allocate_pages(self, vsm, page_tables_dev, occupancy_dev, physical_page_count, requests_dev, request_capacity, allocator_dev,
+                           free_list_dev, dirty_coords_dev, dirty_flags_dev):
+        vc = np.ascontiguousarray(vsm)
+        _check(self.lib.oxc_vsm_allocate_pages(self.h, _ptr(vc), _ptr(page_tables_dev), _ptr(occupancy_dev), physical_page_count, _ptr(requests_dev),
+                                               request_capacity, _ptr(allocator_dev), _ptr(free_list_dev), _ptr(dirty_coords_dev),
+                                               _ptr(dirty_flags_dev), self.stream), "oxc_vsm_allocate_pages")
+
+    def vsm_clear_dirty_pages(self, vsm, allocator_dev, dirty_coords_dev, atlas_dev):
+        vc = np.ascontiguousarray(vsm)
+        _check(self.lib.oxc_vsm_clear_dirty_pages(self.h, _ptr(vc), _ptr(allocator_dev), _ptr(dirty_coords_dev), _ptr(atlas_dev), self.stream),
+               "oxc_vsm_clear_dirty_pages")
+
+    def cull_meshlets_hpb_dirty_dev(self, cam, clipmaps, dirty_flags_dev, hpb_dev, hpb_size, hpb_levels):
+        cm = np.ascontiguousarray(clipmaps)
+        _check(self.lib.oxc_cull_meshlets_hpb_dirty_dev(self.h, _ptr(cam), _ptr(cm), _ptr(dirty_flags_dev), len(cm), _ptr(hpb_dev), hpb_size,
+                                                        hpb_levels, self.stream), "oxc_cull_meshlets_hpb_dirty_dev")
+
     def build_hpb(self, page_table_dev, size, layers, hpb_dev, levels):
         _check(self.lib.oxc_build_hpb(self.h, _ptr(page_table_dev), size, layers, _ptr(hpb_dev), levels, self.stream), "oxc_build_hpb")
 
@@ -617,6 +654,29 @@ class Renderer:
         _check(self.lib.oxr_wait(self.h, ticket, C.byref(res)), "oxr_wait")
         return dict(total=res.total, early=res.early, late=res.late, raster_triangles=res.raster_triangles,
                     draw_index_count_early=res.draw_index_count_early, draw_index_count_late=res.draw_index_count_late)
+
+    def vsm_update_pages(self, vsm, clipmaps, inv_projection_view, resolution, sun_moved=False, dirty_mesh_instances=(), hpb_levels=7):
+        """oxr_vsm_update_pages: one VSM frame from the depth of the last rendered frame; returns vsm_pages()"""
+        c = abi.VsmPageContext()
+        vc = np.ascontiguousarray(vsm, dtype=abi.VSM_CONTEXT_DT)
+        cm = np.zeros(abi.VSM_MAX_CLIPMAPS, dtype=abi.CLIPMAP_DT)
+        cm[: len(clipmaps)] = clipmaps
+        C.memmove(c.vsm, vc.ctypes.data, vc.nbytes)
+        C.memmove(c.clipmaps, cm.ctypes.data, cm.nbytes)
+        c.inv_projection_view[:] = [float(x) for x in np.asarray(inv_projection_view, dtype=np.float32).reshape(16)]
+        c.resolution[:] = [float(x) for x in np.asarray(resolution, dtype=np.float32).reshape(2)]
+        dirty = np.ascontiguousarray(dirty_mesh_instances, dtype=np.uint32)
+        c.sun_moved, c.dirty_mesh_instance_count = int(bool(sun_moved)), len(dirty)
+        c.dirty_mesh_instances = dirty.ctypes.data if len(dirty) else None
+        c.hpb_levels = hpb_levels
+        _check(self.lib.oxr_vsm_update_pages(self.h, C.byref(c)), "oxr_vsm_update_pages")
+        return self.vsm_pages()
+
+    def vsm_pages(self):
+        """oxr_vsm_pages: abi.VsmPages of device pointers and sizes"""
+        out = abi.VsmPages()
+        _check(self.lib.oxr_vsm_pages(self.h, C.byref(out)), "oxr_vsm_pages")
+        return out
 
     def close(self):
         if getattr(self, "h", None):

@@ -105,6 +105,8 @@ RendererInstance::~RendererInstance() {
     if (sl.ev_copy) cudaEventDestroy(static_cast<cudaEvent_t>(sl.ev_copy));
   }
   drop_graphs();
+  vsm_release();
+  cudaFree(d_transforms_previous_);
   for (int k = 0; k < 2; k++) { cudaFree(d_cam_[k]); if (h_cam_[k]) cudaFreeHost(h_cam_[k]); }
   if (ev_window_) cudaEventDestroy(static_cast<cudaEvent_t>(ev_window_));
   if (copy_stream_) cudaStreamDestroy(static_cast<cudaStream_t>(copy_stream_));
@@ -118,12 +120,142 @@ auto RendererInstance::update(const RendererInstanceUpdateInfo& info) -> int {
   error_.clear();
   drop_graphs(); // the scene tables may be reallocated: captured launches would keep the old addresses
   oxc_bind_camera_buffer(ctx_, nullptr);
-  return fail(oxc_set_scene(ctx_, &info.scene, stream_));
+  int rc = oxc_set_scene(ctx_, &info.scene, stream_);
+  if (rc != OXC_OK) return fail(rc);
+  // a new scene has no motion yet: previous transforms = current
+  const uint32_t n = info.scene.transform_count;
+  transforms_.assign(info.scene.transforms, info.scene.transforms + n);
+  if (n > transforms_previous_capacity_) {
+    cudaFree(d_transforms_previous_);
+    d_transforms_previous_ = nullptr;
+    transforms_previous_capacity_ = 0;
+    if (cudaMalloc(reinterpret_cast<void**>(&d_transforms_previous_), (size_t)n * sizeof(OxcTransformWorld)) != cudaSuccess) return fail(OXC_E_CUDA);
+    transforms_previous_capacity_ = n;
+  }
+  if (n && cudaMemcpyAsync(d_transforms_previous_, transforms_.data(), (size_t)n * sizeof(OxcTransformWorld), cudaMemcpyHostToDevice,
+                           static_cast<cudaStream_t>(stream_)) != cudaSuccess)
+    return fail(OXC_E_CUDA);
+  return OXC_OK;
 }
 
 auto RendererInstance::update_transforms(const OxcTransformWorld* transforms, uint32_t first, uint32_t count) -> int {
   if (!ctx_) return OXC_E_STATE;
-  return fail(oxc_update_transforms(ctx_, transforms, first, count, stream_));
+  int rc = oxc_update_transforms(ctx_, transforms, first, count, stream_);
+  if (rc != OXC_OK) return fail(rc);
+  // the replaced values become the previous transforms (pageable source: the copy has left transforms_ when the call returns)
+  if (count && cudaMemcpyAsync(d_transforms_previous_ + first, transforms_.data() + first, (size_t)count * sizeof(OxcTransformWorld),
+                               cudaMemcpyHostToDevice, static_cast<cudaStream_t>(stream_)) != cudaSuccess)
+    return fail(OXC_E_CUDA);
+  std::memcpy(transforms_.data() + first, transforms, (size_t)count * sizeof(OxcTransformWorld));
+  return OXC_OK;
+}
+
+void RendererInstance::vsm_release() {
+  OxrVsmPages& v = vsm_.pages;
+  cudaFree(v.page_tables); cudaFree(v.hpb); cudaFree(v.page_occupancy); cudaFree(v.requests); cudaFree(v.allocator);
+  cudaFree(v.free_page_list); cudaFree(v.dirty_physical_page_coords); cudaFree(v.clipmap_dirty_flags); cudaFree(v.physical_atlas);
+  cudaFree(vsm_.d_dirty_instances);
+  vsm_ = Vsm();
+}
+
+// RendererInstance's vsm_* attachments (created with the renderer in the reference) and the transient buffers of
+// Shadowmaps.cpp:100-128, sized from the VSM context; a new shape starts from a cleared table and a zeroed atlas
+int RendererInstance::vsm_allocate(const OxcVsmContext& vsm, uint32_t hpb_levels) {
+  const uint32_t size = (uint32_t)vsm.page_table_size, layers = (uint32_t)vsm.clipmap_count;
+  const uint32_t per_row = (uint32_t)(vsm.physical_page_table_size / vsm.page_size), atlas = (uint32_t)vsm.physical_page_table_size;
+  OxrVsmPages& v = vsm_.pages;
+  if (v.page_tables && v.page_table_size == size && v.clipmap_count == layers && v.physical_atlas_size == atlas &&
+      v.physical_page_count == per_row * per_row && v.hpb_levels == hpb_levels && vsm_.shape.page_size == vsm.page_size)
+    return OXC_OK;
+  vsm_release();
+  const size_t entries = (size_t)layers * size * size, pages = (size_t)per_row * per_row;
+  size_t hpb_bytes = 0;
+  for (uint32_t l = 0; l < hpb_levels; l++) { const size_t sl = (size >> l) ? (size >> l) : 1u; hpb_bytes += layers * sl * sl; }
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  bool ok = cudaMalloc(reinterpret_cast<void**>(&v.page_tables), entries * 4) == cudaSuccess &&
+            cudaMalloc(reinterpret_cast<void**>(&v.hpb), hpb_bytes) == cudaSuccess &&
+            cudaMalloc(reinterpret_cast<void**>(&v.page_occupancy), pages * 4) == cudaSuccess &&
+            cudaMalloc(reinterpret_cast<void**>(&v.requests), entries * 12) == cudaSuccess &&
+            cudaMalloc(reinterpret_cast<void**>(&v.allocator), sizeof(OxcVsmAllocator)) == cudaSuccess &&
+            cudaMalloc(reinterpret_cast<void**>(&v.free_page_list), pages * 4) == cudaSuccess &&
+            cudaMalloc(reinterpret_cast<void**>(&v.dirty_physical_page_coords), entries * 8) == cudaSuccess &&
+            cudaMalloc(reinterpret_cast<void**>(&v.clipmap_dirty_flags), layers * 4) == cudaSuccess &&
+            cudaMalloc(reinterpret_cast<void**>(&v.physical_atlas), (size_t)atlas * atlas * 4) == cudaSuccess;
+  ok = ok && cudaMemsetAsync(v.page_tables, 0, entries * 4, s) == cudaSuccess && cudaMemsetAsync(v.hpb, 0, hpb_bytes, s) == cudaSuccess &&
+       cudaMemsetAsync(v.allocator, 0, sizeof(OxcVsmAllocator), s) == cudaSuccess &&
+       cudaMemsetAsync(v.clipmap_dirty_flags, 0, layers * 4, s) == cudaSuccess &&
+       cudaMemsetAsync(v.physical_atlas, 0, (size_t)atlas * atlas * 4, s) == cudaSuccess;
+  if (!ok) {
+    vsm_release();
+    error_ = std::string("virtual shadow map allocation failed: ") + cudaGetErrorString(cudaGetLastError());
+    return OXC_E_CUDA;
+  }
+  v.page_table_size = size; v.clipmap_count = layers; v.physical_page_count = (uint32_t)pages; v.physical_atlas_size = atlas;
+  v.hpb_levels = hpb_levels; v.request_capacity = (uint32_t)entries; // every entry is requested at most once per frame
+  vsm_.shape = vsm;
+  return OXC_OK;
+}
+
+// Shadowmaps.cpp:100-430 up to the shadow raster, on stream_, from the depth of the last frame.  The vuk passes become the
+// oxc_vsm_* calls; step numbers as in include/oxcull.h.
+auto RendererInstance::update_virtual_shadow_pages(VsmPageContext& context) -> int {
+  if (!ctx_ || !error_.empty()) return OXC_E_STATE;
+  const OxcVsmContext& vsm = context.vsm;
+  if (context.hpb_levels < 1 || context.hpb_levels > 16) return OXC_E_INVALID;
+  if (context.dirty_mesh_instance_count && !context.dirty_mesh_instances) return OXC_E_INVALID;
+  if (vsm.clipmap_count < 1 || vsm.clipmap_count > 10 || vsm.page_table_size < 1 || vsm.page_size < 1 ||
+      vsm.physical_page_table_size % vsm.page_size != 0)
+    return OXC_E_INVALID;
+  if (vsm.depth_extent[0] != (int32_t)width_ || vsm.depth_extent[1] != (int32_t)height_) return OXC_E_INVALID;
+  int rc = vsm_allocate(vsm, context.hpb_levels);
+  if (rc != OXC_OK) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  OxrVsmPages& v = vsm_.pages;
+  if (context.dirty_mesh_instance_count > vsm_.dirty_capacity) {
+    cudaFree(vsm_.d_dirty_instances);
+    vsm_.d_dirty_instances = nullptr;
+    vsm_.dirty_capacity = 0;
+    if (cudaMalloc(reinterpret_cast<void**>(&vsm_.d_dirty_instances), (size_t)context.dirty_mesh_instance_count * 4) != cudaSuccess)
+      return fail(OXC_E_CUDA);
+    vsm_.dirty_capacity = context.dirty_mesh_instance_count;
+  }
+  const bool invalidate = !context.sun_moved && context.dirty_mesh_instance_count > 0; // :203
+  if (invalidate && cudaMemcpyAsync(vsm_.d_dirty_instances, context.dirty_mesh_instances, (size_t)context.dirty_mesh_instance_count * 4,
+                                    cudaMemcpyHostToDevice, s) != cudaSuccess)
+    return fail(OXC_E_CUDA);
+  // the frame's depth attachment: the depth half of the packed vis buffer
+  if ((rc = oxc_resolve_visbuffer(ctx_, d_vis64_, width_, height_, nullptr, d_depth_, stream_)) != OXC_OK) return fail(rc);
+  // steps 0, 1, 3
+  if ((rc = oxc_vsm_begin_frame(ctx_, &vsm, (int)context.sun_moved, v.page_tables, v.page_occupancy, v.physical_page_count,
+                                &v.allocator->active_request_count, stream_)) != OXC_OK) return fail(rc);
+  // step 2
+  if (invalidate && (rc = oxc_vsm_invalidate_pages(ctx_, &vsm, context.clipmaps, vsm_.d_dirty_instances, context.dirty_mesh_instance_count,
+                                                   d_transforms_previous_, v.page_tables, stream_)) != OXC_OK) return fail(rc);
+  // step 4
+  if ((rc = oxc_mark_visible_pages(ctx_, context.inv_projection_view, context.resolution, context.clipmaps, &vsm, d_depth_, v.page_tables,
+                                   v.page_occupancy, &v.allocator->active_request_count, v.requests, v.request_capacity, stream_)) != OXC_OK)
+    return fail(rc);
+  // steps 5, 6, 7, 9
+  if ((rc = oxc_vsm_allocate_pages(ctx_, &vsm, v.page_tables, v.page_occupancy, v.physical_page_count, v.requests, v.request_capacity,
+                                   v.allocator, v.free_page_list, v.dirty_physical_page_coords, v.clipmap_dirty_flags, stream_)) != OXC_OK)
+    return fail(rc);
+  // step 8
+  if ((rc = oxc_build_hpb(ctx_, v.page_tables, v.page_table_size, v.clipmap_count, v.hpb, v.hpb_levels, stream_)) != OXC_OK) return fail(rc);
+  // step 10
+  if ((rc = oxc_vsm_clear_dirty_pages(ctx_, &vsm, v.allocator, v.dirty_physical_page_coords, v.physical_atlas, stream_)) != OXC_OK)
+    return fail(rc);
+  if (cudaStreamSynchronize(s) != cudaSuccess) {
+    error_ = cudaGetErrorString(cudaGetLastError());
+    return OXC_E_CUDA;
+  }
+  return OXC_OK;
+}
+
+auto RendererInstance::virtual_shadow_pages(OxrVsmPages* out) const -> int {
+  if (!out) return OXC_E_INVALID;
+  if (!vsm_.pages.page_tables) return OXC_E_STATE;
+  *out = vsm_.pages;
+  return OXC_OK;
 }
 
 // MainGeometryContext::draw_overdraw (RendererInstance.cpp:771-776; debug view "Overdraw"): the encode pass's fragment counter for
@@ -571,6 +703,17 @@ int oxr_submit(OxrRenderer* r, const OxcCullCamera* camera, uint32_t* vis32_host
 int oxr_wait(OxrRenderer* r, int ticket, OxrFrameResult* result) {
   if (!r) return OXC_E_INVALID;
   return r->impl.wait(ticket, result);
+}
+
+int oxr_vsm_update_pages(OxrRenderer* r, const OxrVsmPageContext* context) {
+  if (!r || !context) return OXC_E_INVALID;
+  ox::VsmPageContext c = *context;
+  return r->impl.update_virtual_shadow_pages(c);
+}
+
+int oxr_vsm_pages(OxrRenderer* r, OxrVsmPages* out) {
+  if (!r) return OXC_E_INVALID;
+  return r->impl.virtual_shadow_pages(out);
 }
 
 int oxr_render(OxrRenderer* r, const OxcCullCamera* camera, const float* occluder_depth_host, uint32_t* vis32_host,

@@ -35,6 +35,10 @@ struct MainGeometryContext {
   uint32_t width = 0, height = 0;
 };
 
+// RMVSMContext's per-frame inputs (RendererInstance.hpp:259-280 with the clipmaps calculate_virtual_shadow_matrices produced,
+// Shadowmaps.cpp:9-63, and the frame's dirty mesh instances, RendererInstance.cpp:1704-1716)
+using VsmPageContext = OxrVsmPageContext;
+
 // Scene.cpp:1280-1290 RendererInstanceUpdateInfo (the fields this path consumes)
 struct RendererInstanceUpdateInfo {
   uint32_t mesh_instance_count = 0;
@@ -64,6 +68,9 @@ public:
   auto cull_geometry(CullGeometryContext& context) -> int;
   auto generate_hiz(MainGeometryContext& context) -> int;
   auto draw_for_visbuffer(MainGeometryContext& context) -> int;
+  // draw_virtual_shadowmap's page loop (Shadowmaps.cpp:100-430) up to the shadow raster, from the depth of the last frame
+  auto update_virtual_shadow_pages(VsmPageContext& context) -> int;
+  auto virtual_shadow_pages(OxrVsmPages* out) const -> int;
 
   // RendererInstance::render geometry section: run_geometry_pass(false) -> generate_hiz -> run_geometry_pass(true)
   auto render(const OxcCullCamera& camera, const float* occluder_depth_host, uint32_t* vis32_host, float* depth_host,
@@ -131,6 +138,20 @@ private:
   float* d_occluder_ = nullptr;
   uint32_t* d_overdraw_ = nullptr; // allocated by the first overdraw()
   bool has_external_depth_ = false;
+  // transforms as the host last uploaded them, and on the device the values before the upload that last changed each of them
+  // (TransformPrevious::previous_world, RendererInstance.cpp:1600-1609)
+  std::vector<OxcTransformWorld> transforms_;
+  OxcTransformWorld* d_transforms_previous_ = nullptr;
+  uint32_t transforms_previous_capacity_ = 0;
+  // virtual shadow map state (RendererInstance.hpp:259-280 vsm_* attachments, Shadowmaps.cpp:100-128 transient buffers)
+  struct Vsm {
+    OxrVsmPages pages{};
+    OxcVsmContext shape{};
+    uint32_t* d_dirty_instances = nullptr;
+    uint32_t dirty_capacity = 0;
+  } vsm_;
+  int vsm_allocate(const OxcVsmContext& vsm, uint32_t hpb_levels);
+  void vsm_release();
   void* h_pinned_ = nullptr; // staging for small readbacks
   std::string error_;
 };

@@ -820,6 +820,7 @@ struct HpbParams {
   const uint8_t* hpb;
   uint32_t hpb_size, hpb_levels, clipmap_count, inst_stride;
   uint32_t dirty_mask;           // bit c: clipmap_dirty_flags[c] != 0
+  const uint32_t* dirty_dev;     // k_cull_meshlets_hpb<true>: the flags in device memory instead (CullGeometry.cpp:214-259)
   float view_dir[3];             // camera.position (= -light_dir)
   float z_near[OXC_MAX_VIEWS];
   int page_offset[OXC_MAX_VIEWS][2];
@@ -860,9 +861,15 @@ OXC_DI bool test_vsm_page(const HpbParams& p, const ScreenAabb& a, uint32_t laye
   return tl | tr | bl | br;
 }
 
+template <bool DEV_FLAGS>
 __global__ void __launch_bounds__(CULL_THREADS) k_cull_meshlets_hpb(const __grid_constant__ HpbParams p) {
   __shared__ uint32_t warp_cnt[CULL_THREADS / 32];
   __shared__ uint32_t base_s;
+  uint32_t dirty_mask = p.dirty_mask;
+  if (DEV_FLAGS) {
+    dirty_mask = 0u;
+    for (uint32_t ci = 0; ci < p.clipmap_count; ci++) dirty_mask |= (__ldg(&p.dirty_dev[ci]) != 0u ? 1u : 0u) << ci;
+  }
   const uint32_t total = p.vis->total_visible_meshlet_instances;
   const uint32_t id_base = p.id_base ? __ldg(p.id_base) : 0u;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -888,7 +895,7 @@ __global__ void __launch_bounds__(CULL_THREADS) k_cull_meshlets_hpb(const __grid
       }
       if (cone_vis && test_frustum_planes(ic->plane, cx, cy, cz, ex, ey, ez)) { // :56
         for (uint32_t ci = 0; ci < p.clipmap_count; ci++) { // :59-79
-          if (!((p.dirty_mask >> ci) & 1u)) continue;
+          if (!((dirty_mask >> ci) & 1u)) continue;
           const InstView* v = p.views + (size_t)ci * p.inst_stride + mi.x;
           if (!test_frustum_planes(v->plane, cx, cy, cz, ex, ey, ez)) continue;
           ScreenAabb sa;

@@ -21,6 +21,7 @@
 #include "kernels_mgpu.cuh"
 #include "kernels_tri.cuh"
 #include "kernels_alpha.cuh"
+#include "kernels_vsm.cuh"
 
 using namespace oxc;
 
@@ -1049,9 +1050,13 @@ int oxc_device_free(OxcContext* c, void* p) {
   return OXC_OK;
 }
 
-int oxc_cull_meshlets_hpb(OxcContext* c, const OxcCullCamera* cam, const OxcVirtualClipmap* clipmaps, const uint32_t* dirty,
-                          uint32_t n, const uint8_t* hpb_dev, uint32_t hpb_size, uint32_t hpb_levels, void* stream) {
-  if (!c || !cam || !clipmaps || !dirty || !hpb_dev || n == 0 || hpb_size == 0 || hpb_levels == 0) return fail(OXC_E_INVALID, "bad argument");
+} // extern "C"
+
+namespace {
+// oxc_cull_meshlets_hpb (dirty flags on the host) and oxc_cull_meshlets_hpb_dirty_dev (on the device): exactly one is non-null
+int cull_meshlets_hpb(OxcContext* c, const OxcCullCamera* cam, const OxcVirtualClipmap* clipmaps, const uint32_t* dirty,
+                      const uint32_t* dirty_dev, uint32_t n, const uint8_t* hpb_dev, uint32_t hpb_size, uint32_t hpb_levels, void* stream) {
+  if (!c || !cam || !clipmaps || !(dirty || dirty_dev) || !hpb_dev || n == 0 || hpb_size == 0 || hpb_levels == 0) return fail(OXC_E_INVALID, "bad argument");
   if (n > c->info.max_views || !c->d_inst_views) return fail(OXC_E_CAPACITY, "clipmap_count %u > max_views %u", n, c->info.max_views);
   if (!c->scene_set) return fail(OXC_E_STATE, "oxc_set_scene first");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1064,7 +1069,7 @@ int oxc_cull_meshlets_hpb(OxcContext* c, const OxcCullCamera* cam, const OxcVirt
     memcpy(vm.m[v], clipmaps[v].projection_view_mat, sizeof vm.m[v]);
     p.z_near[v] = clipmaps[v].z_near;
     p.page_offset[v][0] = clipmaps[v].page_offset[0]; p.page_offset[v][1] = clipmaps[v].page_offset[1];
-    if (dirty[v]) p.dirty_mask |= 1u << v;
+    if (dirty && dirty[v]) p.dirty_mask |= 1u << v;
   }
   uint32_t first, count;
   shard_range(c, c->cached_cam.mesh_instance_count, &first, &count);
@@ -1083,9 +1088,26 @@ int oxc_cull_meshlets_hpb(OxcContext* c, const OxcCullCamera* cam, const OxcVirt
   uint32_t grid = (uint32_t)c->sm_count * 4u;
   if (grid > blocks) grid = blocks;
   if (grid == 0) grid = 1;
-  k_cull_meshlets_hpb<<<grid, CULL_THREADS, 0, s>>>(p);
+  p.dirty_dev = dirty_dev;
+  if (dirty_dev) k_cull_meshlets_hpb<true><<<grid, CULL_THREADS, 0, s>>>(p);
+  else k_cull_meshlets_hpb<false><<<grid, CULL_THREADS, 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
+}
+} // namespace
+
+extern "C" {
+
+int oxc_cull_meshlets_hpb(OxcContext* c, const OxcCullCamera* cam, const OxcVirtualClipmap* clipmaps, const uint32_t* dirty,
+                          uint32_t n, const uint8_t* hpb_dev, uint32_t hpb_size, uint32_t hpb_levels, void* stream) {
+  if (!dirty) return fail(OXC_E_INVALID, "bad argument");
+  return cull_meshlets_hpb(c, cam, clipmaps, dirty, nullptr, n, hpb_dev, hpb_size, hpb_levels, stream);
+}
+
+int oxc_cull_meshlets_hpb_dirty_dev(OxcContext* c, const OxcCullCamera* cam, const OxcVirtualClipmap* clipmaps, const uint32_t* dirty_dev,
+                                    uint32_t n, const uint8_t* hpb_dev, uint32_t hpb_size, uint32_t hpb_levels, void* stream) {
+  if (!dirty_dev) return fail(OXC_E_INVALID, "null clipmap_dirty_flags_dev");
+  return cull_meshlets_hpb(c, cam, clipmaps, nullptr, dirty_dev, n, hpb_dev, hpb_size, hpb_levels, stream);
 }
 
 int oxc_cull_terrain(OxcContext* c, const OxcTerrainData* terrain, const float* patch_minmax_dev, const OxcCullCamera* cam,
@@ -1192,6 +1214,114 @@ int oxc_build_hpb(OxcContext* c, const uint32_t* page_table_dev, uint32_t size, 
     src_off = dst_off;
     dst_off += n;
   }
+  return OXC_OK;
+}
+
+} // extern "C"
+
+namespace {
+// the OxcVsmContext checks every VSM entry point shares (include/oxcull.h); physical_page_count == UINT32_MAX: not an argument
+int check_vsm(const OxcVsmContext* vsm, uint32_t physical_page_count) {
+  if (vsm->clipmap_count < 1 || vsm->clipmap_count > VSM_MAX_CLIPMAPS)
+    return fail(OXC_E_INVALID, "clipmap_count %d outside 1..%d (shared_clipmaps[10], rmvsm_mark_visible_pages.slang:17)", vsm->clipmap_count, VSM_MAX_CLIPMAPS);
+  if (vsm->page_table_size < 1) return fail(OXC_E_INVALID, "page_table_size %d < 1", vsm->page_table_size);
+  if (vsm->page_size < 1 || vsm->physical_page_table_size < 1 || vsm->physical_page_table_size % vsm->page_size != 0)
+    return fail(OXC_E_INVALID, "page_size %d does not divide physical_page_table_size %d", vsm->page_size, vsm->physical_page_table_size);
+  const uint64_t per_row = (uint64_t)(vsm->physical_page_table_size / vsm->page_size);
+  if (per_row * per_row > 65536u)
+    return fail(OXC_E_INVALID, "%llu physical pages: more than the 16-bit physical address holds (65536, rmvsm.slang:33-34)",
+                (unsigned long long)(per_row * per_row));
+  if ((uint64_t)vsm->clipmap_count * vsm->page_table_size * vsm->page_table_size > (1ull << 30))
+    return fail(OXC_E_INVALID, "page table of %d x %d x %d entries is too large", vsm->clipmap_count, vsm->page_table_size, vsm->page_table_size);
+  if (physical_page_count != 0xFFFFFFFFu && physical_page_count != per_row * per_row)
+    return fail(OXC_E_INVALID, "physical_page_count %u != (physical_page_table_size / page_size)^2 = %llu", physical_page_count,
+                (unsigned long long)(per_row * per_row));
+  return OXC_OK;
+}
+
+uint32_t vsm_entries(const OxcVsmContext* vsm) { return (uint32_t)vsm->clipmap_count * vsm->page_table_size * vsm->page_table_size; }
+} // namespace
+
+extern "C" {
+
+int oxc_vsm_begin_frame(OxcContext* c, const OxcVsmContext* vsm, int sun_moved, uint32_t* page_tables_dev, uint32_t* occupancy_dev,
+                        uint32_t physical_page_count, uint32_t* request_count_dev, void* stream) {
+  if (!c || !vsm || !page_tables_dev || !occupancy_dev || !request_count_dev) return fail(OXC_E_INVALID, "null argument");
+  int rc = check_vsm(vsm, physical_page_count);
+  if (rc != OXC_OK) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  const uint32_t n = std::max(vsm_entries(vsm), physical_page_count);
+  k_vsm_begin_frame<<<(n + 255) / 256, 256, 0, s>>>(page_tables_dev, vsm_entries(vsm), occupancy_dev, physical_page_count, request_count_dev,
+                                                    sun_moved ? 1 : 0);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_vsm_invalidate_pages(OxcContext* c, const OxcVsmContext* vsm, const OxcVirtualClipmap* clipmaps, const uint32_t* dirty_mesh_instances_dev,
+                             uint32_t dirty_count, const OxcTransformWorld* previous_transforms_dev, uint32_t* page_tables_dev, void* stream) {
+  if (!c || !vsm || !clipmaps || !dirty_mesh_instances_dev || !previous_transforms_dev || !page_tables_dev) return fail(OXC_E_INVALID, "null argument");
+  int rc = check_vsm(vsm, 0xFFFFFFFFu);
+  if (rc != OXC_OK) return rc;
+  if (!c->scene_set) return fail(OXC_E_STATE, "oxc_set_scene first");
+  if (dirty_count == 0) return OXC_OK;
+  if ((uint64_t)dirty_count * vsm->clipmap_count * 2u * 32u > 0xFFFFFFFFull) return fail(OXC_E_INVALID, "dirty_count %u too large", dirty_count);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  VsmInvalidateParams p{};
+  for (int k = 0; k < vsm->clipmap_count; k++) {
+    memcpy(p.clip_pv[k], clipmaps[k].projection_view_mat, sizeof p.clip_pv[k]);
+    p.z_near[k] = clipmaps[k].z_near;
+    p.page_offset[k][0] = clipmaps[k].page_offset[0]; p.page_offset[k][1] = clipmaps[k].page_offset[1];
+  }
+  p.mesh_instances = c->d_mesh_instances; p.meshes = c->d_meshes; p.transforms = c->d_transforms; p.previous_transforms = previous_transforms_dev;
+  p.dirty = dirty_mesh_instances_dev; p.dirty_count = dirty_count;
+  p.mesh_instance_count = c->mesh_instance_count; p.mesh_count = c->mesh_count; p.transform_count = c->transform_count;
+  p.page_tables = page_tables_dev; p.size = vsm->page_table_size; p.clipmap_count = vsm->clipmap_count;
+  const uint64_t threads = (uint64_t)dirty_count * vsm->clipmap_count * 2u * 32u;
+  k_vsm_invalidate_pages<<<(uint32_t)((threads + 255) / 256), 256, 0, s>>>(p);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_vsm_allocate_pages(OxcContext* c, const OxcVsmContext* vsm, uint32_t* page_tables_dev, const uint32_t* occupancy_dev,
+                           uint32_t physical_page_count, const int32_t* requests_dev, uint32_t request_capacity, OxcVsmAllocator* allocator_dev,
+                           uint32_t* free_list_dev, uint32_t* dirty_coords_dev, uint32_t* clipmap_dirty_flags_dev, void* stream) {
+  if (!c || !vsm || !page_tables_dev || !occupancy_dev || !requests_dev || !allocator_dev || !free_list_dev || !dirty_coords_dev ||
+      !clipmap_dirty_flags_dev)
+    return fail(OXC_E_INVALID, "null argument");
+  int rc = check_vsm(vsm, physical_page_count);
+  if (rc != OXC_OK) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  VsmAllocParams p{};
+  p.page_tables = page_tables_dev; p.occupancy = occupancy_dev; p.requests = requests_dev; p.allocator = allocator_dev;
+  p.free_list = free_list_dev; p.dirty_coords = dirty_coords_dev; p.dirty_flags = clipmap_dirty_flags_dev;
+  p.entries = vsm_entries(vsm); p.physical_page_count = physical_page_count; p.request_capacity = request_capacity;
+  p.phys_per_row = (uint32_t)(vsm->physical_page_table_size / vsm->page_size); p.size = vsm->page_table_size; p.clipmap_count = vsm->clipmap_count;
+  k_vsm_allocate<<<1, VSM_ALLOC_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_vsm_clear_dirty_pages(OxcContext* c, const OxcVsmContext* vsm, const OxcVsmAllocator* allocator_dev, const uint32_t* dirty_coords_dev,
+                              float* physical_atlas_dev, void* stream) {
+  if (!c || !vsm || !allocator_dev || !dirty_coords_dev || !physical_atlas_dev) return fail(OXC_E_INVALID, "null argument");
+  int rc = check_vsm(vsm, 0xFFFFFFFFu);
+  if (rc != OXC_OK) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  VsmClearParams p{};
+  p.allocator = allocator_dev; p.dirty_coords = reinterpret_cast<const uint2*>(dirty_coords_dev); p.atlas = physical_atlas_dev;
+  p.page_size = (uint32_t)vsm->page_size; p.atlas_size = (uint32_t)vsm->physical_page_table_size; p.phys_per_row = p.atlas_size / p.page_size;
+  p.vec4 = (p.page_size % 4u == 0u && (reinterpret_cast<uintptr_t>(physical_atlas_dev) & 15u) == 0u) ? 1 : 0;
+  p.row_shift = -1;
+  if (p.vec4 && is_pow2(p.page_size / 4u)) p.row_shift = (int)ilog2(p.page_size / 4u);
+  // up to 8 CTAs per SM, never more than there can be dirty pages: a frame with few dirty pages costs a short, mostly idle launch
+  const uint32_t pages = p.phys_per_row * p.phys_per_row;
+  const uint32_t grid = std::min<uint32_t>((uint32_t)c->sm_count * 8u, pages ? pages : 1u);
+  k_vsm_clear_dirty_pages<<<grid, 256, 0, s>>>(p);
+  LAUNCHED();
   return OXC_OK;
 }
 
