@@ -2,9 +2,14 @@
 // Reference: Oxylus/src/Render/Shaders/passes/{cull_meshes,cull_meshlets_hiz,cull_meshlets,cull_meshlets_hpb}.slang
 #pragma once
 #include "oxc_filtered.cuh"
-#include "oxc_tma.cuh"
 
 namespace oxc {
+
+#ifdef OXC_HOST_SOUNDNESS_HARNESS
+OXC_DI void prefetch_l1(const void*) {} // host builds of the headers (tests/): a hint has no result
+#else
+OXC_DI void prefetch_l1(const void* ptr) { asm volatile("prefetch.global.L1 [%0];" ::"l"(ptr)); }
+#endif
 
 #ifndef OXC_CULL_MESHES_THREADS
 #define OXC_CULL_MESHES_THREADS 64
@@ -369,7 +374,6 @@ __global__ void __launch_bounds__(CULL_MESHES_THREADS) k_expand_meshlet_instance
 constexpr int CULL_WARPS = CULL_THREADS / 32;
 constexpr int CULL_Q = 64;        // queue capacity per warp (< 32 carried over + <= 32 appended)
 constexpr int CULL_EMIT = 128;    // survivor staging per warp (flushed above 96)
-constexpr uint32_t CULL_TILE_BYTES = CULL_TILE * sizeof(OxcMeshletInstance);
 
 // queue 0 entry (early pass): where the bounds are + what to update.  16 + 4 B.
 // queue 1 / 2 entry: decoded bounds + the same bookkeeping.  32 + 4 B.
@@ -386,12 +390,6 @@ struct __align__(16) CullShared {
   uint4 q2b[CULL_WARPS][CULL_Q];
   uint32_t q2c[CULL_WARPS][CULL_Q];
   uint32_t emit[CULL_WARPS][CULL_EMIT];
-  // TMA landing zone of the slab's 32 MeshletBounds (512 contiguous bytes when the slab lies in one mesh instance): two slabs are
-  // in flight per warp (the one being tested and the one resolved ahead)
-#ifdef OXC_CULL_TMA_BOUNDS
-  uint4 bnd[CULL_WARPS][Q0 ? 1 : 2][Q0 ? 1 : 32];
-  uint64_t bnd_bar[CULL_WARPS][2];
-#endif
 };
 
 template <bool HIZ, bool OCC, bool LATE, bool ZERO>
@@ -521,17 +519,11 @@ struct CullWarp {
       ex = dequantize_half_hw(b.z & 0xFFFFu); ey = dequantize_half_hw(b.z >> 16); ez = dequantize_half_hw(b.w & 0xFFFFu);
       // :59 frustum (the three tests commute).  Skipped when the whole instance is provably inside every plane for the
       // canonical test (InstCull::nrm[2].w, see k_cull_meshes); else decided by the centre-inside filter when it can.
-#ifndef OXC_EXP_NO_FRUSTUM
       if (__ldg(&ic->nrm[2].w) == 0.0f && !frustum_centre_inside(ic->plane, cx, cy, cz, ex, ey, ez))
         visible = test_frustum_planes(ic->plane, cx, cy, cz, ex, ey, ez);
-#endif
       // :58 cone
       const float cutoff = sh.s8_lut[((b.w >> 24) + 128u) & 0xFFu];
-#ifdef OXC_EXP_NO_CONE
-      if (false) {
-#else
       if (visible && cutoff < 1.0f) {
-#endif
         const ConeInputs ci = cone_inputs(ic, cx, cy, cz, ex, ey, ez, sh.s8_lut[(((b.y >> 16) & 0xFFu) + 128u) & 0xFFu],
                                           sh.s8_lut[((b.y >> 24) + 128u) & 0xFFu], sh.s8_lut[(((b.w >> 16) & 0xFFu) + 128u) & 0xFFu],
                                           cam_pos[0], cam_pos[1], cam_pos[2]);
@@ -539,11 +531,7 @@ struct CullWarp {
         visible = t == TRI_AMBIGUOUS ? cone_visible_exact(ci, cutoff) : (t == TRI_TRUE);
       }
       // :61-65 occlusion
-#ifdef OXC_EXP_NO_OCC // timing experiment only (results are wrong)
-      if (false) {
-#else
       if (HIZ && (OCC || LATE) && visible) {
-#endif
         queue = true;
         if (ZERO) queue = !cleared_hiz_surely_visible(__ldg(&ic->mvp_row[2]), __ldg(&ic->mvp_row[3]), cx, cy, cz, ex, ey, ez);
       }
@@ -587,10 +575,7 @@ struct CullWarp {
     uint4 bounds;
     uint32_t maskw, inst, idx, vi;
     bool valid;
-    bool tma; // warp-uniform: the bounds arrive through the bulk-copy engine in sh.bnd[warp][slab parity]
   };
-  uint32_t n_resolved = 0, n_consumed = 0; // slab counters: landing buffer = count & 1
-  uint32_t bnd_phase = 0;                  // bit b: parity the next wait on buffer b's mbarrier uses (flips per TMA slab consumed)
 
   OXC_DI uint2 load_slab_entry(uint32_t s, uint32_t n_slabs) const { return s < n_slabs ? __ldg(&p.slabs[s]) : make_uint2(0u, 0u); }
   OXC_DI uint4 load_tail(uint32_t s, uint32_t n_slabs, uint2 sl) const {
@@ -600,7 +585,6 @@ struct CullWarp {
   // pass needs every item (late / no mask) — the bounds in flight
   OXC_DI Resolved resolve(uint32_t s, uint32_t total, uint2 sl, uint4 tail) {
     Resolved r;
-    r.tma = false;
     r.idx = s * 32u + lane;
     r.valid = r.idx < total; // also false for s >= n_slabs
     uint32_t cur = sl.x, m = sl.y + lane;
@@ -625,31 +609,10 @@ struct CullWarp {
     if (OCC && !LATE) { // early pass: the bounds are fetched by stage A for the was_visible items only; keep the address
       r.bounds.x = (uint32_t)(uint64_t)bptr; r.bounds.y = (uint32_t)((uint64_t)bptr >> 32);
       if (r.valid) prefetch_l1(bptr);
-    } else {
-      // Every item of the pass needs its bounds.  When the whole slab lies in ONE mesh instance (the common case: a slab is 32
-      // meshlets, an instance 64-256) they are 32 consecutive 16-byte records: one elected lane hands the run to the bulk-copy
-      // engine (TMA, cp.async.bulk -> SASS UBLKCP) and the warp picks the records up from shared memory a slab later —
-      // north_star's "meshlet bounds ... staged through TMA into shared memory".  A slab that straddles instances falls back
-      // to one 128-bit load per lane.
-      // OPT-IN build flag OXC_CULL_TMA_BOUNDS: bit-identical, but a warp-wide LDG.128 of 512 contiguous bytes is already four
-      // full 128-byte lines in one instruction, issued a slab ahead; the bulk copy adds two votes, an mbarrier round trip and a
-      // shared-memory read per slab and saves nothing.  Default: off.
-#ifdef OXC_CULL_TMA_BOUNDS
-      const uint32_t nv = __popc(__ballot_sync(0xffffffffu, r.valid)); // validity is a prefix of the lanes
-      const bool uniform = nv > 0 && __all_sync(0xffffffffu, !r.valid || cur == sl.x);
-      const uint32_t buf = n_resolved & 1u;
-      if (uniform) {
-        r.tma = true;
-        if (lane == 0) {
-          mbar_expect_tx(&sh.bnd_bar[warp][buf], nv * 16u);
-          tma_load_1d(sh.bnd[warp][buf], bptr, nv * 16u, &sh.bnd_bar[warp][buf]);
-        }
-      } else
-#endif
-      if (r.valid) {
-        r.bounds = __ldg(bptr); // MeshletBounds, one 128-bit load (consecutive lanes: consecutive 16 B records of one LOD)
-      }
-      n_resolved++;
+    } else if (r.valid) {
+      // every item of the pass needs its bounds: one 128-bit load per lane, issued a slab ahead (when the slab lies in one mesh
+      // instance, the warp's 32 consecutive 16-byte records are four full 128-byte lines in one instruction)
+      r.bounds = __ldg(bptr);
     }
     return r;
   }
@@ -671,17 +634,7 @@ struct CullWarp {
         if (n0 >= 32) stage_a_from_q0(32);
       }
     } else {
-      uint4 b = r.bounds;
-#ifdef OXC_CULL_TMA_BOUNDS
-      const uint32_t buf = n_consumed & 1u;
-      if (r.tma) {
-        mbar_wait(&sh.bnd_bar[warp][buf], (bnd_phase >> buf) & 1u); // a barrier only advances on the slabs that used it
-        bnd_phase ^= 1u << buf;
-        b = sh.bnd[warp][buf][lane]; // lanes beyond the copied run read stale bytes they never use (need == false)
-      }
-#endif
-      n_consumed++;
-      stage_a(need, b, r.inst, r.idx, r.vi, was);
+      stage_a(need, r.bounds, r.inst, r.idx, r.vi, was);
     }
   }
 
@@ -725,13 +678,6 @@ __global__ void __launch_bounds__(CULL_THREADS, OXC_CULL_MIN_BLOCKS) k_cull_mesh
   Shared& sh = *reinterpret_cast<Shared*>(cull_smem_raw);
   if (threadIdx.x < OXC_HIZ_MAX_LEVELS) sh.hiz_off[threadIdx.x] = p.hiz.level_offset[threadIdx.x];
   sh.s8_lut[threadIdx.x] = s8_over_127((int)threadIdx.x - 128);
-#ifdef OXC_CULL_TMA_BOUNDS
-  if ((threadIdx.x & 31) == 0) {
-    mbar_init(&sh.bnd_bar[threadIdx.x >> 5][0], 1);
-    mbar_init(&sh.bnd_bar[threadIdx.x >> 5][1], 1);
-    mbar_fence_init();
-  }
-#endif
   __syncthreads();
   const uint32_t total = p.vis->total_visible_meshlet_instances; // :26
   const uint32_t early_count = LATE ? p.vis->early_visible_meshlet_instances : 0u; // :73 (final: the early kernel has completed)

@@ -8,7 +8,6 @@
 
 #include "oxc_exact.cuh"
 #include "oxc_raster_core.cuh"
-#include "oxc_tma.cuh"
 
 namespace oxc {
 
@@ -170,7 +169,6 @@ __global__ void __launch_bounds__(TRI_THREADS) k_cull_triangles(const __grid_con
 #ifndef OXC_RASTER_BATCH
 #define OXC_RASTER_BATCH 32
 #endif
-constexpr int MICRO_STAGE_BYTES = 224;               // 15 (alignment skew) + 192 (64 triangles x 3) rounded up to 16
 constexpr int RASTER_BATCH = OXC_RASTER_BATCH;       // meshlets per work grab
 static_assert(RASTER_BATCH >= 1 && RASTER_BATCH <= 32, "one header per lane: a grab holds at most 32 meshlets");
 constexpr int RASTER_BIG_PIXELS = OXC_RASTER_BIG_PIXELS; // bbox area above which the whole warp rasterises the triangle together
@@ -311,28 +309,10 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
   __shared__ float4 clip_all[TRI_WARPS][OXC_MESHLET_MAX_VERTICES];
   __shared__ ScreenVert scr_all[TRI_WARPS][OXC_MESHLET_MAX_VERTICES];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#ifndef OXC_RASTER_NO_SMEM_MICRO
-#define OXC_RASTER_SMEM_MICRO 1
-#endif
-#ifdef OXC_RASTER_SMEM_MICRO
   // the meshlet's micro-index run (<= 192 B, scene.slang:336-342) staged in shared memory: 49 words cover it plus the byte skew
   // of its start.  Two coalesced loads per warp, issued before the vertex transform, replace three dependent L1 loads + shifts
-  // per triangle.  (The same staging through the bulk-copy engine, OXC_RASTER_TMA_MICRO below, adds live mbarrier state to a
-  // kernel that already spills at its register bound; not timed on H100.)
+  // per triangle.
   __shared__ uint32_t micro_w[TRI_WARPS][52];
-#endif
-#ifdef OXC_RASTER_TMA_MICRO
-  // OPT-IN (north_star: "micro-index data staged through TMA into shared memory"): the meshlet's micro-index run (<= 192 B,
-  // scene.slang:336-342) is staged by the bulk-copy engine (cp.async.bulk -> SASS UBLKCP) while the vertices are transformed, and
-  // the 3 byte fetches per triangle become shared-memory byte loads.  Bit-identical output, but the three extra live values
-  // add spills to a hot loop that already spills at the kernel's register bound (80 at 3 CTAs / SM), and the L1-resident LDG
-  // it replaces is not the bottleneck.  Not timed on H100.  Default off.
-  __shared__ __align__(16) uint8_t micro_all[TRI_WARPS][MICRO_STAGE_BYTES];
-  __shared__ __align__(8) uint64_t micro_bar[TRI_WARPS];
-  if (lane == 0) { mbar_init(&micro_bar[warp], 1); mbar_fence_init(); }
-  __syncwarp();
-  uint32_t micro_phase = 0; // parity of the warp's mbarrier: one bulk copy per meshlet
-#endif
   const uint32_t first = p.late ? p.vis->early_visible_meshlet_instances : 0u; // cull_triangles.slang:34-37
   const uint32_t count = p.tri_cmd->x;                                         // dispatch_indirect(cull_triangles_cmd), CullGeometry.cpp:365
   const uint32_t id_base = p.id_base ? __ldg(p.id_base) : 0u;
@@ -404,18 +384,6 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
 #endif
     for (uint32_t j = 0; j < nb; j++) {
       const MeshletHeader w = cur;
-#ifdef OXC_RASTER_TMA_MICRO
-      // micro indices of this meshlet -> shared memory, asynchronously (16-byte aligned window around the run; the blob is
-      // padded so the window never leaves the allocation)
-      const uint64_t micro_addr = reinterpret_cast<uint64_t>(w.micro) + w.tri_offset;
-      const uint32_t micro_skew = (uint32_t)(micro_addr & 15u);
-      if (lane == 0) {
-        const uint32_t bytes = (micro_skew + w.tri_count * 3u + 15u) & ~15u;
-        mbar_expect_tx(&micro_bar[warp], bytes);
-        tma_load_1d(micro_all[warp], reinterpret_cast<const void*>(micro_addr - micro_skew), bytes, &micro_bar[warp]);
-      }
-#endif
-#ifdef OXC_RASTER_SMEM_MICRO
       {  // words [tri_offset / 4, ...) covering the run: two coalesced loads per warp, in flight during the vertex phase
         const uint32_t n_words = ((w.tri_offset & 3u) + w.tri_count * 3u + 3u) >> 2;
         const uint32_t* src = w.micro + (w.tri_offset >> 2);
@@ -424,7 +392,6 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
         micro_w[warp][lane] = m0;
         if (lane < 20) micro_w[warp][lane + 32] = m1;
       }
-#endif
       // positions of this meshlet (indices already here) ...
       const uint2 q0 = lane < w.vertex_count ? __ldg(&w.pos[vi0]) : make_uint2(0, 0);
       const uint2 q1 = lane + 32u < w.vertex_count ? __ldg(&w.pos[vi1]) : make_uint2(0, 0);
@@ -450,11 +417,6 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
         scr_s[lane + 32] = to_screen(c, p.f_width, p.f_height);
       }
       __syncwarp();
-#ifdef OXC_RASTER_TMA_MICRO
-      mbar_wait(&micro_bar[warp], micro_phase); // the micro indices have landed (usually long ago)
-      micro_phase ^= 1u;
-      const uint8_t* micro_s = micro_all[warp] + micro_skew;
-#endif
       const uint32_t rounds = (w.tri_count + 31u) >> 5;
 #if defined(OXC_RASTER_STATS) && OXC_RASTER_STATS == 1
       bool meshlet_draws = false;
@@ -468,15 +430,8 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
         int why_stat = -1;
 #endif
         if (t < w.tri_count) {
-#ifdef OXC_RASTER_TMA_MICRO
-          const uint32_t i0 = micro_s[t * 3u + 0u], i1 = micro_s[t * 3u + 1u], i2 = micro_s[t * 3u + 2u];
-#elif defined(OXC_RASTER_SMEM_MICRO)
           const uint8_t* mb = reinterpret_cast<const uint8_t*>(micro_w[warp]) + (w.tri_offset & 3u) + t * 3u;
           const uint32_t i0 = mb[0], i1 = mb[1], i2 = mb[2];
-#else
-          const uint32_t base = w.tri_offset + t * 3u;
-          const uint32_t i0 = micro_index(w.micro, base + 0u), i1 = micro_index(w.micro, base + 1u), i2 = micro_index(w.micro, base + 2u);
-#endif
           if (max(i0, max(i1, i2)) < w.vertex_count) { // malformed meshlets never index past the transformed vertices
             const float4 c0 = clip_s[i0], c1 = clip_s[i1], c2 = clip_s[i2];
             pass = c0.z >= 0.0f && c1.z >= 0.0f && c2.z >= 0.0f && !triangle_backface(c0, c1, c2); // cull_triangles.slang:68-69

@@ -193,6 +193,27 @@ int dalloc(T** p, size_t n) {
   return OXC_OK;
 }
 
+// Grid of a persistent kernel: blocks_per_sm CTAs per SM (one when the occupancy query found none), but no more CTAs than
+// max_meshlet_instances / items_per_block, and at least one.
+uint32_t persistent_grid(const OxcContext* c, uint32_t items_per_block, int blocks_per_sm) {
+  const uint32_t tiles = (c->info.max_meshlet_instances + items_per_block - 1) / items_per_block;
+  const uint32_t grid = std::min((uint32_t)(c->sm_count * (blocks_per_sm > 0 ? blocks_per_sm : 1)), tiles);
+  return grid ? grid : 1u;
+}
+
+// Grid of a 256-thread grid-stride kernel over n items: one CTA per 256 items, at most 8 per SM, at least one.
+uint32_t capped_grid(const OxcContext* c, size_t n) {
+  const size_t grid = std::min((n + 255) / 256, (size_t)c->sm_count * 8);
+  return grid ? (uint32_t)grid : 1u;
+}
+
+int check_vis_id_bits(const OxcContext* c) {
+  if (c->scene_id_bound > (1ull << (32u - c->prim_bits)))
+    return fail(OXC_E_CAPACITY, "the scene can emit %llu meshlet instances: ids overflow the %u id bits of the vis-buffer word (visbuffer.slang:9-10)%s",
+                (unsigned long long)c->scene_id_bound, 32u - c->prim_bits, c->info.wide_ids ? "" : "; create the context with wide_ids = 1 (26 + 6 bit packing)");
+  return OXC_OK;
+}
+
 void shard_range(const OxcContext* c, uint32_t cam_count, uint32_t* first, uint32_t* count) {
   uint32_t n = cam_count < c->mesh_instance_count ? cam_count : c->mesh_instance_count; // cull_meshes.slang:28
   uint32_t lo = c->shard_first < n ? c->shard_first : n;
@@ -212,6 +233,17 @@ uint64_t shard_need(const std::vector<uint64_t>& prefix, uint32_t first, uint32_
   if (count != 0xFFFFFFFFu && (uint64_t)first + count < hi) hi = (uint64_t)first + count;
   if (hi < lo) hi = lo;
   return prefix[hi] - prefix[lo];
+}
+
+// oxc_set_shard / oxc_set_shard_auto (automatic: oxc_cull_meshes computes the id base into d_id_base_auto; id_base is ignored)
+int set_shard(OxcContext* c, uint32_t first, uint32_t count, const uint32_t* id_base, bool automatic) {
+  if (!c) return fail(OXC_E_INVALID, "null context");
+  if (c->scene_set && shard_need(c->id_prefix, first, count) > c->info.max_meshlet_instances)
+    return fail(OXC_E_CAPACITY, "mesh instances [%u, +%u) can emit %llu meshlet instances > max_meshlet_instances %u", first, count,
+                (unsigned long long)shard_need(c->id_prefix, first, count), c->info.max_meshlet_instances);
+  c->shard_first = first; c->shard_count = count; c->id_base = automatic ? c->d_id_base_auto : id_base; c->id_base_auto = automatic;
+  c->cache_valid = false;
+  return OXC_OK;
 }
 
 bool same_camera(const OxcCullCamera& a, const OxcCullCamera& b) {
@@ -275,7 +307,7 @@ int oxc_create(int device, const OxcCreateInfo* info, OxcContext** out_ctx) {
   TRY(dalloc(&c->d_geom, (size_t)I));
   TRY(dalloc(&c->d_counts, (size_t)I));
   TRY(dalloc(&c->d_block_sums, (size_t)(I + CULL_MESHES_THREADS - 1) / CULL_MESHES_THREADS + 1));
-  TRY(dalloc(&c->d_meshlet_instances, (size_t)N + CULL_TILE)); // + one tile: full-size bulk copies of the last tile stay in bounds
+  TRY(dalloc(&c->d_meshlet_instances, (size_t)N + CULL_TILE)); // + one tile: slack kept from a removed bulk copy of the last tile
   TRY(dalloc(&c->d_slabs, (size_t)N / 32 + 2));
   TRY(dalloc(&c->d_visible, (size_t)N));
   c->mask_words = ((info->max_mask_bits > N ? info->max_mask_bits : N) + 31) / 32; // RendererInstance.cpp:1651
@@ -520,8 +552,8 @@ int oxc_set_scene(OxcContext* c, const OxcSceneDesc* sc, void* stream) {
   }
   if (upload_size > c->blob_cap) {
     CK(cudaFree(c->d_blob)); c->d_blob = nullptr;
-    CK(cudaMalloc(&c->d_blob, (size_t)upload_size + 64)); // + slack: the raster's 16-byte aligned bulk copies of micro-index runs may
-    c->blob_cap = upload_size;                            //   read up to 15 bytes past the last run
+    CK(cudaMalloc(&c->d_blob, (size_t)upload_size + 64)); // + slack: the raster stages micro-index runs in whole words, so a run
+    c->blob_cap = upload_size;                            //   that ends at the blob's last byte is read up to 3 bytes past it
   }
   CK(cudaMemcpyAsync(c->d_meshes, sc->meshes, (size_t)sc->mesh_count * sizeof(OxcMesh), cudaMemcpyHostToDevice, s));
   CK(cudaMemcpyAsync(c->d_mesh_instances, sc->mesh_instances, (size_t)sc->mesh_instance_count * sizeof(OxcMeshInstance), cudaMemcpyHostToDevice, s));
@@ -572,25 +604,8 @@ int oxc_clear_hiz(OxcContext* c, void* stream) {
   return OXC_OK;
 }
 
-int oxc_set_shard(OxcContext* c, uint32_t first, uint32_t count, const uint32_t* id_base_dev) {
-  if (!c) return fail(OXC_E_INVALID, "null context");
-  if (c->scene_set && shard_need(c->id_prefix, first, count) > c->info.max_meshlet_instances)
-    return fail(OXC_E_CAPACITY, "mesh instances [%u, +%u) can emit %llu meshlet instances > max_meshlet_instances %u", first, count,
-                (unsigned long long)shard_need(c->id_prefix, first, count), c->info.max_meshlet_instances);
-  c->shard_first = first; c->shard_count = count; c->id_base = id_base_dev; c->id_base_auto = false;
-  c->cache_valid = false;
-  return OXC_OK;
-}
-
-int oxc_set_shard_auto(OxcContext* c, uint32_t first, uint32_t count) {
-  if (!c) return fail(OXC_E_INVALID, "null context");
-  if (c->scene_set && shard_need(c->id_prefix, first, count) > c->info.max_meshlet_instances)
-    return fail(OXC_E_CAPACITY, "mesh instances [%u, +%u) can emit %llu meshlet instances > max_meshlet_instances %u", first, count,
-                (unsigned long long)shard_need(c->id_prefix, first, count), c->info.max_meshlet_instances);
-  c->shard_first = first; c->shard_count = count; c->id_base = c->d_id_base_auto; c->id_base_auto = true;
-  c->cache_valid = false;
-  return OXC_OK;
-}
+int oxc_set_shard(OxcContext* c, uint32_t first, uint32_t count, const uint32_t* id_base_dev) { return set_shard(c, first, count, id_base_dev, false); }
+int oxc_set_shard_auto(OxcContext* c, uint32_t first, uint32_t count) { return set_shard(c, first, count, nullptr, true); }
 
 int oxc_cull_meshes(OxcContext* c, const OxcCullCamera* cam, uint32_t flags, void* stream) {
   if (!c || !cam) return fail(OXC_E_INVALID, "null argument");
@@ -646,11 +661,7 @@ int oxc_cull_meshlets(OxcContext* c, const OxcCullCamera* cam, uint32_t flags, i
   const bool hizp = use_hiz != 0;
   const bool occ = hizp && (flags & OXC_CULL_TEST_OCCLUSION) != 0;
   const bool late = hizp && (flags & OXC_CULL_LATE_PASS) != 0;
-  const uint32_t tiles = (c->info.max_meshlet_instances + CULL_THREADS - 1) / CULL_THREADS;
-  int occn = c->occ_cull[hizp][occ][late];
-  uint32_t grid = (uint32_t)(c->sm_count * (occn > 0 ? occn : 1));
-  if (grid > tiles) grid = tiles;
-  if (grid == 0) grid = 1;
+  const uint32_t grid = persistent_grid(c, CULL_THREADS, c->occ_cull[hizp][occ][late]);
 #define GO(H, O, L, Z) k_cull_meshlets<H, O, L, Z><<<grid, CULL_THREADS, sizeof(CullShared<O && !L>), s>>>(p)
   const bool zero = hizp && c->hiz_zero;
   if (hizp) {
@@ -722,6 +733,35 @@ static int tri_common(OxcContext* c, const OxcCullCamera* cam, uint32_t flags, c
   return OXC_OK;
 }
 
+// the packed image a raster pass writes, and the chunk queue its large triangles go to (k_raster_big)
+static void raster_target(const OxcContext* c, uint64_t* vis, uint32_t w, uint32_t h, TriParams* p) {
+  p->visbuf = reinterpret_cast<unsigned long long*>(vis); p->width = w; p->height = h; p->f_width = (float)w; p->f_height = (float)h;
+  p->big_queue = c->d_big_queue; p->big_counters = c->d_big_counters; p->big_capacity = c->big_capacity;
+}
+
+// the material table of the alpha test (none when oxc_set_materials holds no alpha-tested material)
+static AlphaParams alpha_materials(const OxcContext* c) {
+  AlphaParams ap{};
+  ap.mesh_instances = c->d_mesh_instances;
+  if (c->alpha_active) { ap.materials = c->d_alpha_materials; ap.material_count = c->alpha_material_count; }
+  return ap;
+}
+
+// visbuffer_encode.slang:54-66: splits the pass's survivors by material (kernels_alpha.cuh) and points *pm, what the plain
+// raster walks, at the opaque part
+static int split_alpha(OxcContext* c, const TriParams& p, cudaStream_t s, TriParams* pm, AlphaParams* ap) {
+  *ap = alpha_materials(c);
+  ap->opaque_list = c->d_alpha_lists; ap->masked_list = c->d_alpha_lists + c->info.max_meshlet_instances;
+  ap->opaque_cmd = reinterpret_cast<OxcDispatchIndirectCommand*>(c->d_alpha_cmd);
+  ap->masked_cmd = reinterpret_cast<OxcDispatchIndirectCommand*>(c->d_alpha_cmd + 16);
+  CK(cudaMemsetAsync(c->d_alpha_cmd, 0, 64, s));
+  k_partition_alpha<<<c->sm_count * 4, 256, 0, s>>>(p, *ap);
+  LAUNCHED();
+  pm->visible_indices = ap->opaque_list; pm->tri_cmd = ap->opaque_cmd;
+  pm->vis = reinterpret_cast<const OxcMeshletInstanceVisibility*>(c->d_alpha_cmd + 32); // the list starts at 0 in either pass
+  return OXC_OK;
+}
+
 static int cull_triangles_impl(OxcContext* c, const OxcCullCamera* cam, uint32_t flags, uint32_t spc, uint32_t w, uint32_t h, void* stream);
 
 int oxc_cull_triangles(OxcContext* c, const OxcCullCamera* cam, uint32_t flags, void* stream) {
@@ -747,11 +787,7 @@ static int cull_triangles_impl(OxcContext* c, const OxcCullCamera* cam, uint32_t
   p.small_primitive_cull = spc; p.width = w; p.height = h; p.f_width = (float)w; p.f_height = (float)h;
   k_reset_draw_cmd<<<1, 1, 0, s>>>(c->d_draw_cmd); // CullGeometry.cpp:380-382
   LAUNCHED();
-  uint32_t tiles = (c->info.max_meshlet_instances + TRI_WARPS - 1) / TRI_WARPS;
-  uint32_t grid = (uint32_t)(c->sm_count * (c->occ_tri > 0 ? c->occ_tri : 1));
-  if (grid > tiles) grid = tiles;
-  if (grid == 0) grid = 1;
-  k_cull_triangles<<<grid, TRI_THREADS, 0, s>>>(p);
+  k_cull_triangles<<<persistent_grid(c, TRI_WARPS, c->occ_tri), TRI_THREADS, 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }
@@ -770,36 +806,24 @@ int oxc_clear_visbuffer(OxcContext* c, uint64_t* vis, uint32_t w, uint32_t h, vo
 int oxc_raster_visbuffer(OxcContext* c, const OxcCullCamera* cam, uint32_t flags, uint32_t w, uint32_t h, uint64_t* vis,
                          int small_primitive_cull, void* stream) {
   if (!c || !cam || !vis) return fail(OXC_E_INVALID, "null argument");
-  if (c->scene_id_bound > (1ull << (32u - c->prim_bits)))
-    return fail(OXC_E_CAPACITY, "the scene can emit %llu meshlet instances: ids overflow the %u id bits of the vis-buffer word (visbuffer.slang:9-10)%s",
-                (unsigned long long)c->scene_id_bound, 32u - c->prim_bits, c->info.wide_ids ? "" : "; create the context with wide_ids = 1 (26 + 6 bit packing)");
+  int rc = check_vis_id_bits(c);
+  if (rc != OXC_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
   TriParams p{};
-  int rc = tri_common(c, cam, flags, s, &p);
+  rc = tri_common(c, cam, flags, s, &p);
   if (rc != OXC_OK) return rc;
-  p.visbuf = reinterpret_cast<unsigned long long*>(vis); p.width = w; p.height = h; p.f_width = (float)w; p.f_height = (float)h;
+  raster_target(c, vis, w, h, &p);
   p.small_primitive_cull = small_primitive_cull ? 1u : 0u;
   p.work_counter = c->d_raster_work;
   CK(cudaMemsetAsync(c->d_raster_work, 0, 16, s)); // work counter, chunk-queue counters, clip-queue counter
-  uint32_t tiles = (c->info.max_meshlet_instances + TRI_WARPS - 1) / TRI_WARPS;
-  uint32_t grid = (uint32_t)(c->sm_count * (c->occ_raster > 0 ? c->occ_raster : 1));
-  if (grid > tiles) grid = tiles;
-  if (grid == 0) grid = 1;
-  p.big_queue = c->d_big_queue; p.big_counters = c->d_big_counters; p.big_capacity = c->big_capacity;
+  const uint32_t grid = persistent_grid(c, TRI_WARPS, c->occ_raster);
   p.clip_queue = c->d_clip_queue; p.clip_counter = c->d_clip_counter; p.clip_capacity = c->clip_capacity;
   TriParams pm = p; // what the plain raster kernel walks: the pass's survivors, or their opaque part
   AlphaParams ap{};
-  if (c->alpha_active) { // visbuffer_encode.slang:54-66: split the survivors by material (kernels_alpha.cuh)
-    ap.mesh_instances = c->d_mesh_instances; ap.materials = c->d_alpha_materials; ap.material_count = c->alpha_material_count;
-    ap.opaque_list = c->d_alpha_lists; ap.masked_list = c->d_alpha_lists + c->info.max_meshlet_instances;
-    ap.opaque_cmd = reinterpret_cast<OxcDispatchIndirectCommand*>(c->d_alpha_cmd);
-    ap.masked_cmd = reinterpret_cast<OxcDispatchIndirectCommand*>(c->d_alpha_cmd + 16);
-    CK(cudaMemsetAsync(c->d_alpha_cmd, 0, 64, s));
-    k_partition_alpha<<<c->sm_count * 4, 256, 0, s>>>(p, ap);
-    LAUNCHED();
-    pm.visible_indices = ap.opaque_list; pm.tri_cmd = ap.opaque_cmd;
-    pm.vis = reinterpret_cast<const OxcMeshletInstanceVisibility*>(c->d_alpha_cmd + 32); // the list starts at 0 in either pass
+  if (c->alpha_active) {
+    rc = split_alpha(c, p, s, &pm, &ap);
+    if (rc != OXC_OK) return rc;
   }
   if (p.late) k_raster_visbuffer<true><<<grid, TRI_THREADS, 0, s>>>(pm);
   else k_raster_visbuffer<false><<<grid, TRI_THREADS, 0, s>>>(pm);
@@ -826,9 +850,8 @@ int oxc_raster_overdraw(OxcContext* c, const OxcCullCamera* cam, uint32_t flags,
   int rc = tri_common(c, cam, flags, s, &p);
   if (rc != OXC_OK) return rc;
   p.width = w; p.height = h; p.f_width = (float)w; p.f_height = (float)h;
-  AlphaParams ap{};
-  ap.mesh_instances = c->d_mesh_instances; ap.overdraw = overdraw; ap.count_from_visibility = after_frame ? 1u : 0u;
-  if (c->alpha_active) { ap.materials = c->d_alpha_materials; ap.material_count = c->alpha_material_count; }
+  AlphaParams ap = alpha_materials(c);
+  ap.overdraw = overdraw; ap.count_from_visibility = after_frame ? 1u : 0u;
   k_raster_alpha<true><<<c->sm_count * 8, ALPHA_THREADS, 0, s>>>(p, ap);
   LAUNCHED();
   return OXC_OK;
@@ -917,35 +940,22 @@ int oxc_set_materials(OxcContext* c, const OxcMaterialTable* t, void* stream) {
 int oxc_raster_visbuffer_clip_pass(OxcContext* c, const OxcCullCamera* cam, uint32_t flags, uint32_t w, uint32_t h, uint64_t* vis,
                                    void* stream) {
   if (!c || !cam || !vis) return fail(OXC_E_INVALID, "null argument");
-  if (c->scene_id_bound > (1ull << (32u - c->prim_bits)))
-    return fail(OXC_E_CAPACITY, "the scene can emit %llu meshlet instances: ids overflow the %u id bits of the vis-buffer word (visbuffer.slang:9-10)%s",
-                (unsigned long long)c->scene_id_bound, 32u - c->prim_bits, c->info.wide_ids ? "" : "; create the context with wide_ids = 1 (26 + 6 bit packing)");
+  int rc = check_vis_id_bits(c);
+  if (rc != OXC_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
   TriParams p{};
-  int rc = tri_common(c, cam, flags, s, &p);
+  rc = tri_common(c, cam, flags, s, &p);
   if (rc != OXC_OK) return rc;
-  p.visbuf = reinterpret_cast<unsigned long long*>(vis); p.width = w; p.height = h; p.f_width = (float)w; p.f_height = (float)h;
-  p.big_queue = c->d_big_queue; p.big_counters = c->d_big_counters; p.big_capacity = c->big_capacity;
+  raster_target(c, vis, w, h, &p);
   CK(cudaMemsetAsync(c->d_big_counters, 0, 8, s));
-  uint32_t tiles = (c->info.max_meshlet_instances + TRI_WARPS - 1) / TRI_WARPS;
-  uint32_t grid = (uint32_t)(c->sm_count * 4);
-  if (grid > tiles) grid = tiles;
-  if (grid == 0) grid = 1;
   TriParams pm = p;
   if (c->alpha_active) { // alpha-tested meshlets clip in place (k_raster_alpha) and never depend on the queue: walk the others only
-    AlphaParams ap{};
-    ap.mesh_instances = c->d_mesh_instances; ap.materials = c->d_alpha_materials; ap.material_count = c->alpha_material_count;
-    ap.opaque_list = c->d_alpha_lists; ap.masked_list = c->d_alpha_lists + c->info.max_meshlet_instances;
-    ap.opaque_cmd = reinterpret_cast<OxcDispatchIndirectCommand*>(c->d_alpha_cmd);
-    ap.masked_cmd = reinterpret_cast<OxcDispatchIndirectCommand*>(c->d_alpha_cmd + 16);
-    CK(cudaMemsetAsync(c->d_alpha_cmd, 0, 64, s));
-    k_partition_alpha<<<c->sm_count * 4, 256, 0, s>>>(p, ap);
-    LAUNCHED();
-    pm.visible_indices = ap.opaque_list; pm.tri_cmd = ap.opaque_cmd;
-    pm.vis = reinterpret_cast<const OxcMeshletInstanceVisibility*>(c->d_alpha_cmd + 32);
+    AlphaParams ap;
+    rc = split_alpha(c, p, s, &pm, &ap);
+    if (rc != OXC_OK) return rc;
   }
-  k_raster_clip_pass<<<grid, TRI_THREADS, 0, s>>>(pm);
+  k_raster_clip_pass<<<persistent_grid(c, TRI_WARPS, 4), TRI_THREADS, 0, s>>>(pm);
   LAUNCHED();
   k_raster_big<<<c->sm_count * 8, 256, 0, s>>>(p);
   LAUNCHED();
@@ -1006,11 +1016,7 @@ int oxc_cull_meshlets_multiview(OxcContext* c, const OxcCullCamera* views, uint3
     p.view_pos[v][0] = views[v].position[0]; p.view_pos[v][1] = views[v].position[1]; p.view_pos[v][2] = views[v].position[2];
     p.view_pos[v][3] = 0.f;
   }
-  uint32_t blocks = (c->info.max_meshlet_instances + CULL_THREADS - 1) / CULL_THREADS;
-  uint32_t grid = (uint32_t)(c->sm_count * (c->occ_mv > 0 ? c->occ_mv : 1));
-  if (grid > blocks) grid = blocks;
-  if (grid == 0) grid = 1;
-  k_cull_meshlets_multiview<<<grid, CULL_THREADS, 0, s>>>(p);
+  k_cull_meshlets_multiview<<<persistent_grid(c, CULL_THREADS, c->occ_mv), CULL_THREADS, 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }
@@ -1084,10 +1090,7 @@ int cull_meshlets_hpb(OxcContext* c, const OxcCullCamera* cam, const OxcVirtualC
   p.visible_indices = c->d_visible; p.tri_cmd = c->d_cull_triangles_cmd; p.id_base = c->id_base; p.hpb = hpb_dev;
   p.hpb_size = hpb_size; p.hpb_levels = hpb_levels; p.clipmap_count = n; p.inst_stride = stride;
   p.view_dir[0] = cam->position[0]; p.view_dir[1] = cam->position[1]; p.view_dir[2] = cam->position[2];
-  uint32_t blocks = (c->info.max_meshlet_instances + CULL_THREADS - 1) / CULL_THREADS;
-  uint32_t grid = (uint32_t)c->sm_count * 4u;
-  if (grid > blocks) grid = blocks;
-  if (grid == 0) grid = 1;
+  const uint32_t grid = persistent_grid(c, CULL_THREADS, 4);
   p.dirty_dev = dirty_dev;
   if (dirty_dev) k_cull_meshlets_hpb<true><<<grid, CULL_THREADS, 0, s>>>(p);
   else k_cull_meshlets_hpb<false><<<grid, CULL_THREADS, 0, s>>>(p);
@@ -1130,13 +1133,12 @@ int oxc_decode_visbuffer(OxcContext* c, const OxcCullCamera* cam, const uint64_t
   if (!c || !cam || !t) return fail(OXC_E_INVALID, "null argument");
   if ((vis64_dev == nullptr) == (vis32_dev == nullptr)) return fail(OXC_E_INVALID, "exactly one of vis64_dev / vis32_dev");
   if (!c->scene_set) return fail(OXC_E_STATE, "oxc_set_scene first");
-  if (c->scene_id_bound > (1ull << (32u - c->prim_bits)))
-    return fail(OXC_E_CAPACITY, "the scene can emit %llu meshlet instances: ids overflow the %u id bits of the vis-buffer word (visbuffer.slang:9-10)%s",
-                (unsigned long long)c->scene_id_bound, 32u - c->prim_bits, c->info.wide_ids ? "" : "; create the context with wide_ids = 1 (26 + 6 bit packing)");
+  int rc = check_vis_id_bits(c);
+  if (rc != OXC_OK) return rc;
   if (w == 0 || h == 0) return OXC_OK;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
-  int rc = refresh_inst_cache(c, cam, s); // world rows / normal-matrix rows of the frame's mesh instances
+  rc = refresh_inst_cache(c, cam, s); // world rows / normal-matrix rows of the frame's mesh instances
   if (rc != OXC_OK) return rc;
   DecodeParams p{};
   p.vis64 = reinterpret_cast<const unsigned long long*>(vis64_dev); p.vis32 = vis32_dev;
@@ -1208,8 +1210,7 @@ int oxc_build_hpb(OxcContext* c, const uint32_t* page_table_dev, uint32_t size, 
   for (uint32_t l = 0; l < levels; l++) { // Shadowmaps.cpp:338-360
     const uint32_t sl = (size >> l) ? (size >> l) : 1u, ps = l ? ((size >> (l - 1)) ? (size >> (l - 1)) : 1u) : size;
     const size_t n = (size_t)layers * sl * sl;
-    const uint32_t grid = (uint32_t)((n + 255) / 256 < (size_t)c->sm_count * 8 ? (n + 255) / 256 : (size_t)c->sm_count * 8);
-    k_hpb_level<<<grid ? grid : 1, 256, 0, s>>>(page_table_dev, hpb_dev + src_off, hpb_dev + dst_off, ps, sl, layers, l == 0);
+    k_hpb_level<<<capped_grid(c, n), 256, 0, s>>>(page_table_dev, hpb_dev + src_off, hpb_dev + dst_off, ps, sl, layers, l == 0);
     LAUNCHED();
     src_off = dst_off;
     dst_off += n;
@@ -1616,8 +1617,7 @@ int oxc_mgpu_exchange_hiz(OxcContext* c, const uint64_t* vis, uint32_t w, uint32
   if (m.world == 1) return oxc_build_hiz_packed(c, vis, w, h, stream);
   const size_t n = (size_t)c->hiz.width * c->hiz.height;
   if (m.peer_hiz) {
-    const uint32_t grid = (uint32_t)((n + 255) / 256 < (size_t)c->sm_count * 8 ? (n + 255) / 256 : (size_t)c->sm_count * 8);
-    k_mgpu_hiz_push<<<grid, 256, 0, s>>>(reinterpret_cast<const unsigned long long*>(vis), w, h, c->hiz.width, c->hiz.height, ilog2(c->hiz.width),
+    k_mgpu_hiz_push<<<capped_grid(c, n), 256, 0, s>>>(reinterpret_cast<const unsigned long long*>(vis), w, h, c->hiz.width, c->hiz.height, ilog2(c->hiz.width),
                                          ilog2(c->hiz.height), m.peers, m.d_seq);
     LAUNCHED();
     k_mgpu_signal<<<1, 32, 0, s>>>(m.peers, m.d_seq);
