@@ -254,11 +254,13 @@ enum {
 };
 int oxc_check_status(OxcContext* ctx, void* stream, uint32_t* flags_out /* may be NULL */);
 /* CUDA-graph support: while a DEVICE camera buffer is bound, oxc_cull_meshes / oxc_cull_meshlets (and the InstCull refresh of
- * the triangle passes) read projection_view / position / near_clip / resolution / acceptable_lod_error from it instead of from the
- * by-value copy of their `camera` argument, so a captured frame replays with whatever camera the host copied into the buffer
- * before the launch (the host mirror's oxr_submit does exactly that).  The `camera` argument is still required: host-side
- * decisions (mesh_instance_count, "same camera as the InstCull cache") use it; pass the same camera for every pass of a frame.
- * NULL unbinds. */
+ * the triangle passes and of oxc_decode_visbuffer) read projection_view / position / near_clip / resolution / acceptable_lod_error
+ * from it instead of from the by-value copy of their `camera` argument, so a captured frame replays with whatever camera the host
+ * copied into the buffer before the launch (the host mirror's oxr_submit does exactly that).  The `camera` argument is still
+ * required: host-side decisions (mesh_instance_count, "same camera as the InstCull cache") use it; pass the same camera for every
+ * main-view pass of a frame.  The passes with views of their own never read the bound buffer: oxc_cull_meshlets_hpb /
+ * _hpb_dirty_dev cull against their coarse `camera` argument and oxc_cull_meshlets_multiview / oxc_cull_terrain against their
+ * arguments, bound camera or not.  NULL unbinds. */
 int oxc_bind_camera_buffer(OxcContext* ctx, const OxcCullCamera* camera_dev);
 /* Fills a device camera buffer from PINNED host memory (cudaMallocHost / cudaHostRegister) with a kernel that reads the 96
  * bytes over the bus: capturable, re-reads the host location at every replay, and does not occupy a copy engine. */
@@ -477,7 +479,8 @@ int oxc_cull_meshlets_multiview(OxcContext* ctx, const OxcCullCamera* views, uin
  * z_near, and the hierarchical page-bitmap test test_vsm_page (cull.slang:137-166; nearest, clamped sampling of an R8UI
  * pyramid: 4 corner taps at mip = clamp(ceil(log2(box extent in pages)), 0, levels-1), visible iff any tap != 0); a
  * projection failure counts as visible; first visible clipmap wins.  Survivors are appended like the plain variant
- * (base index from cull_triangles_cmd.x, which is reset first).  Requires OxcCreateInfo::max_views >= clipmap_count.
+ * (base index from cull_triangles_cmd.x, which is reset first).  Requires OxcCreateInfo::max_views >= clipmap_count and
+ * hpb_levels in 1..16 (the range oxc_build_hpb accepts); OXC_E_INVALID otherwise.
  * hpb_dev layout: for level l = 0..levels-1 (side s_l = max(1, hpb_size >> l)): layers x s_l x s_l bytes, layer-major. */
 typedef struct OxcVirtualClipmap { /* SceneGPU.hpp:339-343, scalar layout, 76 B */
   float projection_view_mat[16];

@@ -508,6 +508,10 @@ class Context:
     def mark_hiz_dirty(self):
         _check(self.lib.oxc_mark_hiz_dirty(self.h), "oxc_mark_hiz_dirty")
 
+    def bind_camera_buffer(self, camera_dev):
+        """oxc_bind_camera_buffer: a device OxcCullCamera the main-view passes read instead of their argument (None unbinds)"""
+        _check(self.lib.oxc_bind_camera_buffer(self.h, _ptr(camera_dev)), "oxc_bind_camera_buffer")
+
     # ---- plumbing ----
     def sync(self):
         _check(self.lib.oxc_sync(self.h, self.stream), "oxc_sync")
@@ -588,11 +592,11 @@ class Context:
 class Renderer:
     """OxrRenderer wrapper: the host mirror of RendererInstance (HOST buffers in, HOST buffers out)."""
 
-    def __init__(self, device, scene, alloc_reordered_indices=False):
+    def __init__(self, device, scene, alloc_reordered_indices=False, max_views=0):
         self.lib = load()
         hw, hh = scene.hiz_extent()
         info = abi.CreateInfo(max(1, scene.mesh_instance_count), max(1, scene.max_meshlet_instance_count), hw, hh,
-                              int(alloc_reordered_indices), 0)
+                              int(alloc_reordered_indices), max_views)
         h = C.c_void_p()
         rc = self.lib.oxr_create(device, C.byref(info), scene.width, scene.height, C.byref(h))
         _check(rc, "oxr_create")

@@ -251,15 +251,17 @@ bool same_camera(const OxcCullCamera& a, const OxcCullCamera& b) {
          memcmp(a.position, b.position, sizeof a.position) == 0;
 }
 
-// (re)build InstCull for `cam` without touching LOD selection / counts
-int refresh_inst_cache(OxcContext* c, const OxcCullCamera* cam, cudaStream_t s) {
+// (re)build InstCull for `cam` without touching LOD selection / counts.  bound_camera: the kernel reads a camera bound with
+// oxc_bind_camera_buffer instead of `cam` (the main view's passes); the shadow-clipmap cull passes false, since its coarse view
+// is never the bound frame camera
+int refresh_inst_cache(OxcContext* c, const OxcCullCamera* cam, cudaStream_t s, bool bound_camera = true) {
   if (c->cache_valid && same_camera(c->cached_cam, *cam)) return OXC_OK;
   if (!c->cache_valid) return fail(OXC_E_STATE, "oxc_cull_meshes must run before the meshlet/triangle passes");
   MeshesParams p{};
   p.meshes = c->d_meshes; p.mesh_instances = c->d_mesh_instances; p.transforms = c->d_transforms;
   p.inst = c->d_inst; p.geom = c->d_geom; p.counts = c->d_counts; p.block_sums = c->d_block_sums; p.lod_aabb = c->d_lod_aabb;
   shard_range(c, c->cached_cam.mesh_instance_count, &p.first, &p.count);
-  p.flags = 0; p.select = 0; p.cam = *cam; p.cam_dev = c->cam_dev;
+  p.flags = 0; p.select = 0; p.cam = *cam; p.cam_dev = bound_camera ? c->cam_dev : nullptr;
   if (p.count) {
     k_cull_meshes<<<(p.count + CULL_MESHES_THREADS - 1) / CULL_MESHES_THREADS, CULL_MESHES_THREADS, 0, s>>>(p);
     LAUNCHED();
@@ -1062,12 +1064,13 @@ namespace {
 // oxc_cull_meshlets_hpb (dirty flags on the host) and oxc_cull_meshlets_hpb_dirty_dev (on the device): exactly one is non-null
 int cull_meshlets_hpb(OxcContext* c, const OxcCullCamera* cam, const OxcVirtualClipmap* clipmaps, const uint32_t* dirty,
                       const uint32_t* dirty_dev, uint32_t n, const uint8_t* hpb_dev, uint32_t hpb_size, uint32_t hpb_levels, void* stream) {
-  if (!c || !cam || !clipmaps || !(dirty || dirty_dev) || !hpb_dev || n == 0 || hpb_size == 0 || hpb_levels == 0) return fail(OXC_E_INVALID, "bad argument");
+  if (!c || !cam || !clipmaps || !(dirty || dirty_dev) || !hpb_dev || n == 0 || hpb_size == 0) return fail(OXC_E_INVALID, "bad argument");
+  if (hpb_levels == 0 || hpb_levels > 16) return fail(OXC_E_INVALID, "hpb_levels %u outside 1..16 (oxc_build_hpb's range)", hpb_levels);
   if (n > c->info.max_views || !c->d_inst_views) return fail(OXC_E_CAPACITY, "clipmap_count %u > max_views %u", n, c->info.max_views);
   if (!c->scene_set) return fail(OXC_E_STATE, "oxc_set_scene first");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
-  int rc = refresh_inst_cache(c, cam, s); // InstCull for the coarse view
+  int rc = refresh_inst_cache(c, cam, s, false); // InstCull for the coarse view, from the argument even while a camera is bound
   if (rc != OXC_OK) return rc;
   ViewMatrices vm{};
   HpbParams p{};

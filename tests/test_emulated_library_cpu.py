@@ -97,6 +97,17 @@ def test_gpu_variants_on_the_simt_emulator(emulated):
     assert res.returncode == 0 and m and int(m.group(1)) >= 18 and "skipped" not in res.stdout, res.stdout[-3000:] + res.stderr[-2000:]
 
 
+def test_gpu_culls_on_the_simt_emulator(emulated):
+    """tests/test_gpu_culls.py: the shadow-clipmap cull at every pyramid shape, dirty mask, page offset and clipmap count, steered
+    page edges, shards, the engine's pass order with and without a bound device camera (the Renderer case runs eagerly here: no
+    graph capture), the multi-view cull at 1-16 views, the terrain cull at every grid but 512 x 512, flag subset and Hi-Z state.
+    All 17 of those cases must pass."""
+    res = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", "test_gpu_culls.py"), "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider",
+                          "-k", "not 512x512"], cwd=ROOT, env=emulated, capture_output=True, text=True, timeout=900)
+    m = re.search(r"(\d+) passed", res.stdout)
+    assert res.returncode == 0 and m and int(m.group(1)) >= 17 and "skipped" not in res.stdout, res.stdout[-3000:] + res.stderr[-2000:]
+
+
 @pytest.mark.parametrize("order", ["default", "shuffle"])
 def test_gpu_raster_on_the_simt_emulator(emulated, order):
     """tests/test_gpu_raster.py at the emulator's grid (2 SMs, one raster CTA each: 1024 survivors start a pass at 32-meshlet
