@@ -692,6 +692,35 @@ int oxc_cull_meshlets_hpb_dirty_dev(OxcContext* ctx, const OxcCullCamera* camera
                                     const uint32_t* clipmap_dirty_flags_dev, uint32_t clipmap_count, const uint8_t* hpb_dev,
                                     uint32_t hpb_size, uint32_t hpb_levels, void* stream);
 
+/* The VSM shadow raster into the physical atlas: the last step of draw_virtual_shadowmap (Shadowmaps.cpp:433-754,
+ * rmvsm_build_draw_commands.slang, rmvsm_draw_physical_pages.slang), drawn in software.  Draws the survivors of the context's
+ * last oxc_cull_meshlets_hpb / _hpb_dirty_dev (its list and count stay on the device) into physical_atlas_dev (R32F,
+ * physical_page_table_size^2 texels, row-major, written through its R32UI view).  Specification (oracle/oxc_oracle_vsm_draw.c
+ * orc_vsm_draw_pages, bit for bit):
+ *   - triangles: exactly those cull_triangles keeps with the COARSE camera (all three clip.z >= 0 and det < 1e-4 of PV . W,
+ *     cull_triangles.slang:62-69), evaluated once per triangle;
+ *   - for every clipmap c with clipmap_dirty_flags_dev[c] != 0 (read on the device): clip = mul(clipmaps[c].projection_view_mat,
+ *     (mul(world, (p, 1)).xyz, 1)) in the canonical order; raster target W = H = physical_page_table_size;
+ *   - the raster specification of oxc_raster_visbuffer (24.8 snapping, pixel-centre samples, top-left tie-break, z = (za + E_b*dzb)
+ *     + E_c*dzc) drawing BOTH windings (cullMode None: a triangle of the other winding is re-oriented; zero area draws nothing);
+ *     triangles with a vertex at w <= 0 or beyond the 2^22 snap range go through the vis raster's Sutherland-Hodgman clipper;
+ *   - per sample, in f32 in the shader's order: virtual_uv = (px + 0.5, py + 0.5) / physical_page_table_size, page =
+ *     i32(floor(virtual_uv * page_table_size)) wrapped by the clipmap's page_offset (rmvsm.slang:129-138); only an entry that is
+ *     Backed && Dirty is written, whatever its Visible bit; texel = physical page coordinates * page_size +
+ *     i32(mod(floor(virtual_uv * physical_page_table_size), page_size)); a texel outside the atlas is not written;
+ *   - the alpha test of oxc_set_materials (the same as the vis-buffer encode's, uv carried through the clipper);
+ *   - the sink: fragments with z outside [0, 1] are dropped, texel = min(texel bits, asuint(z)) as u32 (-0 stored as +0).
+ * Deviation: the depth is NDC z = clip.z / clip.w.  The reference writes SV_Position.z / SV_Position.w, which is NDC z for the
+ * orthographic clipmaps it builds (w = 1) whichever convention the compiler uses for SV_Position.w.
+ * The context's scratch (page bitmap, work queue) is allocated by the first call: capture the call into a CUDA graph after one
+ * eager call.  Same argument checks as the other oxc_vsm_* calls, plus physical_page_table_size <= 16384 (the snap range);
+ * OXC_E_STATE without a scene or before oxc_cull_meshes. */
+int oxc_vsm_draw_pages(OxcContext* ctx, const OxcVsmContext* vsm, const OxcCullCamera* coarse, const OxcVirtualClipmap* clipmaps /* host */,
+                       const uint32_t* clipmap_dirty_flags_dev, const uint32_t* page_tables_dev, float* physical_atlas_dev, void* stream);
+/* Counters of the last oxc_vsm_draw_pages on `stream` (synchronous): out[0] = (triangle, clipmap, dirty page) work items,
+ * out[1] = (meshlet, clipmap) pairs whose page rectangle held a dirty page and so reached triangle work. */
+int oxc_vsm_draw_stats(OxcContext* ctx, uint32_t out[2], void* stream);
+
 int oxc_get_outputs(OxcContext* ctx, OxcOutputs* out);
 /* Instrumentation hook: 128 u64 counters that builds with -DOXC_RASTER_STATS fill (tools/raster_stats.py); zero otherwise. */
 void* oxc_debug_stats_ptr(OxcContext* ctx);
@@ -784,6 +813,18 @@ typedef struct OxrVsmPages {               /* device pointers, valid until the n
 } OxrVsmPages;
 int oxr_vsm_update_pages(OxrRenderer* r, const OxrVsmPageContext* context);
 int oxr_vsm_pages(OxrRenderer* r, OxrVsmPages* out);
+/* RendererInstance::draw_virtual_shadowmap's last step (Shadowmaps.cpp:433-754): cull_geometry with use_hpb for the coarse camera
+ * (clipmap 9's projection_view as projection_view, near_clip = z_near, position = -light_dir): oxc_cull_meshes, then
+ * oxc_cull_meshlets_hpb_dirty_dev on the device dirty flags, then oxc_vsm_draw_pages into the renderer's atlas, with the clipmaps,
+ * flags, HPB and page table of the last oxr_vsm_update_pages, on the renderer's stream.  Synchronous.  It runs on a second context
+ * the renderer keeps with the same scene, transforms and materials, so the next oxr_render / oxr_submit computes exactly what it
+ * would have without it, and oxr_overdraw still sees the last frame's survivors.  OXC_E_STATE before an oxr_vsm_update_pages.
+ * Footprint: oxr_create makes that context with the renderer's OxcCreateInfo (max_views raised to 10), and every oxr_update /
+ * oxr_update_transforms / oxr_set_materials is applied to it as well — a second device copy of the scene blob and tables and of
+ * the per-meshlet-instance buffers, plus 16 MiB of draw scratch at the first call.  The scene reaches the renderer only through
+ * oxr_update, so the context cannot be made later from it.  If the context cannot be created or kept in step (out of device memory),
+ * the camera path is unaffected and this call returns OXC_E_CAPACITY. */
+int oxr_vsm_draw_shadows(OxrRenderer* r, const OxcCullCamera* coarse);
 
 /* ------------------------------------------------------------------------------------------------
  * oxb_* — mesh builder (SURVEY §8f.2): host-side producer of the blob layout above, mirroring build_gltf_mesh

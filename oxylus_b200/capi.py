@@ -21,12 +21,13 @@ SYMBOLS = [
     "oxc_raster_visbuffer", "oxc_raster_visbuffer_clip_pass", "oxc_set_materials", "oxc_raster_overdraw", "oxc_clear_overdraw", "oxc_resolve_visbuffer", "oxc_merge_depth", "oxc_clear_visbuffer_with_depth", "oxc_cull_meshlets_multiview", "oxc_cull_meshlets_hpb", "oxc_cull_terrain",
     "oxc_decode_visbuffer", "oxc_build_hpb", "oxc_mark_visible_pages",
     "oxc_vsm_begin_frame", "oxc_vsm_invalidate_pages", "oxc_vsm_allocate_pages", "oxc_vsm_clear_dirty_pages", "oxc_cull_meshlets_hpb_dirty_dev",
+    "oxc_vsm_draw_pages", "oxc_vsm_draw_stats",
     "oxc_get_outputs", "oxc_check_status", "oxc_mark_hiz_dirty", "oxc_bind_camera_buffer", "oxc_load_camera", "oxc_debug_stats_ptr",
     "oxc_mgpu_get_unique_id", "oxc_mgpu_init", "oxc_mgpu_init_with_comm", "oxc_mgpu_shutdown", "oxc_mgpu_info", "oxc_mgpu_exchange_hiz",
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
     "oxb_last_error", "oxb_build_mesh", "oxb_mesh_blob_size", "oxb_mesh_lod0_meshlet_count", "oxb_mesh_emit", "oxb_mesh_free", "oxb_simplify",
     "oxr_create", "oxr_destroy", "oxr_context", "oxr_update", "oxr_update_transforms", "oxr_set_external_depth", "oxr_set_materials", "oxr_overdraw", "oxr_render", "oxr_submit", "oxr_wait",
-    "oxr_vsm_update_pages", "oxr_vsm_pages",
+    "oxr_vsm_update_pages", "oxr_vsm_pages", "oxr_vsm_draw_shadows",
 ]
 
 
@@ -90,6 +91,8 @@ def load(build_if_missing=True):
     lib.oxc_vsm_allocate_pages.argtypes = [vp, vp, vp, vp, u32, vp, u32, vp, vp, vp, vp, vp]
     lib.oxc_vsm_clear_dirty_pages.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.oxc_cull_meshlets_hpb_dirty_dev.argtypes = [vp, vp, vp, vp, u32, vp, u32, u32, vp]
+    lib.oxc_vsm_draw_pages.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.oxc_vsm_draw_stats.argtypes = [vp, vp, vp]
     lib.oxc_get_outputs.argtypes = [vp, C.POINTER(abi.Outputs)]
     lib.oxc_check_status.argtypes = [vp, vp, C.POINTER(C.c_uint32)]
     lib.oxc_mark_hiz_dirty.argtypes = [vp]
@@ -136,6 +139,7 @@ def load(build_if_missing=True):
     lib.oxr_render.argtypes = [vp, vp, vp, vp, vp, vp, u32, C.POINTER(abi.FrameResult)]
     lib.oxr_vsm_update_pages.argtypes = [vp, C.POINTER(abi.VsmPageContext)]
     lib.oxr_vsm_pages.argtypes = [vp, C.POINTER(abi.VsmPages)]
+    lib.oxr_vsm_draw_shadows.argtypes = [vp, vp]
     _LIB = lib
     return lib
 
@@ -447,6 +451,18 @@ class Context:
         _check(self.lib.oxc_cull_meshlets_hpb_dirty_dev(self.h, _ptr(cam), _ptr(cm), _ptr(dirty_flags_dev), len(cm), _ptr(hpb_dev), hpb_size,
                                                         hpb_levels, self.stream), "oxc_cull_meshlets_hpb_dirty_dev")
 
+    def vsm_draw_pages(self, vsm, coarse, clipmaps, dirty_flags_dev, page_tables_dev, atlas_dev):
+        """oxc_vsm_draw_pages: the survivors of the last HPB cull drawn into the physical atlas (device pointers)"""
+        vc, cm = np.ascontiguousarray(vsm), np.ascontiguousarray(clipmaps)
+        _check(self.lib.oxc_vsm_draw_pages(self.h, _ptr(vc), _ptr(coarse), _ptr(cm), _ptr(dirty_flags_dev), _ptr(page_tables_dev), _ptr(atlas_dev),
+                                           self.stream), "oxc_vsm_draw_pages")
+
+    def vsm_draw_stats(self):
+        """oxc_vsm_draw_stats: dict(items=, pairs=) of the last oxc_vsm_draw_pages"""
+        out = np.zeros(2, dtype=np.uint32)
+        _check(self.lib.oxc_vsm_draw_stats(self.h, _ptr(out), self.stream), "oxc_vsm_draw_stats")
+        return dict(items=int(out[0]), pairs=int(out[1]))
+
     def build_hpb(self, page_table_dev, size, layers, hpb_dev, levels):
         _check(self.lib.oxc_build_hpb(self.h, _ptr(page_table_dev), size, layers, _ptr(hpb_dev), levels, self.stream), "oxc_build_hpb")
 
@@ -675,6 +691,11 @@ class Renderer:
         c.hpb_levels = hpb_levels
         _check(self.lib.oxr_vsm_update_pages(self.h, C.byref(c)), "oxr_vsm_update_pages")
         return self.vsm_pages()
+
+    def vsm_draw_shadows(self, coarse):
+        """oxr_vsm_draw_shadows: the shadow casters of the last vsm_update_pages drawn into the renderer's atlas (coarse: the
+        clipmap-9 camera, Shadowmaps.cpp:433-463)"""
+        _check(self.lib.oxr_vsm_draw_shadows(self.h, _ptr(coarse)), "oxr_vsm_draw_shadows")
 
     def vsm_pages(self):
         """oxr_vsm_pages: abi.VsmPages of device pointers and sizes"""

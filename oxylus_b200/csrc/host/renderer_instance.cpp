@@ -50,6 +50,11 @@ RendererInstance::RendererInstance(int device, const OxcCreateInfo& info, uint32
     ctx_ = nullptr;
     return;
   }
+  { // the shadow draw's context; a card without room for it keeps the camera path (oxr_vsm_draw_shadows then refuses)
+    OxcCreateInfo si = info;
+    si.max_views = si.max_views > 10 ? si.max_views : 10;
+    if (oxc_create(device, &si, &shadow_ctx_) != OXC_OK) shadow_ctx_ = nullptr;
+  }
   cudaStream_t s = nullptr;
   const size_t px = (size_t)width * height;
   if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess ||
@@ -111,6 +116,7 @@ RendererInstance::~RendererInstance() {
   if (ev_window_) cudaEventDestroy(static_cast<cudaEvent_t>(ev_window_));
   if (copy_stream_) cudaStreamDestroy(static_cast<cudaStream_t>(copy_stream_));
   if (stream_) cudaStreamDestroy(static_cast<cudaStream_t>(stream_));
+  oxc_destroy(shadow_ctx_);
   oxc_destroy(ctx_);
 }
 
@@ -122,6 +128,7 @@ auto RendererInstance::update(const RendererInstanceUpdateInfo& info) -> int {
   oxc_bind_camera_buffer(ctx_, nullptr);
   int rc = oxc_set_scene(ctx_, &info.scene, stream_);
   if (rc != OXC_OK) return fail(rc);
+  if (shadow_ctx_ && oxc_set_scene(shadow_ctx_, &info.scene, stream_) != OXC_OK) drop_shadow_context(); // camera path unaffected
   // a new scene has no motion yet: previous transforms = current
   const uint32_t n = info.scene.transform_count;
   transforms_.assign(info.scene.transforms, info.scene.transforms + n);
@@ -142,6 +149,7 @@ auto RendererInstance::update_transforms(const OxcTransformWorld* transforms, ui
   if (!ctx_) return OXC_E_STATE;
   int rc = oxc_update_transforms(ctx_, transforms, first, count, stream_);
   if (rc != OXC_OK) return fail(rc);
+  if (shadow_ctx_ && oxc_update_transforms(shadow_ctx_, transforms, first, count, stream_) != OXC_OK) drop_shadow_context();
   // the replaced values become the previous transforms (pageable source: the copy has left transforms_ when the call returns)
   if (count && cudaMemcpyAsync(d_transforms_previous_ + first, transforms_.data() + first, (size_t)count * sizeof(OxcTransformWorld),
                                cudaMemcpyHostToDevice, static_cast<cudaStream_t>(stream_)) != cudaSuccess)
@@ -207,6 +215,7 @@ auto RendererInstance::update_virtual_shadow_pages(VsmPageContext& context) -> i
       vsm.physical_page_table_size % vsm.page_size != 0)
     return OXC_E_INVALID;
   if (vsm.depth_extent[0] != (int32_t)width_ || vsm.depth_extent[1] != (int32_t)height_) return OXC_E_INVALID;
+  vsm_.updated = false;
   int rc = vsm_allocate(vsm, context.hpb_levels);
   if (rc != OXC_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream_);
@@ -248,7 +257,36 @@ auto RendererInstance::update_virtual_shadow_pages(VsmPageContext& context) -> i
     error_ = cudaGetErrorString(cudaGetLastError());
     return OXC_E_CUDA;
   }
+  std::memcpy(vsm_.clipmaps, context.clipmaps, sizeof vsm_.clipmaps);
+  vsm_.updated = true;
   return OXC_OK;
+}
+
+// Shadowmaps.cpp:433-754 after the page loop: cull_geometry(use_hpb) for the coarse camera (cull_meshes, the HPB cull on the device
+// dirty flags), then rmvsm_build_draw_commands + rmvsm_draw_physical_pages as one oxc_vsm_draw_pages, on stream_, synchronous
+auto RendererInstance::draw_virtual_shadows(const OxcCullCamera& coarse) -> int {
+  if (!ctx_ || !error_.empty()) return OXC_E_STATE;
+  if (!shadow_ctx_) return OXC_E_CAPACITY; // its context could not be created or kept in step with the scene
+  if (!vsm_.updated) return OXC_E_STATE;
+  const OxrVsmPages& v = vsm_.pages;
+  int rc;
+  if ((rc = oxc_cull_meshes(shadow_ctx_, &coarse, OXC_CULL_TEST_ALL, stream_)) != OXC_OK) return fail(rc);
+  if ((rc = oxc_cull_meshlets_hpb_dirty_dev(shadow_ctx_, &coarse, vsm_.clipmaps, v.clipmap_dirty_flags, v.clipmap_count, v.hpb, v.page_table_size,
+                                            v.hpb_levels, stream_)) != OXC_OK) return fail(rc);
+  if ((rc = oxc_vsm_draw_pages(shadow_ctx_, &vsm_.shape, &coarse, vsm_.clipmaps, v.clipmap_dirty_flags, v.page_tables, v.physical_atlas,
+                               stream_)) != OXC_OK) return fail(rc);
+  if (cudaStreamSynchronize(static_cast<cudaStream_t>(stream_)) != cudaSuccess) {
+    error_ = cudaGetErrorString(cudaGetLastError());
+    return OXC_E_CUDA;
+  }
+  return OXC_OK;
+}
+
+// the shadow context is an optional part: losing it must not take the camera path down with it
+void RendererInstance::drop_shadow_context() {
+  cudaStreamSynchronize(static_cast<cudaStream_t>(stream_));
+  oxc_destroy(shadow_ctx_);
+  shadow_ctx_ = nullptr;
 }
 
 auto RendererInstance::virtual_shadow_pages(OxrVsmPages* out) const -> int {
@@ -282,7 +320,9 @@ auto RendererInstance::set_materials(const OxcMaterialTable* table) -> int {
   if (!ctx_) return OXC_E_STATE;
   error_.clear();
   drop_graphs(); // the raster's launch sequence depends on whether a table is set
-  return fail(oxc_set_materials(ctx_, table, stream_));
+  int rc = oxc_set_materials(ctx_, table, stream_);
+  if (rc == OXC_OK && shadow_ctx_ && oxc_set_materials(shadow_ctx_, table, stream_) != OXC_OK) drop_shadow_context(); // the shadow alpha test
+  return fail(rc);
 }
 
 auto RendererInstance::set_external_depth(const float* depth_host) -> int {
@@ -714,6 +754,11 @@ int oxr_vsm_update_pages(OxrRenderer* r, const OxrVsmPageContext* context) {
 int oxr_vsm_pages(OxrRenderer* r, OxrVsmPages* out) {
   if (!r) return OXC_E_INVALID;
   return r->impl.virtual_shadow_pages(out);
+}
+
+int oxr_vsm_draw_shadows(OxrRenderer* r, const OxcCullCamera* coarse) {
+  if (!r || !coarse) return OXC_E_INVALID;
+  return r->impl.draw_virtual_shadows(*coarse);
 }
 
 int oxr_render(OxrRenderer* r, const OxcCullCamera* camera, const float* occluder_depth_host, uint32_t* vis32_host,

@@ -71,6 +71,10 @@ public:
   // draw_virtual_shadowmap's page loop (Shadowmaps.cpp:100-430) up to the shadow raster, from the depth of the last frame
   auto update_virtual_shadow_pages(VsmPageContext& context) -> int;
   auto virtual_shadow_pages(OxrVsmPages* out) const -> int;
+  // draw_virtual_shadowmap's last step (Shadowmaps.cpp:433-754): cull_geometry with use_hpb for the coarse camera, then the shadow
+  // casters into the dirty pages of the atlas, from the clipmaps, flags and table of the last update_virtual_shadow_pages.  Runs on
+  // a context of its own, so the camera frame's survivors, counters and mask are never touched.
+  auto draw_virtual_shadows(const OxcCullCamera& coarse) -> int;
 
   // RendererInstance::render geometry section: run_geometry_pass(false) -> generate_hiz -> run_geometry_pass(true)
   auto render(const OxcCullCamera& camera, const float* occluder_depth_host, uint32_t* vis32_host, float* depth_host,
@@ -149,7 +153,12 @@ private:
     OxcVsmContext shape{};
     uint32_t* d_dirty_instances = nullptr;
     uint32_t dirty_capacity = 0;
+    bool updated = false;                // update_virtual_shadow_pages has run with this shape
+    OxcVirtualClipmap clipmaps[10] = {}; // of the last update
   } vsm_;
+  // the shadow draw's own context (same scene, transforms and materials as ctx_; max_views >= 10 for the clipmap cull)
+  OxcContext* shadow_ctx_ = nullptr;
+  void drop_shadow_context();
   int vsm_allocate(const OxcVsmContext& vsm, uint32_t hpb_levels);
   void vsm_release();
   void* h_pinned_ = nullptr; // staging for small readbacks

@@ -86,6 +86,41 @@ OXC_DI int tri_setup(const ScreenVert v0, const ScreenVert v1, const ScreenVert 
   return TRI_DRAW;
 }
 
+// tri_setup for a raster that draws both windings (the VSM shadow draw, cullMode None): area2 < 0 is set up exactly as tri_setup;
+// area2 > 0 keeps the submitted order (a, b, c = vertices 0, 1, 2) instead of being rejected; area2 == 0 draws nothing.
+// kept_order = the area2 > 0 case (the caller's per-vertex attributes follow the same order).
+OXC_DI int tri_setup_two_sided(const ScreenVert v0, const ScreenVert v1, const ScreenVert v2, uint32_t W, uint32_t H, TriSetup& s,
+                               bool& kept_order) {
+  if (v0.fx == INT_MIN || v1.fx == INT_MIN || v2.fx == INT_MIN) return TRI_INVALID_VERTEX;
+  const int minx = min(v0.fx, min(v1.fx, v2.fx)), maxx = max(v0.fx, max(v1.fx, v2.fx));
+  const int miny = min(v0.fy, min(v1.fy, v2.fy)), maxy = max(v0.fy, max(v1.fy, v2.fy));
+  s.px0 = max(0, (minx - 128 + 255) >> 8);
+  s.px1 = min((int)W - 1, (maxx - 128) >> 8);
+  s.py0 = max(0, (miny - 128 + 255) >> 8);
+  s.py1 = min((int)H - 1, (maxy - 128) >> 8);
+  if (s.px1 < s.px0 || s.py1 < s.py0) return TRI_NO_SAMPLE;
+  s.narrow = (maxx - minx) < 16384 && (maxy - miny) < 16384;
+  const long long area2 = orient2d(v0.fx, v0.fy, v1.fx, v1.fy, v2.fx, v2.fy);
+  if (area2 == 0) return TRI_BACK_OR_DEGENERATE;
+  kept_order = area2 > 0;
+  const ScreenVert b = kept_order ? v1 : v2, c = kept_order ? v2 : v1;
+  s.ax = v0.fx; s.ay = v0.fy; s.bx = b.fx; s.by = b.fy; s.cx = c.fx; s.cy = c.fy;
+  const float fa_ = (float)(kept_order ? area2 : -area2);
+  s.za = v0.z;
+  s.dzb = fd(fs(b.z, v0.z), fa_);
+  s.dzc = fd(fs(c.z, v0.z), fa_);
+  s.bias = edge_bias_bit(s.bx, s.by, s.cx, s.cy) | (edge_bias_bit(s.cx, s.cy, s.ax, s.ay) << 1) |
+           (edge_bias_bit(s.ax, s.ay, s.bx, s.by) << 2);
+  return TRI_DRAW;
+}
+
+// coverage (step 5) and depth (step 6) of one sample given its three edge-function values: false = not covered or z outside [0, 1]
+OXC_DI bool sample_depth(const TriSetup& s, long long e0, long long e1, long long e2, float& z) {
+  if ((e0 - (s.bias & 1)) < 0 || (e1 - ((s.bias >> 1) & 1)) < 0 || (e2 - ((s.bias >> 2) & 1)) < 0) return false;
+  z = fa(fa(s.za, fm((float)e1, s.dzb)), fm((float)e2, s.dzc));
+  return z >= 0.0f && z <= 1.0f;
+}
+
 // steps 5-6 given the three edge-function values at the pixel centre
 OXC_DI void shade_pixel(const TriSetup& s, long long e0, long long e1, long long e2, int px, int py, uint32_t data,
                         unsigned long long* vis, uint32_t W) {

@@ -22,6 +22,7 @@
 #include "kernels_tri.cuh"
 #include "kernels_alpha.cuh"
 #include "kernels_vsm.cuh"
+#include "kernels_vsm_draw.cuh"
 
 using namespace oxc;
 
@@ -179,6 +180,13 @@ struct OxcContext {
   bool alpha_active = false;           // at least one material has an albedo image
   uint32_t* d_alpha_lists = nullptr;   // [2][max_meshlet_instances]: opaque, alpha-tested
   uint8_t* d_alpha_cmd = nullptr;      // 64 B: opaque cmd @0, alpha-tested cmd @16, an all-zero visibility record @32
+  // VSM shadow draw (oxc_vsm_draw_pages): page bitmap, first pixel per page, work queue, counters; allocated by the first call
+  uint32_t* d_vsm_bitmap = nullptr;
+  int* d_vsm_first_px = nullptr;
+  uint4* d_vsm_queue = nullptr;
+  uint32_t* d_vsm_counters = nullptr;
+  size_t vsm_bitmap_words = 0, vsm_first_px_cap = 0;
+  uint32_t vsm_queue_capacity = VSM_DRAW_QUEUE; // work items; beyond it the lane that finds an item draws it
 };
 
 namespace {
@@ -337,6 +345,10 @@ int oxc_create(int device, const OxcCreateInfo* info, OxcContext** out_ctx) {
     if (v >= 1 && v <= (1l << 24)) c->clip_capacity = (uint32_t)v;
   }
   TRY(dalloc(&c->d_clip_queue, (size_t)c->clip_capacity));
+  if (const char* e = getenv("OXC_VSM_DRAW_CAPACITY")) { // test hook: force the VSM draw's inline path
+    const long v = atol(e);
+    if (v >= 1 && v <= (1l << 24)) c->vsm_queue_capacity = (uint32_t)v;
+  }
   c->d_clip_counter = c->d_raster_work + 3;
   TRY(dalloc(&c->d_id_base_auto, 1));
   TRY(dalloc(&c->d_status, 1));
@@ -408,6 +420,7 @@ void oxc_destroy(OxcContext* c) {
   cudaFree(c->d_reordered); cudaFree(c->d_tri_counter); cudaFree(c->d_raster_work); cudaFree(c->d_big_queue); cudaFree(c->d_clip_queue); cudaFree(c->d_id_base_auto); cudaFree(c->d_status); cudaFree(c->d_hiz);
   cudaFree(c->d_view_planes); cudaFree(c->d_view_bits); cudaFree(c->d_view_counts); cudaFree(c->d_inst_views);
   cudaFree(c->d_alpha_materials); cudaFree(c->d_alpha_lists); cudaFree(c->d_alpha_cmd);
+  cudaFree(c->d_vsm_bitmap); cudaFree(c->d_vsm_first_px); cudaFree(c->d_vsm_queue); cudaFree(c->d_vsm_counters);
   delete c;
 }
 
@@ -1326,6 +1339,71 @@ int oxc_vsm_clear_dirty_pages(OxcContext* c, const OxcVsmContext* vsm, const Oxc
   const uint32_t grid = std::min<uint32_t>((uint32_t)c->sm_count * 8u, pages ? pages : 1u);
   k_vsm_clear_dirty_pages<<<grid, 256, 0, s>>>(p);
   LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_vsm_draw_pages(OxcContext* c, const OxcVsmContext* vsm, const OxcCullCamera* coarse, const OxcVirtualClipmap* clipmaps,
+                       const uint32_t* clipmap_dirty_flags_dev, const uint32_t* page_tables_dev, float* physical_atlas_dev, void* stream) {
+  if (!c || !vsm || !coarse || !clipmaps || !clipmap_dirty_flags_dev || !page_tables_dev || !physical_atlas_dev) return fail(OXC_E_INVALID, "null argument");
+  int rc = check_vsm(vsm, 0xFFFFFFFFu);
+  if (rc != OXC_OK) return rc;
+  if (vsm->physical_page_table_size > VSM_DRAW_MAX_EXTENT)
+    return fail(OXC_E_INVALID, "physical_page_table_size %d > %d: pixel centres beyond the raster's 2^22 sub-pixel snap range", vsm->physical_page_table_size,
+                VSM_DRAW_MAX_EXTENT);
+  if (!c->scene_set) return fail(OXC_E_STATE, "oxc_set_scene first");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  rc = refresh_inst_cache(c, coarse, s, false); // the coarse camera's PV . W for the triangle test, from the argument
+  if (rc != OXC_OK) return rc;
+  const int size = vsm->page_table_size, wpr = (size + 31) / 32;
+  const size_t words = (size_t)vsm->clipmap_count * size * wpr;
+  if (words > c->vsm_bitmap_words) {
+    cudaFree(c->d_vsm_bitmap);
+    c->vsm_bitmap_words = 0;
+    if (dalloc(&c->d_vsm_bitmap, words) != OXC_OK) return OXC_E_CUDA;
+    c->vsm_bitmap_words = words;
+  }
+  if ((size_t)size + 1 > c->vsm_first_px_cap) {
+    cudaFree(c->d_vsm_first_px);
+    c->vsm_first_px_cap = 0;
+    if (dalloc(&c->d_vsm_first_px, (size_t)size + 1) != OXC_OK) return OXC_E_CUDA;
+    c->vsm_first_px_cap = (size_t)size + 1;
+  }
+  if (!c->d_vsm_queue) {
+    if (dalloc(&c->d_vsm_queue, (size_t)c->vsm_queue_capacity) != OXC_OK || dalloc(&c->d_vsm_counters, (size_t)4) != OXC_OK) return OXC_E_CUDA;
+    CK(cudaMemsetAsync(c->d_vsm_counters, 0, 16, s));
+  }
+  VsmDrawParams p{};
+  p.meshlet_instances = c->d_meshlet_instances; p.inst = c->d_inst; p.geom = c->d_geom; p.mesh_instances = c->d_mesh_instances;
+  p.transforms = c->d_transforms; p.visible_indices = c->d_visible; p.tri_cmd = c->d_cull_triangles_cmd; p.id_base = c->id_base;
+  if (c->alpha_active) { p.materials = c->d_alpha_materials; p.material_count = c->alpha_material_count; }
+  for (int k = 0; k < vsm->clipmap_count; k++) {
+    const float* m = clipmaps[k].projection_view_mat;
+    for (int i = 0; i < 4; i++) p.pv_row[k][i] = make_float4(m[i], m[4 + i], m[8 + i], m[12 + i]);
+    p.page_offset[k][0] = clipmaps[k].page_offset[0]; p.page_offset[k][1] = clipmaps[k].page_offset[1];
+  }
+  p.dirty_flags = clipmap_dirty_flags_dev; p.page_tables = page_tables_dev; p.atlas = reinterpret_cast<uint32_t*>(physical_atlas_dev);
+  p.bitmap = c->d_vsm_bitmap; p.first_px = c->d_vsm_first_px; p.queue = c->d_vsm_queue; p.counters = c->d_vsm_counters;
+  p.queue_capacity = c->vsm_queue_capacity;
+  p.size = size; p.page_size = vsm->page_size; p.P = vsm->physical_page_table_size; p.phys_per_row = vsm->physical_page_table_size / vsm->page_size;
+  p.clipmap_count = vsm->clipmap_count; p.words_per_row = wpr;
+  p.fP = (float)p.P; p.fsize = (float)size; p.fpage = (float)vsm->page_size;
+  k_vsm_draw_prepare<<<1, 1024, 0, s>>>(p);
+  LAUNCHED();
+  k_vsm_draw_meshlets<<<persistent_grid(c, VSM_DRAW_WARPS, 8), VSM_DRAW_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  k_vsm_draw_items<<<(uint32_t)c->sm_count * 8u, VSM_DRAW_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_vsm_draw_stats(OxcContext* c, uint32_t out[2], void* stream) {
+  if (!c || !out) return fail(OXC_E_INVALID, "null argument");
+  if (!c->d_vsm_counters) return fail(OXC_E_STATE, "oxc_vsm_draw_pages has not run on this context");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  CK(cudaMemcpyAsync(out, c->d_vsm_counters, 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
   return OXC_OK;
 }
 

@@ -429,6 +429,69 @@ def make_scene(
     return sc
 
 
+def with_ground_caster(scene: Scene, half_size=1200.0, center=(0.0, 0.0, -40.0), grid=32):
+    """`scene` plus one more mesh instance: a tessellated plane y = center.y of 2 * half_size per side, the shadow caster under the
+    other instances.  grid x grid meshlets of 4 x 8 quads (45 vertices, 64 triangles each) over a local [-1, 1]^2 whose vertex
+    coordinates are exact in half precision (multiples of 1 / (8 * grid)); the world matrix scales x and z by half_size."""
+    nx, nz = 4 * grid + 1, 8 * grid + 1
+    gx, gz = np.meshgrid(np.arange(nx) / (2.0 * grid) - 1.0, np.arange(nz) / (4.0 * grid) - 1.0, indexing="ij")
+    pos = np.zeros((nx * nz, 4), dtype=np.uint16)
+    pos[:, 0], pos[:, 2] = quantize_half(gx.reshape(-1).astype(np.float32)), quantize_half(gz.reshape(-1).astype(np.float32))
+    lx, lz = np.meshgrid(np.arange(5), np.arange(9), indexing="ij")
+    local = (lx * 9 + lz).reshape(-1)                    # meshlet-local vertex index of (x, z)
+    q = (np.arange(4)[:, None] * 9 + np.arange(8)[None, :]).reshape(-1)
+    tris = np.stack([np.stack([q, q + 10, q + 9], 1), np.stack([q, q + 1, q + 10], 1)], 1).reshape(-1, 3).astype(np.uint8)
+    mi, mj = np.meshgrid(np.arange(grid), np.arange(grid), indexing="ij")
+    mi, mj = mi.reshape(-1), mj.reshape(-1)
+    n = grid * grid
+    vidx = ((mi[:, None] * 4 + lx.reshape(-1)[None, :]) * nz + mj[:, None] * 8 + lz.reshape(-1)[None, :]).astype(np.uint32)
+    assert (local == np.arange(45)).all()
+    meshlets = np.zeros(n, dtype=abi.MESHLET_DT)
+    meshlets["indirect_vertex_index_offset"] = np.arange(n) * 45
+    meshlets["local_triangle_index_offset"] = np.arange(n) * 192
+    meshlets["vertex_count"], meshlets["triangle_count"] = 45, 64
+    bounds = np.zeros(n, dtype=abi.MESHLET_BOUNDS_DT)
+    cx, cz = (mi * 2 + 1) / grid - 1.0, (mj * 2 + 1) / grid - 1.0
+    bounds["aabb_center"] = quantize_half(np.stack([cx, np.zeros(n), cz], 1).astype(np.float32))
+    bounds["aabb_extent"] = quantize_half(np.tile(np.float32([2.0 / grid, 1.0 / 64, 2.0 / grid]), (n, 1)))
+    bounds["cone_cutoff"] = 127  # no cone: a plane is seen from both sides
+    chunks, off = [], _align(int(scene.blob.size), 16)
+
+    def put(a):
+        nonlocal off
+        start = off
+        raw = np.ascontiguousarray(a).view(np.uint8).reshape(-1)
+        pad = (-raw.size) % 16
+        chunks.append(np.concatenate([raw, np.zeros(pad, dtype=np.uint8)]))
+        off += raw.size + pad
+        return start
+
+    mesh = np.zeros(1, dtype=abi.MESH_DT)
+    mesh["vertex_positions"] = put(pos)
+    mesh["vertex_count"], mesh["lod_count"] = nx * nz, 1
+    lod = np.zeros(1, dtype=abi.MESH_LOD_DT)
+    lod["meshlets"], lod["meshlet_bounds"] = put(meshlets), put(bounds)
+    lod["local_triangle_indices"], lod["indirect_vertex_indices"] = put(np.tile(tris.reshape(-1), n)), put(vidx.reshape(-1))
+    lod["meshlet_count"] = lod["meshlet_bounds_count"] = n
+    lod["local_triangle_indices_count"], lod["indirect_vertex_indices_count"] = n * 192, n * 45
+    mesh["lods"] = put(lod)
+    mesh["bounds"]["aabb_center"][0] = (0.0, 0.0, 0.0)
+    mesh["bounds"]["aabb_extent"][0] = (2.0, 1.0 / 64, 2.0)
+    head = np.concatenate([scene.blob, np.zeros(_align(int(scene.blob.size), 16) - scene.blob.size, dtype=np.uint8)])
+    blob = np.concatenate([head] + chunks)
+    xf = np.zeros(1, dtype=abi.TRANSFORM_DT)
+    w = np.diag([half_size, 1.0, half_size, 1.0]).astype(np.float32)
+    w[3, :3] = center  # [col][row]: column 3 = translation
+    xf["world"][0] = w.reshape(16)
+    inst = np.zeros(1, dtype=abi.MESH_INSTANCE_DT)
+    inst["mesh_index"], inst["transform_index"] = len(scene.meshes), len(scene.transforms)
+    inst["meshlet_instance_visibility_offset"] = scene.max_meshlet_instance_count
+    sc = Scene(np.concatenate([scene.meshes, mesh]), np.concatenate([scene.mesh_instances, inst]), np.concatenate([scene.transforms, xf]),
+               blob, scene.max_meshlet_instance_count + n, scene.width, scene.height, scene.seed, scene.occluder_depth, dict(scene.info))
+    sc.info["ground_caster"] = dict(half_size=half_size, center=tuple(center), meshlets=n, triangles=n * 64)
+    return sc
+
+
 def make_occluder_depth(seed, width, height, n_occluders=32, near=0.1, far=1000.0):
     """Depth (reverse-Z) of n screen-space occluder rectangles at seeded view distances — the stand-in
     for depth laid down by passes outside this path.  0 = nothing (far)."""
