@@ -304,6 +304,28 @@ __global__ void __launch_bounds__(256) k_raster_big(const __grid_constant__ TriP
   }
 }
 
+#if defined(OXC_RASTER_STATS) && OXC_RASTER_STATS == 1
+// Statistics build only. Warp-wide, over every lane's v0 (when has0) and v1 (when has1): true when the snapped pixel box of the
+// vertices, clamped to the image as tri_setup clamps a triangle's, holds no sample centre and no vertex is invalid.  Every
+// triangle's corners are meshlet vertices and snap and clamp are monotone, so every triangle of such a meshlet is TRI_NO_SAMPLE.
+// The coordinates are reduced as unsigned with the sign bit flipped, which orders them as signed ints.
+OXC_DI bool meshlet_covers_no_sample(const ScreenVert& v0, const ScreenVert& v1, bool has0, bool has1, uint32_t W, uint32_t H) {
+  constexpr int FAR = 1 << 30; // identity: beyond the snap range (|fx|, |fy| <= 2^22), and the snap below cannot overflow on it
+  constexpr uint32_t SIGN = 0x80000000u;
+  const bool ok0 = has0 && v0.fx != INT_MIN, ok1 = has1 && v1.fx != INT_MIN;
+  const int lx = min(ok0 ? v0.fx : FAR, ok1 ? v1.fx : FAR), hx = max(ok0 ? v0.fx : -FAR, ok1 ? v1.fx : -FAR);
+  const int ly = min(ok0 ? v0.fy : FAR, ok1 ? v1.fy : FAR), hy = max(ok0 ? v0.fy : -FAR, ok1 ? v1.fy : -FAR);
+  const int minx = (int)(__reduce_min_sync(0xffffffffu, (uint32_t)lx ^ SIGN) ^ SIGN);
+  const int maxx = (int)(__reduce_max_sync(0xffffffffu, (uint32_t)hx ^ SIGN) ^ SIGN);
+  const int miny = (int)(__reduce_min_sync(0xffffffffu, (uint32_t)ly ^ SIGN) ^ SIGN);
+  const int maxy = (int)(__reduce_max_sync(0xffffffffu, (uint32_t)hy ^ SIGN) ^ SIGN);
+  const int px0 = max(0, (minx - 128 + 255) >> 8), px1 = min((int)W - 1, (maxx - 128) >> 8);
+  const int py0 = max(0, (miny - 128 + 255) >> 8), py1 = min((int)H - 1, (maxy - 128) >> 8);
+  const bool any_invalid = __any_sync(0xffffffffu, (has0 && !ok0) || (has1 && !ok1));
+  return (px1 < px0 || py1 < py0) && !any_invalid;
+}
+#endif
+
 template <bool PREFETCH_GRAB>
 __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_visbuffer(const __grid_constant__ TriParams p) {
   __shared__ float4 clip_all[TRI_WARPS][OXC_MESHLET_MAX_VERTICES];
@@ -325,12 +347,15 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
 #endif
   // warps pull batches of up to RASTER_BATCH consecutive survivors from a global work counter (dynamic balance); lanes
   // 0..nb-1 each chase one meshlet header, so nb pointer chases are in flight together.
-  // Guided self-scheduling: the grab size shrinks with the work that is left (remaining / (2 x warps in the grid), between 1
-  // and RASTER_BATCH), so the kernel ends with single-meshlet grabs.
+  // Guided self-scheduling: the grab size shrinks with the work that is left (remaining / (k x warps in the grid), between 1
+  // and RASTER_BATCH), so the kernel ends with single-meshlet grabs.  The early pass divides by the warps (k = 1): its grabs
+  // stay at 32 meshlets until 38 % of the list is left instead of 77 % (1 M meshlet instances / 1080p), and each grab costs a
+  // header chase.  On H100 SXM that takes the early raster from 355-357 to 325-328 us (BASELINE.md 5.8).  The late
+  // pass, which holds a prefetched grab in reserve, keeps k = 2: at k = 1 it took 81 instead of 69 us.
   // A grab is slow (thousands of warps on one L2 atomic address; tools/raster_stats.py times it per warp).  Dealing the list
   // onto 32 interleaved sequences with one counter each would shorten the late pass, but the extra scheduler state is more
   // live registers in a kernel that already spills at its bound, so the single counter stays (not re-timed on H100).
-  const uint32_t n_warps2 = gridDim.x * TRI_WARPS * 2u;
+  const uint32_t grab_divisor = gridDim.x * TRI_WARPS * (PREFETCH_GRAB ? 2u : 1u);
   // PREFETCH_GRAB (late pass): the grab for the NEXT batch is issued before the current batch is processed, so the atomic's
   // round trip (long in the late pass: every warp of the GPU on one address, few meshlets per warp) overlaps a batch of
   // rasterisation.  The early pass (many meshlets per warp, few grabs) loses more balance from the batch each warp holds in
@@ -338,7 +363,7 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
   // issue.
   uint32_t g_next = 0, batch_next = 1;
   if (PREFETCH_GRAB && lane == 0) {
-    batch_next = min((uint32_t)RASTER_BATCH, max(1u, count / n_warps2));
+    batch_next = min((uint32_t)RASTER_BATCH, max(1u, count / grab_divisor));
     g_next = atomicAdd(p.work_counter, batch_next);
   }
   for (;;) {
@@ -350,14 +375,14 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
       if (lane == 0) { // reserve the following batch now; its index is not needed before the next iteration
         const uint32_t seen = g0 + batch; // what had been handed out when this batch was reserved (a lower bound now)
         const uint32_t rem = count > seen ? count - seen : 0u;
-        batch_next = min((uint32_t)RASTER_BATCH, max(1u, rem / n_warps2));
+        batch_next = min((uint32_t)RASTER_BATCH, max(1u, rem / grab_divisor));
         g_next = atomicAdd(p.work_counter, batch_next);
       }
     } else {
       if (lane == 0) {
         const uint32_t seen = *reinterpret_cast<volatile uint32_t*>(p.work_counter); // heuristic only: a stale value is harmless
         const uint32_t rem = count > seen ? count - seen : 0u;
-        batch = min((uint32_t)RASTER_BATCH, max(1u, rem / n_warps2));
+        batch = min((uint32_t)RASTER_BATCH, max(1u, rem / grab_divisor));
         g0 = atomicAdd(p.work_counter, batch);
       }
       g0 = __shfl_sync(0xffffffffu, g0, 0);
@@ -420,6 +445,10 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
       const uint32_t rounds = (w.tri_count + 31u) >> 5;
 #if defined(OXC_RASTER_STATS) && OXC_RASTER_STATS == 1
       bool meshlet_draws = false;
+      // meshlets that a per-meshlet footprint test could settle without any triangle set-up
+      if (meshlet_covers_no_sample(scr_s[lane], scr_s[lane + 32], lane < w.vertex_count, lane + 32u < w.vertex_count, p.width, p.height) &&
+          lane == 0)
+        atomicAdd(reinterpret_cast<unsigned long long*>(p.big_queue) + (size_t)p.big_capacity * 8 + (p.late ? 64 : 0) + 48, 1ull);
 #endif
       for (uint32_t k = 0; k < rounds; k++) {
         const uint32_t t = lane + 32u * k;

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Instrumentation run (variant library built with -DOXC_RASTER_STATS): per round of 32 triangles, how long is the longest
-per-lane pixel loop, how many rounds run the triangle set-up, and how many meshlets draw anything?  Usage:  OXC_LIB_PATH=$PWD/oxylus_b200/liboxcull_stats.so python tools/raster_stats.py"""
+per-lane pixel loop, how many rounds run the triangle set-up, how many meshlets draw anything, and how many could be settled
+once per meshlet (footprint box without a sample centre, no invalid vertex)?  Usage:  OXC_LIB_PATH=$PWD/oxylus_b200/liboxcull_stats.so python tools/raster_stats.py"""
 import os
 import sys
 
@@ -31,6 +32,7 @@ for name, o in (("early", 0), ("late", 64)):
           f"mean max-lane px {st[o + 41] / max(1, rounds):.2f}  drawing lanes/round {st[o + 42] / max(1, rounds):.2f}  "
           f"deferred big tris/frame {st[o + 44] / frames:.0f}")
     print(f"   meshlets with a drawing triangle/frame {st[o + 46] / frames:.0f}  set-up rounds/frame {st[o + 47] / frames:.0f}")
+    print(f"   meshlets whose footprint holds no sample centre and that have no invalid vertex/frame {st[o + 48] / frames:.0f}")
     print("   histogram of max per-lane bbox area per round (0..32, 33+):")
     print("   " + " ".join(f"{int(x / frames)}" for x in h))
     cost_serial = float((h * np.arange(34)).sum())
