@@ -721,6 +721,33 @@ int oxc_vsm_draw_pages(OxcContext* ctx, const OxcVsmContext* vsm, const OxcCullC
  * out[1] = (meshlet, clipmap) pairs whose page rectangle held a dirty page and so reached triangle work. */
 int oxc_vsm_draw_stats(OxcContext* ctx, uint32_t out[2], void* stream);
 
+/* The VSM shadow resolve: RendererInstance::resolve_shadowmap (Shadowmaps.cpp:756-822, passes/resolve_shadowmaps.slang:27-209 with
+ * the rmvsm.slang helpers it calls), the consumer of the physical atlas.  One value per pixel of the depth_extent[0] x
+ * depth_extent[1] image into shadow_dev (R32F, row-major): 1 = lit, 0 = shadowed, the PCF fraction in between.  Inputs are only
+ * read: depth_dev (D32F, 0 = sky), normals_dev (float4 per pixel, oct(world normal) in .zw: the uv_normal plane of
+ * oxc_decode_visbuffer, 0 where the decode discards), page_tables_dev [clipmap][size][size], physical_atlas_dev
+ * (physical_page_table_size^2 R32F).  Specification (oracle/oxc_oracle_vsm_resolve.c orc_vsm_resolve_shadows, bit for bit), in
+ * IEEE binary32 with no contraction, IEEE divide / sqrt, dot = (x*x' + y*y') + z*z', mul in row order:
+ *   - pixel (x, y): position = (x + 0.5, y + 0.5), tex_coord = position / depth_extent; depth == 0 gives 1;
+ *   - normal: both .zw components rounded to binary16 (round to nearest even; the reference's attachment is R16G16B16A16Sfloat),
+ *     then normalize(oct_to_vec3(e)) (common/encoding.slang:7-15, which normalizes once itself), normalize(v) = v / sqrt(dot(v, v));
+ *   - world point: unproject (scene.slang:189-193); clipmap: exactly oxc_mark_visible_pages' rule (canonical_log2, bias, ceil,
+ *     saturating u32, clamp to clipmap_count - 1);
+ *   - PCSS (:84-185): 1 centre tap, 16 blocker-search taps, up to 24 PCF taps; noise = hash2(position) (:27-30); a tap looks up the
+ *     base clipmap, then base - 1, then base + 1 (indices -1 and clipmap_count miss); a page outside the table or not Backed misses;
+ *     a fetched value equal to -1.0 counts as a miss, as in the shader; pow(2, k + 1) is exact; fract(x) = x - floor(x);
+ *     lerp(a, b, t) = a + (b - a) * t; base_bias = (quantize + b) + term; max / min return the other operand for a NaN;
+ *     accum_depth_world is summed in sample order; hammersley2d(i, N) = (i / N, reversebits(i) * 2^-32);
+ *   - sin / cos: the library's own canonical_sincos (oxc_exact.cuh == oracle orc_sincos_canonical): binary64 reduction by
+ *     pi/2 and Taylor polynomials, one rounding to binary32; <= 1 ulp on [0, 2 pi], <= 2^-24 absolute for |x| <= 2^21.  The
+ *     reference's driver sin / cos under fast-math are not bit-defined.
+ * Deviation: a physical address whose texel lies outside the atlas reads 0.0, what robustImageAccess returns (the draw does not
+ * write such a texel).  No scratch: graph-capturable from the first call.  Same argument checks as the other oxc_vsm_* calls,
+ * plus depth_extent >= 1 and a 16-byte aligned normals_dev. */
+int oxc_vsm_resolve_shadows(OxcContext* ctx, const OxcVsmContext* vsm, const float inv_projection_view[16], const float resolution[2],
+                            const OxcVirtualClipmap* clipmaps /* host */, const float* depth_dev, const float* normals_dev,
+                            const uint32_t* page_tables_dev, const float* physical_atlas_dev, float* shadow_dev, void* stream);
+
 int oxc_get_outputs(OxcContext* ctx, OxcOutputs* out);
 /* Instrumentation hook: 128 u64 counters that builds with -DOXC_RASTER_STATS fill (tools/raster_stats.py); zero otherwise. */
 void* oxc_debug_stats_ptr(OxcContext* ctx);
@@ -825,6 +852,13 @@ int oxr_vsm_pages(OxrRenderer* r, OxrVsmPages* out);
  * oxr_update, so the context cannot be made later from it.  If the context cannot be created or kept in step (out of device memory),
  * the camera path is unaffected and this call returns OXC_E_CAPACITY. */
 int oxr_vsm_draw_shadows(OxrRenderer* r, const OxcCullCamera* coarse);
+/* RendererInstance::resolve_shadowmap (Shadowmaps.cpp:756-822): on the frame oxr_render / oxr_wait completed last, oxc_decode_visbuffer
+ * with `camera` (the camera that frame was rendered with) into a uv_normal plane the renderer allocates at the first call, then
+ * oxc_vsm_resolve_shadows with the shape, clipmaps, inv_projection_view and resolution of the last oxr_vsm_update_pages, the
+ * renderer's atlas and the frame's depth; width x height floats to shadow_host.  Synchronous.  The camera frame's outputs, the page
+ * table and the atlas are left as they were.  OXC_E_STATE before an oxr_vsm_update_pages;
+ * OXC_E_CAPACITY, with the camera path left usable, when the 20 B / pixel of its own planes cannot be allocated. */
+int oxr_vsm_resolve_shadows(OxrRenderer* r, const OxcCullCamera* camera, float* shadow_host);
 
 /* ------------------------------------------------------------------------------------------------
  * oxb_* — mesh builder (SURVEY §8f.2): host-side producer of the blob layout above, mirroring build_gltf_mesh

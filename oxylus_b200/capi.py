@@ -21,13 +21,13 @@ SYMBOLS = [
     "oxc_raster_visbuffer", "oxc_raster_visbuffer_clip_pass", "oxc_set_materials", "oxc_raster_overdraw", "oxc_clear_overdraw", "oxc_resolve_visbuffer", "oxc_merge_depth", "oxc_clear_visbuffer_with_depth", "oxc_cull_meshlets_multiview", "oxc_cull_meshlets_hpb", "oxc_cull_terrain",
     "oxc_decode_visbuffer", "oxc_build_hpb", "oxc_mark_visible_pages",
     "oxc_vsm_begin_frame", "oxc_vsm_invalidate_pages", "oxc_vsm_allocate_pages", "oxc_vsm_clear_dirty_pages", "oxc_cull_meshlets_hpb_dirty_dev",
-    "oxc_vsm_draw_pages", "oxc_vsm_draw_stats",
+    "oxc_vsm_draw_pages", "oxc_vsm_draw_stats", "oxc_vsm_resolve_shadows",
     "oxc_get_outputs", "oxc_check_status", "oxc_mark_hiz_dirty", "oxc_bind_camera_buffer", "oxc_load_camera", "oxc_debug_stats_ptr",
     "oxc_mgpu_get_unique_id", "oxc_mgpu_init", "oxc_mgpu_init_with_comm", "oxc_mgpu_shutdown", "oxc_mgpu_info", "oxc_mgpu_exchange_hiz",
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
     "oxb_last_error", "oxb_build_mesh", "oxb_mesh_blob_size", "oxb_mesh_lod0_meshlet_count", "oxb_mesh_emit", "oxb_mesh_free", "oxb_simplify",
     "oxr_create", "oxr_destroy", "oxr_context", "oxr_update", "oxr_update_transforms", "oxr_set_external_depth", "oxr_set_materials", "oxr_overdraw", "oxr_render", "oxr_submit", "oxr_wait",
-    "oxr_vsm_update_pages", "oxr_vsm_pages", "oxr_vsm_draw_shadows",
+    "oxr_vsm_update_pages", "oxr_vsm_pages", "oxr_vsm_draw_shadows", "oxr_vsm_resolve_shadows",
 ]
 
 
@@ -93,6 +93,7 @@ def load(build_if_missing=True):
     lib.oxc_cull_meshlets_hpb_dirty_dev.argtypes = [vp, vp, vp, vp, u32, vp, u32, u32, vp]
     lib.oxc_vsm_draw_pages.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     lib.oxc_vsm_draw_stats.argtypes = [vp, vp, vp]
+    lib.oxc_vsm_resolve_shadows.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.oxc_get_outputs.argtypes = [vp, C.POINTER(abi.Outputs)]
     lib.oxc_check_status.argtypes = [vp, vp, C.POINTER(C.c_uint32)]
     lib.oxc_mark_hiz_dirty.argtypes = [vp]
@@ -140,6 +141,7 @@ def load(build_if_missing=True):
     lib.oxr_vsm_update_pages.argtypes = [vp, C.POINTER(abi.VsmPageContext)]
     lib.oxr_vsm_pages.argtypes = [vp, C.POINTER(abi.VsmPages)]
     lib.oxr_vsm_draw_shadows.argtypes = [vp, vp]
+    lib.oxr_vsm_resolve_shadows.argtypes = [vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -463,6 +465,14 @@ class Context:
         _check(self.lib.oxc_vsm_draw_stats(self.h, _ptr(out), self.stream), "oxc_vsm_draw_stats")
         return dict(items=int(out[0]), pairs=int(out[1]))
 
+    def vsm_resolve_shadows(self, vsm, inv_pv, resolution, clipmaps, depth_dev, normals_dev, page_tables_dev, atlas_dev, shadow_dev):
+        """oxc_vsm_resolve_shadows: the PCSS shadow factor per pixel of vsm's depth_extent into shadow_dev (device pointers; normals_dev:
+        float4 per pixel, oct(world normal) in .zw)"""
+        vc, cm = np.ascontiguousarray(vsm), np.ascontiguousarray(clipmaps)
+        ipv, res = np.ascontiguousarray(inv_pv, dtype=np.float32), np.ascontiguousarray(resolution, dtype=np.float32)
+        _check(self.lib.oxc_vsm_resolve_shadows(self.h, _ptr(vc), _ptr(ipv), _ptr(res), _ptr(cm), _ptr(depth_dev), _ptr(normals_dev),
+                                                _ptr(page_tables_dev), _ptr(atlas_dev), _ptr(shadow_dev), self.stream), "oxc_vsm_resolve_shadows")
+
     def build_hpb(self, page_table_dev, size, layers, hpb_dev, levels):
         _check(self.lib.oxc_build_hpb(self.h, _ptr(page_table_dev), size, layers, _ptr(hpb_dev), levels, self.stream), "oxc_build_hpb")
 
@@ -696,6 +706,13 @@ class Renderer:
         """oxr_vsm_draw_shadows: the shadow casters of the last vsm_update_pages drawn into the renderer's atlas (coarse: the
         clipmap-9 camera, Shadowmaps.cpp:433-463)"""
         _check(self.lib.oxr_vsm_draw_shadows(self.h, _ptr(coarse)), "oxr_vsm_draw_shadows")
+
+    def vsm_resolve_shadows(self, cam):
+        """oxr_vsm_resolve_shadows: the shadow factor (float32 [height, width]) of the frame rendered last with `cam`, from the pages,
+        clipmaps and atlas of the last vsm_update_pages / vsm_draw_shadows"""
+        out = np.zeros((self.scene.height, self.scene.width), dtype=np.float32)
+        _check(self.lib.oxr_vsm_resolve_shadows(self.h, _ptr(cam), _ptr(out)), "oxr_vsm_resolve_shadows")
+        return out
 
     def vsm_pages(self):
         """oxr_vsm_pages: abi.VsmPages of device pointers and sizes"""

@@ -162,7 +162,7 @@ void RendererInstance::vsm_release() {
   OxrVsmPages& v = vsm_.pages;
   cudaFree(v.page_tables); cudaFree(v.hpb); cudaFree(v.page_occupancy); cudaFree(v.requests); cudaFree(v.allocator);
   cudaFree(v.free_page_list); cudaFree(v.dirty_physical_page_coords); cudaFree(v.clipmap_dirty_flags); cudaFree(v.physical_atlas);
-  cudaFree(vsm_.d_dirty_instances);
+  cudaFree(vsm_.d_dirty_instances); cudaFree(vsm_.d_normals); cudaFree(vsm_.d_shadow);
   vsm_ = Vsm();
 }
 
@@ -258,6 +258,8 @@ auto RendererInstance::update_virtual_shadow_pages(VsmPageContext& context) -> i
     return OXC_E_CUDA;
   }
   std::memcpy(vsm_.clipmaps, context.clipmaps, sizeof vsm_.clipmaps);
+  std::memcpy(vsm_.inv_projection_view, context.inv_projection_view, sizeof vsm_.inv_projection_view);
+  std::memcpy(vsm_.resolution, context.resolution, sizeof vsm_.resolution);
   vsm_.updated = true;
   return OXC_OK;
 }
@@ -279,6 +281,36 @@ auto RendererInstance::draw_virtual_shadows(const OxcCullCamera& coarse) -> int 
     error_ = cudaGetErrorString(cudaGetLastError());
     return OXC_E_CUDA;
   }
+  return OXC_OK;
+}
+
+// Shadowmaps.cpp:756-822 resolve_shadowmap on stream_, synchronous: the vis decode's normals of the last frame (the reference's
+// normal_attachment), its depth, then the fullscreen resolve with the VSM state of the last update
+auto RendererInstance::resolve_shadowmap(const OxcCullCamera& camera, float* shadow_host) -> int {
+  if (!ctx_ || !error_.empty()) return OXC_E_STATE;
+  if (!shadow_host) return OXC_E_INVALID;
+  if (!vsm_.updated) return OXC_E_STATE;
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  const size_t px = (size_t)width_ * height_;
+  // the resolve's own planes are an optional part, as the shadow draw's context is: without room for them the camera path stays
+  // usable and this call returns OXC_E_CAPACITY (the sticky error is not set)
+  if (!vsm_.d_normals && (cudaMalloc(reinterpret_cast<void**>(&vsm_.d_normals), px * 16) != cudaSuccess ||
+                          cudaMalloc(reinterpret_cast<void**>(&vsm_.d_shadow), px * 4) != cudaSuccess)) {
+    cudaGetLastError(); // clear the allocation error so that the next launch check does not report it
+    cudaFree(vsm_.d_normals); vsm_.d_normals = nullptr;
+    return OXC_E_CAPACITY;
+  }
+  const OxrVsmPages& v = vsm_.pages;
+  int rc;
+  if ((rc = oxc_bind_camera_buffer(ctx_, nullptr)) != OXC_OK) return fail(rc); // as render(): the camera comes from the argument
+  OxcDecodeTargets targets{};
+  targets.uv_normal = vsm_.d_normals;
+  if ((rc = oxc_decode_visbuffer(ctx_, &camera, d_vis64_, nullptr, width_, height_, &targets, stream_)) != OXC_OK) return fail(rc);
+  if ((rc = oxc_resolve_visbuffer(ctx_, d_vis64_, width_, height_, nullptr, d_depth_, stream_)) != OXC_OK) return fail(rc);
+  if ((rc = oxc_vsm_resolve_shadows(ctx_, &vsm_.shape, vsm_.inv_projection_view, vsm_.resolution, vsm_.clipmaps, d_depth_, vsm_.d_normals,
+                                    v.page_tables, v.physical_atlas, vsm_.d_shadow, stream_)) != OXC_OK) return fail(rc);
+  if (cudaMemcpyAsync(shadow_host, vsm_.d_shadow, px * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
+    return fail(OXC_E_CUDA);
   return OXC_OK;
 }
 
@@ -759,6 +791,11 @@ int oxr_vsm_pages(OxrRenderer* r, OxrVsmPages* out) {
 int oxr_vsm_draw_shadows(OxrRenderer* r, const OxcCullCamera* coarse) {
   if (!r || !coarse) return OXC_E_INVALID;
   return r->impl.draw_virtual_shadows(*coarse);
+}
+
+int oxr_vsm_resolve_shadows(OxrRenderer* r, const OxcCullCamera* camera, float* shadow_host) {
+  if (!r || !camera) return OXC_E_INVALID;
+  return r->impl.resolve_shadowmap(*camera, shadow_host);
 }
 
 int oxr_render(OxrRenderer* r, const OxcCullCamera* camera, const float* occluder_depth_host, uint32_t* vis32_host,

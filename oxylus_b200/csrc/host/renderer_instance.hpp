@@ -75,6 +75,9 @@ public:
   // casters into the dirty pages of the atlas, from the clipmaps, flags and table of the last update_virtual_shadow_pages.  Runs on
   // a context of its own, so the camera frame's survivors, counters and mask are never touched.
   auto draw_virtual_shadows(const OxcCullCamera& coarse) -> int;
+  // resolve_shadowmap (Shadowmaps.cpp:756-822): decode the last frame's normals, then the PCSS shadow factor per pixel from the pages,
+  // clipmaps and atlas of the last update_virtual_shadow_pages; width x height floats to the host
+  auto resolve_shadowmap(const OxcCullCamera& camera, float* shadow_host) -> int;
 
   // RendererInstance::render geometry section: run_geometry_pass(false) -> generate_hiz -> run_geometry_pass(true)
   auto render(const OxcCullCamera& camera, const float* occluder_depth_host, uint32_t* vis32_host, float* depth_host,
@@ -155,6 +158,10 @@ private:
     uint32_t dirty_capacity = 0;
     bool updated = false;                // update_virtual_shadow_pages has run with this shape
     OxcVirtualClipmap clipmaps[10] = {}; // of the last update
+    float inv_projection_view[16] = {};  // of the last update
+    float resolution[2] = {};
+    float* d_normals = nullptr;          // uv_normal plane of the resolve's decode (float4 per pixel), allocated by its first call
+    float* d_shadow = nullptr;           // the resolve's output
   } vsm_;
   // the shadow draw's own context (same scene, transforms and materials as ctx_; max_views >= 10 for the clipmap cull)
   OxcContext* shadow_ctx_ = nullptr;

@@ -7,6 +7,7 @@
 // Arithmetic is the canonical binary32 order of oracle/oxc_oracle.c::orc_decode_visbuffer (bit-exact).
 #pragma once
 #include "oxc_exact.cuh"
+#include "oxc_vsm_resolve.cuh" // vsm_unproject: shared with the shadow resolve
 
 namespace oxc {
 
@@ -253,13 +254,6 @@ struct VsmMarkParams {
   int width, height, size, clipmap_count;
   float texel_length, bias;
 };
-
-OXC_DI void vsm_unproject(const VsmMarkParams& p, float u, float v, float depth, float& x, float& y, float& z) {
-  const float nx = fs(fm(u, 2.0f), 1.0f), ny = fs(fm(v, 2.0f), 1.0f);
-  const float hx = row_dot4(p.inv_pv_row[0], nx, ny, depth, 1.0f), hy = row_dot4(p.inv_pv_row[1], nx, ny, depth, 1.0f);
-  const float hz = row_dot4(p.inv_pv_row[2], nx, ny, depth, 1.0f), hw = row_dot4(p.inv_pv_row[3], nx, ny, depth, 1.0f);
-  x = fd(hx, hw); y = fd(hy, hw); z = fd(hz, hw);
-}
 
 __global__ void __launch_bounds__(256) k_vsm_mark_visible_pages(const __grid_constant__ VsmMarkParams p) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);

@@ -244,6 +244,66 @@ OXC_DI float canonical_log2(float x) {
   return fa((float)e, fm(t, p));
 }
 
+// binary64 operations of canonical_sincos: the device intrinsics are never contracted; the host build runs -ffp-contract=off
+OXC_DI double dmul64(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+OXC_DI double dadd64(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+OXC_DI float d2f_rn(double a) {
+#ifdef __CUDA_ARCH__
+  return __double2float_rn(a);
+#else
+  return (float)a;
+#endif
+}
+
+// sin and cos for decision paths (VSM shadow resolve), bit-identical to oracle/oxc_oracle_vsm_resolve.c orc_sincos_canonical.  Binary64 throughout: k = rint(x * 2/pi),
+// r = (x - k * PIO2_HI) - k * PIO2_LO (PIO2_HI has 33 significant bits, so k * PIO2_HI is exact for |k| < 2^20), Taylor
+// polynomials of sin (to r^15) and cos (to r^16) on |r| <= pi/4, the quadrant k mod 4, one rounding to binary32.
+// Error against the exact sin / cos: <= 1 ulp of the binary32 result on [0, 2 pi]; <= 2^-24 absolute for |x| <= 2^21 (the hash's
+// arguments reach 1.43e6 at 3840 x 2160).  Non-finite x gives NaN.
+OXC_DI void canonical_sincos(float xf, float& s_out, float& c_out) {
+  const double x = (double)xf;
+  if (!(x - x == 0.0)) { s_out = c_out = xf - xf; return; } // inf / NaN -> NaN
+  const double k = rint(dmul64(x, 0.63661977236758134308));
+  const double r = dadd64(dadd64(x, -dmul64(k, 1.57079632673412561417e+00)), -dmul64(k, 6.07710050650619224932e-11));
+  const double z = dmul64(r, r);
+  double ps = -7.6471637318198164759e-13;                    // -1/15!
+  ps = dadd64(1.6059043836821614599e-10, dmul64(z, ps));     // 1/13!
+  ps = dadd64(-2.5052108385441718775e-08, dmul64(z, ps));    // -1/11!
+  ps = dadd64(2.7557319223985890653e-06, dmul64(z, ps));     // 1/9!
+  ps = dadd64(-1.9841269841269841270e-04, dmul64(z, ps));    // -1/7!
+  ps = dadd64(8.3333333333333333333e-03, dmul64(z, ps));     // 1/5!
+  ps = dadd64(-1.6666666666666666667e-01, dmul64(z, ps));    // -1/3!
+  const double sn = dadd64(r, dmul64(dmul64(r, z), ps));
+  double pc = 4.7794773323873852974e-14;                     // 1/16!
+  pc = dadd64(-1.1470745597729724714e-11, dmul64(z, pc));    // -1/14!
+  pc = dadd64(2.0876756987868098979e-09, dmul64(z, pc));     // 1/12!
+  pc = dadd64(-2.7557319223985890653e-07, dmul64(z, pc));    // -1/10!
+  pc = dadd64(2.4801587301587301587e-05, dmul64(z, pc));     // 1/8!
+  pc = dadd64(-1.3888888888888888889e-03, dmul64(z, pc));    // -1/6!
+  pc = dadd64(4.1666666666666666667e-02, dmul64(z, pc));     // 1/4!
+  pc = dadd64(-0.5, dmul64(z, pc));                          // -1/2!
+  const double cs = dadd64(1.0, dmul64(z, pc));
+  const int q = (int)dadd64(k, -dmul64(4.0, floor(dmul64(k, 0.25)))); // k mod 4, exact for every finite k
+  const double sv = q == 0 ? sn : (q == 1 ? cs : (q == 2 ? -sn : -cs));
+  const double cv = q == 0 ? cs : (q == 1 ? -sn : (q == 2 ? -cs : sn));
+  s_out = d2f_rn(sv);
+  c_out = d2f_rn(cv);
+}
+OXC_DI float canonical_sin(float x) { float s, c; canonical_sincos(x, s, c); return s; }
+OXC_DI float canonical_cos(float x) { float s, c; canonical_sincos(x, s, c); return c; }
+
 // cull.slang:169-171: determinant(f32x3x3(c0.xyw, c1.xyw, c2.xyw)) >= 0.0001
 OXC_DI bool triangle_backface(float4 c0, float4 c1, float4 c2) {
   const float m00 = c0.x, m01 = c0.y, m02 = c0.w;

@@ -23,6 +23,7 @@
 #include "kernels_alpha.cuh"
 #include "kernels_vsm.cuh"
 #include "kernels_vsm_draw.cuh"
+#include "kernels_vsm_resolve.cuh"
 
 using namespace oxc;
 
@@ -1171,6 +1172,20 @@ int oxc_decode_visbuffer(OxcContext* c, const OxcCullCamera* cam, const uint64_t
   return OXC_OK;
 }
 
+} // extern "C"
+
+namespace {
+// rmvsm.slang:147-154 get_first_clipmap_texel_length with the oracle's operation order (host floats: IEEE, no contraction)
+float vsm_first_texel_length(const OxcVsmContext* vsm) {
+  volatile float scale_ratio = (float)(vsm->page_table_size - 1) / (float)vsm->page_table_size;
+  volatile float effective_width = vsm->first_clipmap_width * scale_ratio;
+  volatile float twice = effective_width * 2.0f;
+  return twice / vsm->virtual_extent;
+}
+} // namespace
+
+extern "C" {
+
 int oxc_mark_visible_pages(OxcContext* c, const float inv_pv[16], const float resolution[2], const OxcVirtualClipmap* clipmaps,
                            const OxcVsmContext* vsm, const float* depth_dev, uint32_t* page_tables_dev, uint32_t* page_occupancy_dev,
                            uint32_t* request_count_dev, int32_t* requests_dev, uint32_t request_capacity, void* stream) {
@@ -1192,12 +1207,7 @@ int oxc_mark_visible_pages(OxcContext* c, const float inv_pv[16], const float re
   p.depth = depth_dev; p.page_tables = page_tables_dev; p.page_occupancy = page_occupancy_dev; p.request_count = request_count_dev;
   p.requests = requests_dev; p.request_capacity = request_capacity;
   p.width = vsm->depth_extent[0]; p.height = vsm->depth_extent[1]; p.size = vsm->page_table_size; p.clipmap_count = vsm->clipmap_count;
-  {  // rmvsm.slang:147-154
-    volatile float scale_ratio = (float)(vsm->page_table_size - 1) / (float)vsm->page_table_size;
-    volatile float effective_width = vsm->first_clipmap_width * scale_ratio;
-    volatile float twice = effective_width * 2.0f;
-    p.texel_length = twice / vsm->virtual_extent;
-  }
+  p.texel_length = vsm_first_texel_length(vsm);
   p.bias = vsm->clipmap_selection_bias;
   const dim3 grid((p.width + 31) / 32, (p.height + 7) / 8);
   k_vsm_mark_visible_pages<<<grid, 256, 0, s>>>(p);
@@ -1404,6 +1414,43 @@ int oxc_vsm_draw_stats(OxcContext* c, uint32_t out[2], void* stream) {
   CK(cudaSetDevice(c->device));
   CK(cudaMemcpyAsync(out, c->d_vsm_counters, 8, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
+  return OXC_OK;
+}
+
+int oxc_vsm_resolve_shadows(OxcContext* c, const OxcVsmContext* vsm, const float inv_pv[16], const float resolution[2],
+                            const OxcVirtualClipmap* clipmaps, const float* depth_dev, const float* normals_dev, const uint32_t* page_tables_dev,
+                            const float* physical_atlas_dev, float* shadow_dev, void* stream) {
+  if (!c || !vsm || !inv_pv || !resolution || !clipmaps || !depth_dev || !normals_dev || !page_tables_dev || !physical_atlas_dev || !shadow_dev)
+    return fail(OXC_E_INVALID, "null argument");
+  int rc = check_vsm(vsm, 0xFFFFFFFFu);
+  if (rc != OXC_OK) return rc;
+  if (vsm->depth_extent[0] < 1 || vsm->depth_extent[1] < 1)
+    return fail(OXC_E_INVALID, "depth_extent %d x %d is empty", vsm->depth_extent[0], vsm->depth_extent[1]);
+  if (reinterpret_cast<uintptr_t>(normals_dev) & 15u) return fail(OXC_E_INVALID, "normals_dev is not 16-byte aligned (float4 per pixel)");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  VsmResolveParams p{};
+  for (int i = 0; i < 4; i++) p.inv_pv_row[i] = make_float4(inv_pv[i], inv_pv[4 + i], inv_pv[8 + i], inv_pv[12 + i]);
+  p.inv_res_half[0] = (1.0f / resolution[0]) * 0.5f; p.inv_res_half[1] = (1.0f / resolution[1]) * 0.5f; // as oxc_mark_visible_pages
+  for (int k = 0; k < vsm->clipmap_count; k++) {
+    const float* m = clipmaps[k].projection_view_mat;
+    for (int i = 0; i < 4; i++)
+      for (int j = 0; j < 4; j++) p.clipmap_row[k][i][j] = m[j * 4 + i];
+    p.page_offset[k][0] = clipmaps[k].page_offset[0]; p.page_offset[k][1] = clipmaps[k].page_offset[1];
+    p.ortho[k] = m[3] == 0.0f && m[7] == 0.0f && m[11] == 0.0f && m[15] == 1.0f;
+  }
+  for (int i = 0; i < VSM_RESOLVE_BLOCKER_SAMPLES; i++) vsm_hammersley((uint32_t)i, VSM_RESOLVE_BLOCKER_SAMPLES, p.ham[i][0], p.ham[i][1]);
+  for (int i = 0; i < VSM_RESOLVE_PCF_SAMPLES; i++)
+    vsm_hammersley((uint32_t)i, VSM_RESOLVE_PCF_SAMPLES, p.ham[VSM_RESOLVE_BLOCKER_SAMPLES + i][0], p.ham[VSM_RESOLVE_BLOCKER_SAMPLES + i][1]);
+  for (int i = 0; i < 3; i++) p.light[i] = vsm->directional_light_dir[i];
+  p.depth = depth_dev; p.normals = reinterpret_cast<const float4*>(normals_dev); p.page_tables = page_tables_dev; p.atlas = physical_atlas_dev;
+  p.shadow = shadow_dev;
+  p.width = vsm->depth_extent[0]; p.height = vsm->depth_extent[1]; p.size = vsm->page_table_size; p.clipmap_count = vsm->clipmap_count;
+  p.page_size = vsm->page_size; p.atlas_size = vsm->physical_page_table_size; p.phys_per_row = vsm->physical_page_table_size / vsm->page_size;
+  p.texel_length = vsm_first_texel_length(vsm); p.bias = vsm->clipmap_selection_bias; p.z_length = vsm->z_length;
+  const dim3 grid((p.width + VSM_RESOLVE_TILE_X - 1) / VSM_RESOLVE_TILE_X, (p.height + VSM_RESOLVE_TILE_Y - 1) / VSM_RESOLVE_TILE_Y);
+  k_vsm_resolve_shadows<<<grid, VSM_RESOLVE_THREADS, 0, s>>>(p);
+  LAUNCHED();
   return OXC_OK;
 }
 

@@ -132,6 +132,31 @@ def make_ortho_view(direction, center, half_size, depth_range, mesh_instance_cou
     return cam
 
 
+def make_vsm_clipmaps(light_dir, camera_position, count=10, first_clipmap_width=10.0, max_shadow_dist=1000.0, page_table_size=64):
+    """The directional light's virtual clipmaps as the reference builds them (Passes/Shadowmaps.cpp:9-60): light_dir points TOWARDS the
+    light (the view looks along -light_dir), glm::lookAtRH from the origin, glm::orthoRH_ZO(+-extent, near = -max_shadow_dist,
+    far = +max_shadow_dist) with y flipped, so a point closer to the light has the SMALLER depth; the projection is shifted by whole
+    pages so that the camera sits in the centre page, and page_offset is that shift.  Returns an abi.CLIPMAP_DT array."""
+    fwd = -np.asarray(light_dir, dtype=np.float64)
+    fwd /= np.linalg.norm(fwd)
+    up = (0.0, 1.0, 0.0) if 1.0 - abs(fwd[1]) >= 1e-5 else (0.0, 0.0, 1.0)
+    view = look_at((0.0, 0.0, 0.0), fwd, up).reshape(4, 4).T.astype(np.float64)  # row-major
+    cm = np.zeros(count, dtype=abi.CLIPMAP_DT)
+    for k in range(count):
+        e = first_clipmap_width * float(1 << k)
+        n, f = -max_shadow_dist, max_shadow_dist
+        proj = np.eye(4)
+        proj[0, 0], proj[1, 1], proj[2, 2], proj[2, 3] = 1.0 / e, -1.0 / e, -1.0 / (f - n), -n / (f - n)  # orthoRH_ZO, [1][1] *= -1
+        clip = proj @ view @ np.append(np.asarray(camera_position, dtype=np.float64), 1.0)
+        offset = np.trunc(clip[:2] / clip[3] * 0.5 * page_table_size).astype(np.int32)  # glm::ivec2 truncates
+        shift = np.eye(4)
+        shift[:2, 3] = -(offset / page_table_size) * 2.0
+        cm["projection_view_mat"][k] = (shift @ proj @ view).astype(np.float32).T.reshape(16)
+        cm["page_offset"][k] = offset
+        cm["z_near"][k] = n
+    return cm
+
+
 # 7x7 grid patch: 49 vertices, 72 triangles, the last 8 dropped -> 64 (SURVEY §8d)
 _GRID = 7
 _VERTS = _GRID * _GRID
