@@ -399,8 +399,23 @@ typedef struct OxcMaterial { /* SceneGPU.hpp:67-82 / scene.slang:51-66, 56 B */
 } OxcMaterial;
 #define OXC_MATERIAL_HAS_ALBEDO_IMAGE (1u << 0) /* MaterialFlag::HasAlbedoImage */
 #define OXC_MATERIAL_ALPHA_MASK (1u << 8)       /* MaterialFlag::AlphaMask (informational: the encode pass tests HasAlbedoImage only) */
+/* read by oxc_decode_gbuffer only */
+#define OXC_MATERIAL_HAS_NORMAL_IMAGE (1u << 1)             /* MaterialFlag::HasNormalImage */
+#define OXC_MATERIAL_HAS_EMISSIVE_IMAGE (1u << 2)           /* MaterialFlag::HasEmissiveImage */
+#define OXC_MATERIAL_HAS_METALLIC_ROUGHNESS_IMAGE (1u << 3) /* MaterialFlag::HasMetallicRoughnessImage */
+#define OXC_MATERIAL_HAS_OCCLUSION_IMAGE (1u << 4)          /* MaterialFlag::HasOcclusionImage */
+#define OXC_MATERIAL_NORMAL_TWO_COMPONENT (1u << 5)         /* MaterialFlag::NormalTwoComponent */
+#define OXC_MATERIAL_NORMAL_FLIP_Y (1u << 6)                /* MaterialFlag::NormalFlipY */
 
-enum OxcImageFormat { OXC_IMAGE_RGBA8_UNORM = 0 /* alpha = byte 3 (sRGB variants: alpha is linear) */, OXC_IMAGE_R8_UNORM = 1 /* alpha only */ };
+/* The alpha test reads byte 3 of the RGBA formats (sRGB or not: alpha is linear) and the byte of R8 as alpha.  oxc_decode_gbuffer
+ * converts a texel as Vulkan does: R8 -> (r, 0, 0, 1), RG8 -> (r, g, 0, 1), sRGB rgb through the EOTF.  oxc_set_materials accepts
+ * RGBA8_UNORM, RGBA8_SRGB and R8_UNORM for an albedo image; RG8_UNORM is for the decode's other images (two-component normal maps). */
+enum OxcImageFormat {
+  OXC_IMAGE_RGBA8_UNORM = 0,
+  OXC_IMAGE_R8_UNORM = 1,
+  OXC_IMAGE_RGBA8_SRGB = 2, /* glTF base colour and emissive images (AssetManager_GLTF.cpp:887) */
+  OXC_IMAGE_RG8_UNORM = 3
+};
 typedef struct OxcAlphaImage {  /* one entry of the engine's bindless image table, the part this pass reads */
   const void* texels_dev;       /* device pointer to level 0, tightly packed rows; level l (max(1, width >> l) x max(1, height >> l)) */
   uint32_t width, height;       /*   follows level l - 1 immediately (vkCmdCopyImageToBuffer with consecutive regions).  1..65536 */
@@ -514,8 +529,8 @@ int oxc_cull_terrain(OxcContext* ctx, const OxcTerrainData* terrain, const float
  * (scene.slang:363-399), world positions, compute_partial_derivatives (:42-92: analytic perspective-correct
  * barycentrics lambda and their per-pixel derivatives), gradient_of the vertex texture coordinates (:33-40) and the
  * geometric world normal normalize(mul(lambda, to_world_normals)) (:146-147) oct-encoded (common/encoding.slang:17-21).
- * The material evaluation (texture sampling, tangent frame from the sampled normal map, :118-183) needs the engine's
- * material and image tables and is not part of this library.  The frame's oxc_cull_meshes must have run (it resolves
+ * The material evaluation (texture sampling, tangent frame from the sampled normal map, :118-183) is oxc_decode_gbuffer's,
+ * below.  The frame's oxc_cull_meshes must have run (it resolves
  * LODs and pointers).  Exactly one of vis64_dev (our packed image) / vis32_dev (the reference's R32UI attachment).
  * Targets are float4-per-pixel planes, any may be NULL:
  *   lambda    = (lambda.xyz, status)  status 0: discarded (clear / terrain texel, :97-99), 1: decoded,
@@ -533,6 +548,49 @@ typedef struct OxcDecodeTargets {
 int oxc_decode_visbuffer(OxcContext* ctx, const OxcCullCamera* camera, const uint64_t* vis64_dev, const uint32_t* vis32_dev,
                          uint32_t width, uint32_t height, const OxcDecodeTargets* targets /* host struct of device ptrs */,
                          void* stream);
+
+/* Vis-buffer decode into the G-buffer: passes/visbuffer_decode.slang:88-183 with the material functions of scene.slang:110-159.  Same
+ * inputs and preconditions as oxc_decode_visbuffer (exactly one of vis64_dev / vis32_dev, the frame's oxc_cull_meshes has run), and
+ * the material table of the last oxc_set_materials (OXC_E_STATE without one).  Four float4 planes, row-major, 16-byte aligned; any
+ * may be NULL, and a NULL target's images are not sampled:
+ *   albedo                       rgba                                          (SV_Target0)
+ *   normal                       oct(mapped normal).xy, oct(world normal).zw   (SV_Target1; .zw == oxc_decode_visbuffer's uv_normal.zw,
+ *                                                                               so the plane feeds oxc_vsm_resolve_shadows as is)
+ *   emissive                     rgb, w = 0                                    (SV_Target2)
+ *   metallic_roughness_occlusion metallic, roughness, occlusion, w = 0         (SV_Target3)
+ * SPECIFICATION (oracle/oxc_oracle_gbuffer.c orc_decode_gbuffer, bit for bit): IEEE binary32, no contraction, sums in written order.
+ *   1. a pixel oxc_decode_visbuffer discards is NOT written (a fragment discard keeps the attachment's contents); a vertex index
+ *      >= vertex_count, and a mesh instance whose material_index lies outside the table (it raises OXC_STATUS_BAD_MATERIAL), write
+ *      zeros to every target.
+ *   2. lambda, its derivatives, the world positions and the world normal n: exactly oxc_decode_visbuffer's arithmetic.
+ *   3. uv = uv * uv_size + uv_offset, uv_ddx *= uv_size, uv_ddy *= uv_size (dequantize_half of the material's halves).
+ *   4. SampleGrad per image (level-0 size w0 x h0, the material's sampler): mx = uv_ddx.u * w0, my = uv_ddx.v * h0, nx = uv_ddy.u * w0,
+ *      ny = uv_ddy.v * h0; from there the level rule of the alpha test above (canonical log2, mag / min choice, clamp, trilinear or
+ *      nearest level) and its per-channel filter order.  No anisotropy, LOD bias or clamp.
+ *   5. a texel becomes RGBA before filtering: RGBA8_UNORM c / 255; RGBA8_SRGB rgb = the binary32 nearest to the sRGB EOTF of c / 255,
+ *      a = c / 255; R8_UNORM (r / 255, 0, 0, 1) — what Vulkan returns; the alpha test keeps reading R8 as alpha; RG8_UNORM
+ *      (r / 255, g / 255, 0, 1).
+ *   6. albedo = albedo_color * sample (HasAlbedoImage) or albedo_color.
+ *   7. p_i = world_i - camera.position; pos_ddx = (ddx0*p0 + ddx1*p1) + ddx2*p2 (ddy likewise); pos_ddx_s = pos_ddx - dot(pos_ddx, n)*n;
+ *      js = sign(uv_ddx.x*uv_ddy.y - uv_ddx.y*uv_ddy.x) (NaN -> 0); T = js*(uv_ddy.y*pos_ddx_s - uv_ddx.y*pos_ddy_s), normalized if
+ *      js != 0; w = js*sign(dot(pos_ddy, cross(n, pos_ddx))); B = -w*cross(n, T).  HasNormalImage: s = sample.rgb*2 - 1, NormalFlipY
+ *      negates s.y, NormalTwoComponent sets s.z = sqrt(saturate(1 - (s.x*s.x + s.y*s.y))) (saturate(NaN) = 0), normal =
+ *      normalize((s.x*T + s.y*B) + s.z*n); else normal = n.  normalize(v) = v / sqrt(dot(v, v)).
+ *   8. emissive = emissive_color * sample.rgb or emissive_color; (metallic, roughness) = factors * sample.bg or the factors;
+ *      occlusion = sample.r or 1.
+ * Images named by a flag other than HasAlbedoImage are checked here, not by oxc_set_materials: OXC_E_INVALID, naming the material
+ * and the slot, when one lies outside the image table or fails the albedo checks (null or not 4-byte aligned texels, extent,
+ * level_count, format), or when the material's sampler has an unknown mode.  Texels are read in software as aligned 32-bit words.
+ * No scratch: graph-capturable from the first call. */
+typedef struct OxcGBufferTargets { /* host struct of device pointers; float4 per pixel, row-major, 16-byte aligned; any may be NULL */
+  float* albedo;
+  float* normal;
+  float* emissive;
+  float* metallic_roughness_occlusion;
+} OxcGBufferTargets;
+OXC_STATIC_ASSERT(sizeof(OxcGBufferTargets) == 32, "GBufferTargets");
+int oxc_decode_gbuffer(OxcContext* ctx, const OxcCullCamera* camera, const uint64_t* vis64_dev, const uint32_t* vis32_dev,
+                       uint32_t width, uint32_t height, const OxcGBufferTargets* targets, void* stream);
 
 /* Hierarchical page bitmap build (SURVEY §8f.4): passes/rmvsm_downsample_hpb.slang:15-33 dispatched per level by
  * Shadowmaps.cpp:331-366.  Level 0: byte = page is visible && backed && dirty (VSMPageState bits 1 | 4 | 2,
@@ -859,6 +917,13 @@ int oxr_vsm_draw_shadows(OxrRenderer* r, const OxcCullCamera* coarse);
  * table and the atlas are left as they were.  OXC_E_STATE before an oxr_vsm_update_pages;
  * OXC_E_CAPACITY, with the camera path left usable, when the 20 B / pixel of its own planes cannot be allocated. */
 int oxr_vsm_resolve_shadows(OxrRenderer* r, const OxcCullCamera* camera, float* shadow_host);
+/* RendererInstance's vis decode pass (visbuffer_decode.slang:88-183): oxc_decode_gbuffer on the frame oxr_render / oxr_wait completed
+ * last, with `camera` (the camera that frame was rendered with) and the table of the last oxr_set_materials, into planes the renderer
+ * allocates at the first call (64 B / pixel); each non-NULL host pointer receives width x height float4.  Synchronous.  Pixels the
+ * decode discards hold 0.  The frame's outputs are left as they were.  OXC_E_CAPACITY, with the camera path left usable, when the
+ * planes cannot be allocated. */
+int oxr_decode_gbuffer(OxrRenderer* r, const OxcCullCamera* camera, float* albedo_host, float* normal_host, float* emissive_host,
+                       float* metallic_roughness_occlusion_host);
 
 /* ------------------------------------------------------------------------------------------------
  * oxb_* — mesh builder (SURVEY §8f.2): host-side producer of the blob layout above, mirroring build_gltf_mesh

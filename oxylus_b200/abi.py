@@ -141,7 +141,9 @@ MATERIAL_DT = np.dtype(
 )
 assert MATERIAL_DT.itemsize == 56
 MATERIAL_HAS_ALBEDO_IMAGE, MATERIAL_ALPHA_MASK = 1, 1 << 8
-IMAGE_RGBA8_UNORM, IMAGE_R8_UNORM = 0, 1
+IMAGE_RGBA8_UNORM, IMAGE_R8_UNORM, IMAGE_RGBA8_SRGB, IMAGE_RG8_UNORM = 0, 1, 2, 3
+MATERIAL_HAS_NORMAL_IMAGE, MATERIAL_HAS_EMISSIVE_IMAGE, MATERIAL_HAS_METALLIC_ROUGHNESS_IMAGE, MATERIAL_HAS_OCCLUSION_IMAGE = 1 << 1, 1 << 2, 1 << 3, 1 << 4
+MATERIAL_NORMAL_TWO_COMPONENT, MATERIAL_NORMAL_FLIP_Y = 1 << 5, 1 << 6
 FILTER_LINEAR, FILTER_NEAREST = 0, 1
 ADDRESS_REPEAT, ADDRESS_CLAMP_TO_EDGE, ADDRESS_MIRRORED_REPEAT = 0, 1, 2
 MIPMAP_LINEAR, MIPMAP_NEAREST = 0, 1
@@ -292,6 +294,16 @@ class DecodeTargets(C.Structure):
     """OxcDecodeTargets: device pointers of the five float4 planes (any may be NULL)"""
 
     _fields_ = [("lambda_", C.c_void_p), ("ddx", C.c_void_p), ("ddy", C.c_void_p), ("uv_normal", C.c_void_p), ("uv_grad", C.c_void_p)]
+
+
+class GBufferTargets(C.Structure):
+    """OxcGBufferTargets: device pointers of the four float4 G-buffer planes (any may be NULL)"""
+
+    _fields_ = [("albedo", C.c_void_p), ("normal", C.c_void_p), ("emissive", C.c_void_p), ("metallic_roughness_occlusion", C.c_void_p)]
+
+
+assert C.sizeof(GBufferTargets) == 32
+GBUFFER_PLANES = ("albedo", "normal", "emissive", "metallic_roughness_occlusion")
 
 
 MESH_MAX_LODS = 8

@@ -19,7 +19,7 @@ SYMBOLS = [
     "oxc_update_transforms", "oxc_reset_visibility_mask", "oxc_clear_hiz", "oxc_set_shard", "oxc_set_shard_auto", "oxc_cull_meshes",
     "oxc_cull_meshlets", "oxc_build_hiz", "oxc_build_hiz_packed", "oxc_build_hiz_mip0_packed", "oxc_build_hiz_from_mip0", "oxc_cull_triangles", "oxc_cull_triangles_small_primitive", "oxc_clear_visbuffer",
     "oxc_raster_visbuffer", "oxc_raster_visbuffer_clip_pass", "oxc_set_materials", "oxc_raster_overdraw", "oxc_clear_overdraw", "oxc_resolve_visbuffer", "oxc_merge_depth", "oxc_clear_visbuffer_with_depth", "oxc_cull_meshlets_multiview", "oxc_cull_meshlets_hpb", "oxc_cull_terrain",
-    "oxc_decode_visbuffer", "oxc_build_hpb", "oxc_mark_visible_pages",
+    "oxc_decode_visbuffer", "oxc_decode_gbuffer", "oxc_build_hpb", "oxc_mark_visible_pages",
     "oxc_vsm_begin_frame", "oxc_vsm_invalidate_pages", "oxc_vsm_allocate_pages", "oxc_vsm_clear_dirty_pages", "oxc_cull_meshlets_hpb_dirty_dev",
     "oxc_vsm_draw_pages", "oxc_vsm_draw_stats", "oxc_vsm_resolve_shadows",
     "oxc_get_outputs", "oxc_check_status", "oxc_mark_hiz_dirty", "oxc_bind_camera_buffer", "oxc_load_camera", "oxc_debug_stats_ptr",
@@ -27,7 +27,7 @@ SYMBOLS = [
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
     "oxb_last_error", "oxb_build_mesh", "oxb_mesh_blob_size", "oxb_mesh_lod0_meshlet_count", "oxb_mesh_emit", "oxb_mesh_free", "oxb_simplify",
     "oxr_create", "oxr_destroy", "oxr_context", "oxr_update", "oxr_update_transforms", "oxr_set_external_depth", "oxr_set_materials", "oxr_overdraw", "oxr_render", "oxr_submit", "oxr_wait",
-    "oxr_vsm_update_pages", "oxr_vsm_pages", "oxr_vsm_draw_shadows", "oxr_vsm_resolve_shadows",
+    "oxr_vsm_update_pages", "oxr_vsm_pages", "oxr_vsm_draw_shadows", "oxr_vsm_resolve_shadows", "oxr_decode_gbuffer",
 ]
 
 
@@ -84,6 +84,7 @@ def load(build_if_missing=True):
     lib.oxc_cull_meshlets_hpb.argtypes = [vp, vp, vp, vp, u32, vp, u32, u32, vp]
     lib.oxc_cull_terrain.argtypes = [vp, vp, vp, vp, u32, vp, vp, vp, vp]
     lib.oxc_decode_visbuffer.argtypes = [vp, vp, vp, vp, u32, u32, C.POINTER(abi.DecodeTargets), vp]
+    lib.oxc_decode_gbuffer.argtypes = [vp, vp, vp, vp, u32, u32, C.POINTER(abi.GBufferTargets), vp]
     lib.oxc_build_hpb.argtypes = [vp, vp, u32, u32, vp, u32, vp]
     lib.oxc_mark_visible_pages.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, u32, vp]
     lib.oxc_vsm_begin_frame.argtypes = [vp, vp, i32, vp, vp, u32, vp, vp]
@@ -142,6 +143,7 @@ def load(build_if_missing=True):
     lib.oxr_vsm_pages.argtypes = [vp, C.POINTER(abi.VsmPages)]
     lib.oxr_vsm_draw_shadows.argtypes = [vp, vp]
     lib.oxr_vsm_resolve_shadows.argtypes = [vp, vp, vp]
+    lib.oxr_decode_gbuffer.argtypes = [vp, vp, vp, vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -414,6 +416,13 @@ class Context:
         t = abi.DecodeTargets(*[targets.get(k) for k in ("lambda_", "ddx", "ddy", "uv_normal", "uv_grad")])
         _check(self.lib.oxc_decode_visbuffer(self.h, _ptr(cam), _ptr(vis64_dev), _ptr(vis32_dev), w, h, C.byref(t), self.stream),
                "oxc_decode_visbuffer")
+
+    def decode_gbuffer(self, cam, w, h, targets, vis64_dev=None, vis32_dev=None):
+        """oxc_decode_gbuffer: targets a dict with any of albedo, normal, emissive, metallic_roughness_occlusion -> device pointers
+        (float4 planes); the material table of the last set_materials"""
+        t = abi.GBufferTargets(*[targets.get(k) for k in abi.GBUFFER_PLANES])
+        _check(self.lib.oxc_decode_gbuffer(self.h, _ptr(cam), _ptr(vis64_dev), _ptr(vis32_dev), w, h, C.byref(t), self.stream),
+               "oxc_decode_gbuffer")
 
     def mark_visible_pages(self, inv_pv, resolution, clipmaps, vsm, depth_dev, page_tables_dev, occupancy_dev, request_count_dev, requests_dev,
                            request_capacity):
@@ -713,6 +722,13 @@ class Renderer:
         out = np.zeros((self.scene.height, self.scene.width), dtype=np.float32)
         _check(self.lib.oxr_vsm_resolve_shadows(self.h, _ptr(cam), _ptr(out)), "oxr_vsm_resolve_shadows")
         return out
+
+    def decode_gbuffer(self, cam):
+        """oxr_decode_gbuffer: the G-buffer of the frame rendered last with `cam` as four float32 [height, width, 4] arrays (albedo,
+        normal, emissive, metallic_roughness_occlusion) from the table of the last set_materials"""
+        out = [np.zeros((self.scene.height, self.scene.width, 4), dtype=np.float32) for _ in abi.GBUFFER_PLANES]
+        _check(self.lib.oxr_decode_gbuffer(self.h, _ptr(cam), *[_ptr(o) for o in out]), "oxr_decode_gbuffer")
+        return tuple(out)
 
     def vsm_pages(self):
         """oxr_vsm_pages: abi.VsmPages of device pointers and sizes"""

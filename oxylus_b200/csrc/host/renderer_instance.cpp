@@ -100,7 +100,7 @@ RendererInstance::RendererInstance(int device, const OxcCreateInfo& info, uint32
 
 RendererInstance::~RendererInstance() {
   if (stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(stream_));
-  cudaFree(d_vis64_); cudaFree(d_vis32_); cudaFree(d_depth_); cudaFree(d_occluder_); cudaFree(d_overdraw_);
+  cudaFree(d_vis64_); cudaFree(d_vis32_); cudaFree(d_depth_); cudaFree(d_occluder_); cudaFree(d_overdraw_); cudaFree(d_gbuffer_);
   if (h_pinned_) cudaFreeHost(h_pinned_);
   if (copy_stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(copy_stream_));
   for (auto& sl : slots_) {
@@ -311,6 +311,35 @@ auto RendererInstance::resolve_shadowmap(const OxcCullCamera& camera, float* sha
                                     v.page_tables, v.physical_atlas, vsm_.d_shadow, stream_)) != OXC_OK) return fail(rc);
   if (cudaMemcpyAsync(shadow_host, vsm_.d_shadow, px * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
     return fail(OXC_E_CUDA);
+  return OXC_OK;
+}
+
+// the vis decode pass (RendererInstance's "vis decode", visbuffer_decode.slang:88-183) on stream_, synchronous: the G-buffer of the
+// frame rendered last, from its packed vis buffer and the material table of the last set_materials
+auto RendererInstance::decode_visbuffer(const OxcCullCamera& camera, float* albedo_host, float* normal_host, float* emissive_host, float* mro_host)
+    -> int {
+  if (!ctx_ || !error_.empty()) return OXC_E_STATE;
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  const size_t px = (size_t)width_ * height_;
+  // the planes are an optional part, as the resolve's are: without room for them the camera path stays usable
+  if (!d_gbuffer_ && cudaMalloc(reinterpret_cast<void**>(&d_gbuffer_), px * 64) != cudaSuccess) {
+    cudaGetLastError(); // clear the allocation error so that the next launch check does not report it
+    d_gbuffer_ = nullptr;
+    return OXC_E_CAPACITY;
+  }
+  float* const host[4] = {albedo_host, normal_host, emissive_host, mro_host};
+  OxcGBufferTargets targets{};
+  float** const dev[4] = {&targets.albedo, &targets.normal, &targets.emissive, &targets.metallic_roughness_occlusion};
+  for (int k = 0; k < 4; k++) *dev[k] = host[k] ? d_gbuffer_ + (size_t)k * px * 4 : nullptr;
+  int rc;
+  if ((rc = oxc_bind_camera_buffer(ctx_, nullptr)) != OXC_OK) return fail(rc); // as render(): the camera comes from the argument
+  if (cudaMemsetAsync(d_gbuffer_, 0, px * 64, s) != cudaSuccess) return fail(OXC_E_CUDA); // discarded pixels: the cleared attachment
+  rc = oxc_decode_gbuffer(ctx_, &camera, d_vis64_, nullptr, width_, height_, &targets, stream_);
+  if (rc == OXC_E_STATE || rc == OXC_E_INVALID) return rc; // no or unreadable material table: the frame state is intact
+  if (rc != OXC_OK) return fail(rc);
+  for (int k = 0; k < 4; k++)
+    if (host[k] && cudaMemcpyAsync(host[k], *dev[k], px * 16, cudaMemcpyDeviceToHost, s) != cudaSuccess) return fail(OXC_E_CUDA);
+  if (cudaStreamSynchronize(s) != cudaSuccess) return fail(OXC_E_CUDA);
   return OXC_OK;
 }
 
@@ -796,6 +825,12 @@ int oxr_vsm_draw_shadows(OxrRenderer* r, const OxcCullCamera* coarse) {
 int oxr_vsm_resolve_shadows(OxrRenderer* r, const OxcCullCamera* camera, float* shadow_host) {
   if (!r || !camera) return OXC_E_INVALID;
   return r->impl.resolve_shadowmap(*camera, shadow_host);
+}
+
+int oxr_decode_gbuffer(OxrRenderer* r, const OxcCullCamera* camera, float* albedo_host, float* normal_host, float* emissive_host,
+                       float* metallic_roughness_occlusion_host) {
+  if (!r || !camera) return OXC_E_INVALID;
+  return r->impl.decode_visbuffer(*camera, albedo_host, normal_host, emissive_host, metallic_roughness_occlusion_host);
 }
 
 int oxr_render(OxrRenderer* r, const OxcCullCamera* camera, const float* occluder_depth_host, uint32_t* vis32_host,

@@ -78,6 +78,9 @@ public:
   // resolve_shadowmap (Shadowmaps.cpp:756-822): decode the last frame's normals, then the PCSS shadow factor per pixel from the pages,
   // clipmaps and atlas of the last update_virtual_shadow_pages; width x height floats to the host
   auto resolve_shadowmap(const OxcCullCamera& camera, float* shadow_host) -> int;
+  // the vis decode pass (visbuffer_decode.slang:88-183) on the last rendered frame: albedo, normal, emissive and metallic / roughness /
+  // occlusion planes (float4 per pixel; any host pointer may be null) with the table of the last set_materials
+  auto decode_visbuffer(const OxcCullCamera& camera, float* albedo_host, float* normal_host, float* emissive_host, float* mro_host) -> int;
 
   // RendererInstance::render geometry section: run_geometry_pass(false) -> generate_hiz -> run_geometry_pass(true)
   auto render(const OxcCullCamera& camera, const float* occluder_depth_host, uint32_t* vis32_host, float* depth_host,
@@ -144,6 +147,7 @@ private:
   float* d_depth_ = nullptr;
   float* d_occluder_ = nullptr;
   uint32_t* d_overdraw_ = nullptr; // allocated by the first overdraw()
+  float* d_gbuffer_ = nullptr;      // four float4 planes of decode_visbuffer, allocated by its first call
   bool has_external_depth_ = false;
   // transforms as the host last uploaded them, and on the device the values before the upload that last changed each of them
   // (TransformPrevious::previous_world, RendererInstance.cpp:1600-1609)

@@ -99,6 +99,36 @@ OXC_DI void alpha_interpolate(const AlphaTri& t, long long e0, long long e1, lon
   v = fa(fa(fm(l0, t.v[0]), fm(l1, t.v[1])), fm(l2, t.v[2]));
 }
 
+OXC_DI float lerp_levels(float f, float lo, float hi) { return fa(fm(fs(1.0f, f), lo), fm(f, hi)); }
+OXC_DI float4 lerp_levels(float f, float4 lo, float4 hi) {
+  return make_float4(lerp_levels(f, lo.x, hi.x), lerp_levels(f, lo.y, hi.y), lerp_levels(f, lo.z, hi.z), lerp_levels(f, lo.w, hi.w));
+}
+
+// SampleGrad's level rule (oracle spec 4) from the texel-space derivatives mx = ddx(u) * width0, my = ddx(v) * height0, nx / ny
+// likewise for ddy: the isotropic lambda with the canonical log2, lambda > 0 -> min filter, then the nearest level or the trilinear
+// blend.  sample(level, filter) fetches one level.  alpha_keep below keeps its own written-out copy of this rule: calling the template
+// changed the SASS of k_raster_alpha and of the shadow raster's kernels (DESIGN §4.6).
+template <typename Sample>
+OXC_DI auto sample_grad_levels(float mx, float my, float nx, float ny, uint32_t levels, uint32_t mag_filter, uint32_t min_filter,
+                               uint32_t mipmap_mode, Sample sample) -> decltype(sample(0u, 0u)) {
+  const float rx2 = fa(fm(mx, mx), fm(my, my)), ry2 = fa(fm(nx, nx), fm(ny, ny));
+  const float r2 = rx2 > ry2 ? rx2 : ry2;
+  const float lambda = fm(0.5f, canonical_log2(r2));
+  const uint32_t filter = lambda > 0.0f ? min_filter : mag_filter;
+  const uint32_t qi = levels > 1u ? levels - 1u : 0u;
+  const float q = (float)qi;
+  const float lc = !(lambda > 0.0f) ? 0.0f : (lambda > q ? q : lambda);
+  if (mipmap_mode == OXC_MIPMAP_NEAREST) {
+    uint32_t d = lc <= 0.5f ? 0u : (uint32_t)ceilf(fa(lc, 0.5f)) - 1u;
+    d = d > qi ? qi : d;
+    return sample(d, filter);
+  }
+  const uint32_t d = (uint32_t)floorf(lc), dn = d + 1u > qi ? qi : d + 1u;
+  const float f = fs(lc, (float)d);
+  const auto lo = sample(d, filter), hi = sample(dn, filter);
+  return lerp_levels(f, lo, hi);
+}
+
 // alpha_keep is called from five places of k_raster_alpha (small / whole-warp / clipped paths); inlined everywhere the kernel was
 // 27 k instructions.  One out-of-line copy keeps it at a size the instruction cache can hold; the call costs nothing next to the
 // fetches.  (Host builds of this header — emulated library, tests — just inline it.)

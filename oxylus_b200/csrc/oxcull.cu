@@ -10,6 +10,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <new>
+#include <string>
 #include <vector>
 
 #include <dlfcn.h>
@@ -181,6 +182,11 @@ struct OxcContext {
   bool alpha_active = false;           // at least one material has an albedo image
   uint32_t* d_alpha_lists = nullptr;   // [2][max_meshlet_instances]: opaque, alpha-tested
   uint8_t* d_alpha_cmd = nullptr;      // 64 B: opaque cmd @0, alpha-tested cmd @16, an all-zero visibility record @32
+  // the G-buffer decode's table from the same oxc_set_materials: GBufMaterial[count], then GBufImage[count][GB_SLOTS]
+  uint8_t* d_gbuf_table = nullptr;
+  size_t gbuf_table_bytes = 0;
+  uint32_t gbuf_material_count = 0;    // 0: no table set
+  std::string gbuf_error;              // the first image or sampler of the table the decode cannot read (oxc_decode_gbuffer refuses)
   // VSM shadow draw (oxc_vsm_draw_pages): page bitmap, first pixel per page, work queue, counters; allocated by the first call
   uint32_t* d_vsm_bitmap = nullptr;
   int* d_vsm_first_px = nullptr;
@@ -420,7 +426,7 @@ void oxc_destroy(OxcContext* c) {
   cudaFree(c->d_cull_meshlets_cmd); cudaFree(c->d_cull_triangles_cmd); cudaFree(c->d_draw_cmd);
   cudaFree(c->d_reordered); cudaFree(c->d_tri_counter); cudaFree(c->d_raster_work); cudaFree(c->d_big_queue); cudaFree(c->d_clip_queue); cudaFree(c->d_id_base_auto); cudaFree(c->d_status); cudaFree(c->d_hiz);
   cudaFree(c->d_view_planes); cudaFree(c->d_view_bits); cudaFree(c->d_view_counts); cudaFree(c->d_inst_views);
-  cudaFree(c->d_alpha_materials); cudaFree(c->d_alpha_lists); cudaFree(c->d_alpha_cmd);
+  cudaFree(c->d_alpha_materials); cudaFree(c->d_alpha_lists); cudaFree(c->d_alpha_cmd); cudaFree(c->d_gbuf_table);
   cudaFree(c->d_vsm_bitmap); cudaFree(c->d_vsm_first_px); cudaFree(c->d_vsm_queue); cudaFree(c->d_vsm_counters);
   delete c;
 }
@@ -880,18 +886,6 @@ int oxc_clear_overdraw(OxcContext* c, uint32_t* overdraw, uint32_t w, uint32_t h
   return OXC_OK;
 }
 
-// scene.slang:92-94 on the host (integer bit manipulation: identical to the device's dequantize_half)
-static float host_dequantize_half(uint16_t h) {
-  const uint32_t sgn = ((uint32_t)h & 0x8000u) << 16, em = (uint32_t)h & 0x7fffu;
-  uint32_t r = (em + (112u << 10)) << 13;
-  r = (em < (1u << 10)) ? 0u : r;
-  r += (em >= (31u << 10)) ? (112u << 23) : 0u;
-  const uint32_t bits = sgn | r;
-  float f;
-  memcpy(&f, &bits, 4);
-  return f;
-}
-
 int oxc_set_materials(OxcContext* c, const OxcMaterialTable* t, void* stream) {
   if (!c) return fail(OXC_E_INVALID, "null context");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -899,6 +893,7 @@ int oxc_set_materials(OxcContext* c, const OxcMaterialTable* t, void* stream) {
   if (!t || t->material_count == 0) { // back to the plain encode
     c->alpha_active = false;
     c->alpha_material_count = 0;
+    c->gbuf_material_count = 0;
     return OXC_OK;
   }
   if (!t->materials || (t->image_count && !t->images) || (t->sampler_count && !t->samplers)) return fail(OXC_E_INVALID, "material table: null array");
@@ -913,7 +908,7 @@ int oxc_set_materials(OxcContext* c, const OxcMaterialTable* t, void* stream) {
       return fail(OXC_E_INVALID, "material %u: albedo_image_index %u outside the image table (%u)", i, m.albedo_image_index, t->image_count);
     const OxcAlphaImage& im = t->images[m.albedo_image_index];
     if (!im.texels_dev || im.width == 0 || im.height == 0 || im.width > (1u << 16) || im.height > (1u << 16) ||
-        (im.format != OXC_IMAGE_RGBA8_UNORM && im.format != OXC_IMAGE_R8_UNORM))
+        (im.format != OXC_IMAGE_RGBA8_UNORM && im.format != OXC_IMAGE_R8_UNORM && im.format != OXC_IMAGE_RGBA8_SRGB))
       return fail(OXC_E_INVALID, "image %u: null texels, extent outside 1..65536 or unknown format", m.albedo_image_index);
     uint32_t full_chain = 1;
     for (uint32_t e = im.width > im.height ? im.width : im.height; e > 1; e >>= 1) full_chain++;
@@ -946,10 +941,24 @@ int oxc_set_materials(OxcContext* c, const OxcMaterialTable* t, void* stream) {
     if (dalloc(&c->d_alpha_lists, (size_t)c->info.max_meshlet_instances * 2) != OXC_OK) return OXC_E_CUDA;
     if (dalloc(&c->d_alpha_cmd, (size_t)64) != OXC_OK) return OXC_E_CUDA;
   }
+  std::string gbuf_error;
+  const std::vector<uint8_t> gb = gbuffer_table(t, &gbuf_error);
+  if (gb.size() > c->gbuf_table_bytes) {
+    c->gbuf_material_count = 0;
+    CK(cudaStreamSynchronize(s)); // a decode in flight may still read the old table
+    cudaFree(c->d_gbuf_table);
+    c->d_gbuf_table = nullptr;
+    c->gbuf_table_bytes = 0;
+    if (dalloc(&c->d_gbuf_table, gb.size()) != OXC_OK) return OXC_E_CUDA;
+    c->gbuf_table_bytes = gb.size();
+  }
   CK(cudaMemcpyAsync(c->d_alpha_materials, ms.data(), ms.size() * sizeof(AlphaMaterial), cudaMemcpyHostToDevice, s));
-  CK(cudaStreamSynchronize(s)); // ms is a stack-owned staging copy
+  CK(cudaMemcpyAsync(c->d_gbuf_table, gb.data(), gb.size(), cudaMemcpyHostToDevice, s));
+  CK(cudaStreamSynchronize(s)); // ms and gb are stack-owned staging copies
   c->alpha_material_count = t->material_count;
   c->alpha_active = any;
+  c->gbuf_material_count = t->material_count;
+  c->gbuf_error = gbuf_error;
   return OXC_OK;
 }
 
@@ -1145,6 +1154,17 @@ int oxc_cull_terrain(OxcContext* c, const OxcTerrainData* terrain, const float* 
   return OXC_OK;
 }
 
+// the geometry inputs of both decode kernels (targets left null)
+static void decode_params(const OxcContext* c, const OxcCullCamera* cam, const uint64_t* vis64_dev, const uint32_t* vis32_dev, uint32_t w,
+                          uint32_t h, DecodeParams* p) {
+  p->vis64 = reinterpret_cast<const unsigned long long*>(vis64_dev); p->vis32 = vis32_dev;
+  p->meshlet_instances = c->d_meshlet_instances; p->vis = c->d_vis; p->inst = c->d_inst; p->geom = c->d_geom; p->id_base = c->id_base;
+  const float* m = cam->projection_view; // column-major: row i = (m[i], m[4+i], m[8+i], m[12+i])
+  for (int i = 0; i < 4; i++) p->pv_row[i] = make_float4(m[i], m[4 + i], m[8 + i], m[12 + i]);
+  p->res_x = cam->resolution[0]; p->res_y = cam->resolution[1];
+  p->width = w; p->height = h; p->prim_bits = c->prim_bits;
+}
+
 int oxc_decode_visbuffer(OxcContext* c, const OxcCullCamera* cam, const uint64_t* vis64_dev, const uint32_t* vis32_dev,
                          uint32_t w, uint32_t h, const OxcDecodeTargets* t, void* stream) {
   if (!c || !cam || !t) return fail(OXC_E_INVALID, "null argument");
@@ -1158,16 +1178,46 @@ int oxc_decode_visbuffer(OxcContext* c, const OxcCullCamera* cam, const uint64_t
   rc = refresh_inst_cache(c, cam, s); // world rows / normal-matrix rows of the frame's mesh instances
   if (rc != OXC_OK) return rc;
   DecodeParams p{};
-  p.vis64 = reinterpret_cast<const unsigned long long*>(vis64_dev); p.vis32 = vis32_dev;
-  p.meshlet_instances = c->d_meshlet_instances; p.vis = c->d_vis; p.inst = c->d_inst; p.geom = c->d_geom; p.id_base = c->id_base;
+  decode_params(c, cam, vis64_dev, vis32_dev, w, h, &p);
   p.lambda = reinterpret_cast<float4*>(t->lambda); p.ddx = reinterpret_cast<float4*>(t->ddx); p.ddy = reinterpret_cast<float4*>(t->ddy);
   p.uv_normal = reinterpret_cast<float4*>(t->uv_normal); p.uv_grad = reinterpret_cast<float4*>(t->uv_grad);
-  const float* m = cam->projection_view; // column-major: row i = (m[i], m[4+i], m[8+i], m[12+i])
-  for (int i = 0; i < 4; i++) p.pv_row[i] = make_float4(m[i], m[4 + i], m[8 + i], m[12 + i]);
-  p.res_x = cam->resolution[0]; p.res_y = cam->resolution[1];
-  p.width = w; p.height = h; p.prim_bits = c->prim_bits;
   const dim3 grid((w + DECODE_TX - 1) / DECODE_TX, (h + DECODE_TY - 1) / DECODE_TY);
   k_decode_visbuffer<<<grid, dim3(DECODE_TX, DECODE_TY), 0, s>>>(p);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_decode_gbuffer(OxcContext* c, const OxcCullCamera* cam, const uint64_t* vis64_dev, const uint32_t* vis32_dev, uint32_t w, uint32_t h,
+                       const OxcGBufferTargets* t, void* stream) {
+  if (!c || !cam || !t) return fail(OXC_E_INVALID, "null argument");
+  if ((vis64_dev == nullptr) == (vis32_dev == nullptr)) return fail(OXC_E_INVALID, "exactly one of vis64_dev / vis32_dev");
+  if (w == 0 || h == 0) return fail(OXC_E_INVALID, "empty extent %u x %u", w, h);
+  float* const planes[4] = {t->albedo, t->normal, t->emissive, t->metallic_roughness_occlusion};
+  static const char* const plane_name[4] = {"albedo", "normal", "emissive", "metallic_roughness_occlusion"};
+  for (int k = 0; k < 4; k++)
+    if (reinterpret_cast<uintptr_t>(planes[k]) & 15u) return fail(OXC_E_INVALID, "target %s is not 16-byte aligned (float4 per pixel)", plane_name[k]);
+  if (!c->scene_set) return fail(OXC_E_STATE, "oxc_set_scene first");
+  if (c->gbuf_material_count == 0) return fail(OXC_E_STATE, "oxc_set_materials first: the decode reads the material table");
+  if (!c->gbuf_error.empty()) return fail(OXC_E_INVALID, "material table: %s", c->gbuf_error.c_str());
+  int rc = check_vis_id_bits(c);
+  if (rc != OXC_OK) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  rc = refresh_inst_cache(c, cam, s); // world rows / normal-matrix rows of the frame's mesh instances
+  if (rc != OXC_OK) return rc;
+  GBufferParams p{};
+  decode_params(c, cam, vis64_dev, vis32_dev, w, h, &p.d);
+  p.mesh_instances = c->d_mesh_instances;
+  p.materials = reinterpret_cast<const GBufMaterial*>(c->d_gbuf_table);
+  p.images = reinterpret_cast<const GBufImage*>(c->d_gbuf_table + (size_t)c->gbuf_material_count * sizeof(GBufMaterial));
+  p.material_count = c->gbuf_material_count;
+  for (int k = 0; k < 4; k++) p.want |= planes[k] ? 1u << k : 0u;
+  for (int k = 0; k < 3; k++) p.cam[k] = cam->position[k];
+  p.albedo = reinterpret_cast<float4*>(t->albedo); p.normal = reinterpret_cast<float4*>(t->normal);
+  p.emissive = reinterpret_cast<float4*>(t->emissive); p.mro = reinterpret_cast<float4*>(t->metallic_roughness_occlusion);
+  p.status = c->d_status;
+  const dim3 grid((w + DECODE_TX - 1) / DECODE_TX, (h + DECODE_TY - 1) / DECODE_TY);
+  k_decode_gbuffer<<<grid, dim3(DECODE_TX, DECODE_TY), 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }
