@@ -806,6 +806,69 @@ int oxc_vsm_resolve_shadows(OxcContext* ctx, const OxcVsmContext* vsm, const flo
                             const OxcVirtualClipmap* clipmaps /* host */, const float* depth_dev, const float* normals_dev,
                             const uint32_t* page_tables_dev, const float* physical_atlas_dev, float* shadow_dev, void* stream);
 
+/* Ambient occlusion: RendererInstance::generate_ambient_occlusion (Passes/PBR.cpp:143-311), the visibility-bitmask GTAO of
+ * passes/gtao/vbgtao_prefilter.slang, vbgtao_main.slang and vbgtao_denoise.slang.  Three passes in stream order over a width x height
+ * frame: the depth prefilter (linear depth, 5 mips), the sector pass (edges and noisy occlusion) and the 3 x 3 edge-aware denoise.
+ * Inputs are only read: depth_dev (D32F, reversed Z, 0 = sky), normals_dev (float4 per pixel, oct(world normal) in .zw: the uv_normal
+ * plane of oxc_decode_visbuffer or the normal plane of oxc_decode_gbuffer, which carry the same .zw).  The caller owns every plane
+ * (OxcGtaoTargets), so the call uses no scratch and is graph-capturable from its first call.  camera.resolution is (width, height).
+ * Refused with OXC_E_INVALID: a NULL argument or target, a zero extent or one above 32768, slice_count outside 1..OXC_GTAO_MAX_SLICES,
+ * samples_per_slice_side outside 1..OXC_GTAO_MAX_SAMPLES_PER_SIDE, normals_dev not 16-byte aligned, a plane not naturally aligned.
+ * SPECIFICATION (oracle/oxc_oracle_gtao.c orc_generate_ambient_occlusion, bit for bit): IEEE binary32, no contraction, IEEE divide /
+ * sqrt, sums and products in written order, dot(a, b) = (a.x*b.x + a.y*b.y) + a.z*b.z, mul(M, v) row by row in the same order.
+ *   1. linearize(d) = m23 / (d + m22), (m23, m22) = (projection[3][2], projection[2][2]) (glm [column][row], PBR.cpp:183-186).
+ *   2. virtual pyramid: level 0 at any (x, y) >= 0 is linearize(depth[min(y, H-1)][min(x, W-1)]); level k at t is
+ *      weighted_average(L(k-1, 2t), L(k-1, 2t + (1, 0)), L(k-1, 2t + (0, 1)), L(k-1, 2t + (1, 1))) (vbgtao_prefilter.slang:23-39 with
+ *      its own constants).  Only the texels inside max(1, W >> k) x max(1, H >> k) are stored (depth_mips: levels 0..4 packed in
+ *      order, each row-major).  This is what the reference's 16 x 16-pixel groups compute, including values from beyond the extent.
+ *   3. gathers and point samples are integer texel reads with clamp to edge: the edges read mip 0 at the pixel and its left, right,
+ *      top (y - 1) and bottom (y + 1) neighbours; the normal is the pixel's own; the denoise reads the 3 x 3 neighbourhood of the
+ *      noisy plane and the pixel and its four direct neighbours of the edges plane.
+ *   4. edges (vbgtao_main.slang:69-100): e = (left, right, top, bottom) - centre, slopes, min(|e|, |e + slope|), saturate(1.25 - e /
+ *      (centre * 0.011)), packUnorm4x8 = round to nearest even of saturate(c) * 255, .x in the low byte.  Written for every pixel.
+ *   5. sky: centre linear depth >= far_clip * 0.999 writes 1 to the noisy plane.
+ *   6. SampleLevel(linear_clamp, uv, lambda): levels floor(lambda) and min(floor(lambda) + 1, 4), weight lambda - floor(lambda), both
+ *      always read; each level bilinear at uv * size - 0.5 with binary32 weights, top = a00 + wx * (a10 - a00), bottom likewise,
+ *      top + wy * (bottom - top), clamp to edge, NaN-safe saturating texel indices; blend (1 - f) * lo + f * hi.  No 8-bit weight
+ *      quantisation (deviation, as the alpha test's).  lambda = clamp(canonical_log2(length(offset * resolution)) - 3.3, 0, 4).
+ *   7. normal: .zw rounded to binary16 (round to nearest even; the reference's attachment is R16G16B16A16Sfloat), oct_to_vec3 (which
+ *      normalizes), mul(view, (n, 0)).xyz, normalize; normalize(v) = v / sqrt(dot(v, v)), length(v) = sqrt(dot(v, v)).
+ *   8. noise: index = the reference's 64 x 64 Hilbert index (RendererInstance.cpp:151-170) at (x % 64, y % 64) + 288 * (noise_index
+ *      % 64), then frac(0.5 + float(index) * (0.754877666, 0.569840291)) (R2).
+ *   9. cos / sin of the slice angle: canonical_sincos (as oxc_vsm_resolve_shadows); fast_acos as written; sign(NaN) = 0,
+ *      saturate(NaN) = 0, max / min return the other operand for a NaN, u32(x) truncates and saturates (NaN -> 0), frac(x) = x -
+ *      floor(x), countbits = popcount; constants are the binary32 roundings of the shader literals.
+ *  10. a NaN texel of the mip chain is stored as 0x7FFFFFFF; the noisy occlusion is stored as binary16 (round to nearest even,
+ *      R16F) and read back from it; the final AO is pow(max(denoised, 0), final_power) with canonical_pow (oxc_exact.cuh), written
+ *      as binary32 (the value before the reference's R16F store).
+ * Hostile depth (NaN, Inf, denormal, negative), normals and settings do not fault and follow the same rules. */
+#define OXC_GTAO_MAX_SLICES 16u
+#define OXC_GTAO_MAX_SAMPLES_PER_SIDE 8u
+typedef struct OxcGtaoSettings { /* SceneGPU.hpp:286-293 VBGTAOSettings */
+  float thickness;
+  uint32_t slice_count;            /* 1..OXC_GTAO_MAX_SLICES (the reference's presets use 1..9) */
+  uint32_t samples_per_slice_side; /* 1..OXC_GTAO_MAX_SAMPLES_PER_SIDE (the presets use 2..3) */
+  float effect_radius;
+  uint32_t noise_index;
+  float final_power;
+} OxcGtaoSettings;
+typedef struct OxcGtaoCamera {     /* the Camera fields the three passes read (scene.slang:162-188) */
+  float projection[16];            /* column-major, as Camera::projection */
+  float view[16];                  /* column-major, as Camera::view */
+  float far_clip;
+} OxcGtaoCamera;
+typedef struct OxcGtaoTargets {    /* device pointers, all required */
+  float* depth_mips;               /* levels 0..4, level k = max(1, W>>k) x max(1, H>>k) row-major, packed in order */
+  uint32_t* edges;                 /* "vbgtao depth differences", R32UI, W x H */
+  uint16_t* noisy_occlusion;       /* "vbgtao noisy occlusion", binary16, W x H */
+  float* ambient_occlusion;        /* W x H */
+} OxcGtaoTargets;
+OXC_STATIC_ASSERT(sizeof(OxcGtaoSettings) == 24, "GtaoSettings");
+OXC_STATIC_ASSERT(sizeof(OxcGtaoCamera) == 132, "GtaoCamera");
+OXC_STATIC_ASSERT(sizeof(OxcGtaoTargets) == 32, "GtaoTargets");
+int oxc_generate_ambient_occlusion(OxcContext* ctx, const OxcGtaoCamera* camera, const OxcGtaoSettings* settings, const float* depth_dev,
+                                   const float* normals_dev, uint32_t width, uint32_t height, const OxcGtaoTargets* targets, void* stream);
+
 int oxc_get_outputs(OxcContext* ctx, OxcOutputs* out);
 /* Instrumentation hook: 128 u64 counters that builds with -DOXC_RASTER_STATS fill (tools/raster_stats.py); zero otherwise. */
 void* oxc_debug_stats_ptr(OxcContext* ctx);
@@ -924,6 +987,13 @@ int oxr_vsm_resolve_shadows(OxrRenderer* r, const OxcCullCamera* camera, float* 
  * planes cannot be allocated. */
 int oxr_decode_gbuffer(OxrRenderer* r, const OxcCullCamera* camera, float* albedo_host, float* normal_host, float* emissive_host,
                        float* metallic_roughness_occlusion_host);
+/* RendererInstance::generate_ambient_occlusion (PBR.cpp:143-311): on the frame oxr_render / oxr_wait completed last, oxc_decode_visbuffer
+ * with `camera` into the uv_normal plane oxr_vsm_resolve_shadows uses (one plane for both calls), then oxc_generate_ambient_occlusion
+ * on the frame's depth with gtao_camera and settings; width x height floats to ao_host.  Its own planes (depth mips, edges, noisy and
+ * final occlusion, about 16 B / pixel) are allocated at the first call.  Synchronous.  The frame's outputs are left as they were.
+ * OXC_E_CAPACITY, with the camera path left usable, when the planes cannot be allocated. */
+int oxr_generate_ambient_occlusion(OxrRenderer* r, const OxcCullCamera* camera, const OxcGtaoCamera* gtao_camera,
+                                   const OxcGtaoSettings* settings, float* ao_host);
 
 /* ------------------------------------------------------------------------------------------------
  * oxb_* — mesh builder (SURVEY §8f.2): host-side producer of the blob layout above, mirroring build_gltf_mesh

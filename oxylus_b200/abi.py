@@ -306,6 +306,61 @@ assert C.sizeof(GBufferTargets) == 32
 GBUFFER_PLANES = ("albedo", "normal", "emissive", "metallic_roughness_occlusion")
 
 
+GTAO_MAX_SLICES = 16
+GTAO_MAX_SAMPLES_PER_SIDE = 8
+GTAO_LEVELS = 5
+
+
+class GtaoSettings(C.Structure):
+    """OxcGtaoSettings (SceneGPU.hpp:286-293 VBGTAOSettings)"""
+
+    _fields_ = [("thickness", C.c_float), ("slice_count", C.c_uint32), ("samples_per_slice_side", C.c_uint32), ("effect_radius", C.c_float),
+                ("noise_index", C.c_uint32), ("final_power", C.c_float)]
+
+
+class GtaoCamera(C.Structure):
+    """OxcGtaoCamera: Camera::projection and Camera::view (column-major) and far_clip"""
+
+    _fields_ = [("projection", C.c_float * 16), ("view", C.c_float * 16), ("far_clip", C.c_float)]
+
+
+class GtaoTargets(C.Structure):
+    """OxcGtaoTargets: device pointers of the depth mips, edges (u32), noisy occlusion (binary16) and final occlusion planes"""
+
+    _fields_ = [("depth_mips", C.c_void_p), ("edges", C.c_void_p), ("noisy_occlusion", C.c_void_p), ("ambient_occlusion", C.c_void_p)]
+
+
+assert C.sizeof(GtaoSettings) == 24 and C.sizeof(GtaoCamera) == 132 and C.sizeof(GtaoTargets) == 32
+
+# update_vbgtao_info's quality presets (PBR.cpp:149-170): (slice_count, samples_per_slice_side); the cvar default is 3, "ultra"
+GTAO_PRESETS = {0: (1, 2), 1: (2, 2), 2: (3, 3), 3: (9, 3)}
+
+
+def gtao_settings(quality_level=3, thickness=0.25, radius=0.5, final_power=1.2, noise_index=0):
+    """GtaoSettings as update_vbgtao_info fills them from the cvars (RendererCVar.cpp:36-41 defaults); noise_index stays 0 until
+    there is TAA (PBR.cpp:172-174)"""
+    slices, samples = GTAO_PRESETS[int(quality_level)]
+    return GtaoSettings(thickness, slices, samples, radius, noise_index, final_power)
+
+
+def gtao_camera(projection, view, far_clip):
+    c = GtaoCamera()
+    c.projection[:] = [float(x) for x in np.asarray(projection, dtype=np.float32).reshape(16)]
+    c.view[:] = [float(x) for x in np.asarray(view, dtype=np.float32).reshape(16)]
+    c.far_clip = float(np.float32(far_clip))
+    return c
+
+
+def gtao_mip_layout(width, height):
+    """[(offset, width, height)] of mips 0..4 in the packed depth_mips plane, and the total texel count"""
+    out, off = [], 0
+    for k in range(GTAO_LEVELS):
+        w, h = max(1, width >> k), max(1, height >> k)
+        out.append((off, w, h))
+        off += w * h
+    return out, off
+
+
 MESH_MAX_LODS = 8
 
 

@@ -21,13 +21,14 @@ SYMBOLS = [
     "oxc_raster_visbuffer", "oxc_raster_visbuffer_clip_pass", "oxc_set_materials", "oxc_raster_overdraw", "oxc_clear_overdraw", "oxc_resolve_visbuffer", "oxc_merge_depth", "oxc_clear_visbuffer_with_depth", "oxc_cull_meshlets_multiview", "oxc_cull_meshlets_hpb", "oxc_cull_terrain",
     "oxc_decode_visbuffer", "oxc_decode_gbuffer", "oxc_build_hpb", "oxc_mark_visible_pages",
     "oxc_vsm_begin_frame", "oxc_vsm_invalidate_pages", "oxc_vsm_allocate_pages", "oxc_vsm_clear_dirty_pages", "oxc_cull_meshlets_hpb_dirty_dev",
-    "oxc_vsm_draw_pages", "oxc_vsm_draw_stats", "oxc_vsm_resolve_shadows",
+    "oxc_vsm_draw_pages", "oxc_vsm_draw_stats", "oxc_vsm_resolve_shadows", "oxc_generate_ambient_occlusion",
     "oxc_get_outputs", "oxc_check_status", "oxc_mark_hiz_dirty", "oxc_bind_camera_buffer", "oxc_load_camera", "oxc_debug_stats_ptr",
     "oxc_mgpu_get_unique_id", "oxc_mgpu_init", "oxc_mgpu_init_with_comm", "oxc_mgpu_shutdown", "oxc_mgpu_info", "oxc_mgpu_exchange_hiz",
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
     "oxb_last_error", "oxb_build_mesh", "oxb_mesh_blob_size", "oxb_mesh_lod0_meshlet_count", "oxb_mesh_emit", "oxb_mesh_free", "oxb_simplify",
     "oxr_create", "oxr_destroy", "oxr_context", "oxr_update", "oxr_update_transforms", "oxr_set_external_depth", "oxr_set_materials", "oxr_overdraw", "oxr_render", "oxr_submit", "oxr_wait",
     "oxr_vsm_update_pages", "oxr_vsm_pages", "oxr_vsm_draw_shadows", "oxr_vsm_resolve_shadows", "oxr_decode_gbuffer",
+    "oxr_generate_ambient_occlusion",
 ]
 
 
@@ -95,6 +96,8 @@ def load(build_if_missing=True):
     lib.oxc_vsm_draw_pages.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     lib.oxc_vsm_draw_stats.argtypes = [vp, vp, vp]
     lib.oxc_vsm_resolve_shadows.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.oxc_generate_ambient_occlusion.argtypes = [vp, C.POINTER(abi.GtaoCamera), C.POINTER(abi.GtaoSettings), vp, vp, u32, u32,
+                                                   C.POINTER(abi.GtaoTargets), vp]
     lib.oxc_get_outputs.argtypes = [vp, C.POINTER(abi.Outputs)]
     lib.oxc_check_status.argtypes = [vp, vp, C.POINTER(C.c_uint32)]
     lib.oxc_mark_hiz_dirty.argtypes = [vp]
@@ -144,6 +147,7 @@ def load(build_if_missing=True):
     lib.oxr_vsm_draw_shadows.argtypes = [vp, vp]
     lib.oxr_vsm_resolve_shadows.argtypes = [vp, vp, vp]
     lib.oxr_decode_gbuffer.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.oxr_generate_ambient_occlusion.argtypes = [vp, vp, C.POINTER(abi.GtaoCamera), C.POINTER(abi.GtaoSettings), vp]
     _LIB = lib
     return lib
 
@@ -482,6 +486,14 @@ class Context:
         _check(self.lib.oxc_vsm_resolve_shadows(self.h, _ptr(vc), _ptr(ipv), _ptr(res), _ptr(cm), _ptr(depth_dev), _ptr(normals_dev),
                                                 _ptr(page_tables_dev), _ptr(atlas_dev), _ptr(shadow_dev), self.stream), "oxc_vsm_resolve_shadows")
 
+    def generate_ambient_occlusion(self, gtao_camera, settings, depth_dev, normals_dev, w, h, targets):
+        """oxc_generate_ambient_occlusion: prefilter, sector pass and denoise of a w x h frame.  gtao_camera / settings: abi.GtaoCamera /
+        abi.GtaoSettings; targets: dict depth_mips, edges, noisy_occlusion, ambient_occlusion -> device pointers (or abi.GtaoTargets)"""
+        t = targets if isinstance(targets, abi.GtaoTargets) else abi.GtaoTargets(*[targets.get(k) for k in
+                                                                                    ("depth_mips", "edges", "noisy_occlusion", "ambient_occlusion")])
+        _check(self.lib.oxc_generate_ambient_occlusion(self.h, C.byref(gtao_camera), C.byref(settings), _ptr(depth_dev), _ptr(normals_dev), w, h,
+                                                       C.byref(t), self.stream), "oxc_generate_ambient_occlusion")
+
     def build_hpb(self, page_table_dev, size, layers, hpb_dev, levels):
         _check(self.lib.oxc_build_hpb(self.h, _ptr(page_table_dev), size, layers, _ptr(hpb_dev), levels, self.stream), "oxc_build_hpb")
 
@@ -729,6 +741,14 @@ class Renderer:
         out = [np.zeros((self.scene.height, self.scene.width, 4), dtype=np.float32) for _ in abi.GBUFFER_PLANES]
         _check(self.lib.oxr_decode_gbuffer(self.h, _ptr(cam), *[_ptr(o) for o in out]), "oxr_decode_gbuffer")
         return tuple(out)
+
+    def generate_ambient_occlusion(self, cam, gtao_camera, settings):
+        """oxr_generate_ambient_occlusion: the ambient occlusion (float32 [height, width]) of the frame rendered last with `cam`
+        (gtao_camera: abi.GtaoCamera with that frame's projection, view and far clip; settings: abi.GtaoSettings)"""
+        out = np.zeros((self.scene.height, self.scene.width), dtype=np.float32)
+        _check(self.lib.oxr_generate_ambient_occlusion(self.h, _ptr(cam), C.byref(gtao_camera), C.byref(settings), _ptr(out)),
+               "oxr_generate_ambient_occlusion")
+        return out
 
     def vsm_pages(self):
         """oxr_vsm_pages: abi.VsmPages of device pointers and sizes"""

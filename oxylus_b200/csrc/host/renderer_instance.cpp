@@ -4,6 +4,7 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -101,6 +102,7 @@ RendererInstance::RendererInstance(int device, const OxcCreateInfo& info, uint32
 RendererInstance::~RendererInstance() {
   if (stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(stream_));
   cudaFree(d_vis64_); cudaFree(d_vis32_); cudaFree(d_depth_); cudaFree(d_occluder_); cudaFree(d_overdraw_); cudaFree(d_gbuffer_);
+  cudaFree(d_uv_normal_); cudaFree(d_gtao_);
   if (h_pinned_) cudaFreeHost(h_pinned_);
   if (copy_stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(copy_stream_));
   for (auto& sl : slots_) {
@@ -162,7 +164,7 @@ void RendererInstance::vsm_release() {
   OxrVsmPages& v = vsm_.pages;
   cudaFree(v.page_tables); cudaFree(v.hpb); cudaFree(v.page_occupancy); cudaFree(v.requests); cudaFree(v.allocator);
   cudaFree(v.free_page_list); cudaFree(v.dirty_physical_page_coords); cudaFree(v.clipmap_dirty_flags); cudaFree(v.physical_atlas);
-  cudaFree(vsm_.d_dirty_instances); cudaFree(vsm_.d_normals); cudaFree(vsm_.d_shadow);
+  cudaFree(vsm_.d_dirty_instances); cudaFree(vsm_.d_shadow);
   vsm_ = Vsm();
 }
 
@@ -294,20 +296,20 @@ auto RendererInstance::resolve_shadowmap(const OxcCullCamera& camera, float* sha
   const size_t px = (size_t)width_ * height_;
   // the resolve's own planes are an optional part, as the shadow draw's context is: without room for them the camera path stays
   // usable and this call returns OXC_E_CAPACITY (the sticky error is not set)
-  if (!vsm_.d_normals && (cudaMalloc(reinterpret_cast<void**>(&vsm_.d_normals), px * 16) != cudaSuccess ||
-                          cudaMalloc(reinterpret_cast<void**>(&vsm_.d_shadow), px * 4) != cudaSuccess)) {
+  if (uv_normal_plane() != OXC_OK) return OXC_E_CAPACITY;
+  if (!vsm_.d_shadow && cudaMalloc(reinterpret_cast<void**>(&vsm_.d_shadow), px * 4) != cudaSuccess) {
     cudaGetLastError(); // clear the allocation error so that the next launch check does not report it
-    cudaFree(vsm_.d_normals); vsm_.d_normals = nullptr;
+    vsm_.d_shadow = nullptr;
     return OXC_E_CAPACITY;
   }
   const OxrVsmPages& v = vsm_.pages;
   int rc;
   if ((rc = oxc_bind_camera_buffer(ctx_, nullptr)) != OXC_OK) return fail(rc); // as render(): the camera comes from the argument
   OxcDecodeTargets targets{};
-  targets.uv_normal = vsm_.d_normals;
+  targets.uv_normal = d_uv_normal_;
   if ((rc = oxc_decode_visbuffer(ctx_, &camera, d_vis64_, nullptr, width_, height_, &targets, stream_)) != OXC_OK) return fail(rc);
   if ((rc = oxc_resolve_visbuffer(ctx_, d_vis64_, width_, height_, nullptr, d_depth_, stream_)) != OXC_OK) return fail(rc);
-  if ((rc = oxc_vsm_resolve_shadows(ctx_, &vsm_.shape, vsm_.inv_projection_view, vsm_.resolution, vsm_.clipmaps, d_depth_, vsm_.d_normals,
+  if ((rc = oxc_vsm_resolve_shadows(ctx_, &vsm_.shape, vsm_.inv_projection_view, vsm_.resolution, vsm_.clipmaps, d_depth_, d_uv_normal_,
                                     v.page_tables, v.physical_atlas, vsm_.d_shadow, stream_)) != OXC_OK) return fail(rc);
   if (cudaMemcpyAsync(shadow_host, vsm_.d_shadow, px * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
     return fail(OXC_E_CUDA);
@@ -340,6 +342,52 @@ auto RendererInstance::decode_visbuffer(const OxcCullCamera& camera, float* albe
   for (int k = 0; k < 4; k++)
     if (host[k] && cudaMemcpyAsync(host[k], *dev[k], px * 16, cudaMemcpyDeviceToHost, s) != cudaSuccess) return fail(OXC_E_CUDA);
   if (cudaStreamSynchronize(s) != cudaSuccess) return fail(OXC_E_CUDA);
+  return OXC_OK;
+}
+
+int RendererInstance::uv_normal_plane() {
+  if (d_uv_normal_) return OXC_OK;
+  if (cudaMalloc(reinterpret_cast<void**>(&d_uv_normal_), (size_t)width_ * height_ * 16) != cudaSuccess) {
+    cudaGetLastError(); // clear the allocation error so that the next launch check does not report it
+    d_uv_normal_ = nullptr;
+    return OXC_E_CAPACITY;
+  }
+  return OXC_OK;
+}
+
+// PBR.cpp:143-311 generate_ambient_occlusion on stream_, synchronous: the vis decode's normals of the last frame (the reference's
+// normal_attachment .zw), its depth, then prefilter, sector pass and denoise into the renderer's own planes
+auto RendererInstance::generate_ambient_occlusion(const OxcCullCamera& camera, const OxcGtaoCamera& gtao_camera, const OxcGtaoSettings& settings,
+                                                  float* ao_host) -> int {
+  if (!ctx_ || !error_.empty()) return OXC_E_STATE;
+  if (!ao_host) return OXC_E_INVALID;
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  const size_t px = (size_t)width_ * height_;
+  size_t mip_texels = 0;
+  for (uint32_t k = 0; k < 5; k++) mip_texels += (size_t)std::max(1u, width_ >> k) * std::max(1u, height_ >> k);
+  // the planes are an optional part, as the resolve's are: without room for them the camera path stays usable
+  if (uv_normal_plane() != OXC_OK) return OXC_E_CAPACITY;
+  if (!d_gtao_ && cudaMalloc(&d_gtao_, mip_texels * 4 + px * 10) != cudaSuccess) {
+    cudaGetLastError();
+    d_gtao_ = nullptr;
+    return OXC_E_CAPACITY;
+  }
+  OxcGtaoTargets targets{};
+  targets.depth_mips = static_cast<float*>(d_gtao_);
+  targets.edges = reinterpret_cast<uint32_t*>(targets.depth_mips + mip_texels);
+  targets.ambient_occlusion = reinterpret_cast<float*>(targets.edges + px);
+  targets.noisy_occlusion = reinterpret_cast<uint16_t*>(targets.ambient_occlusion + px);
+  int rc;
+  if ((rc = oxc_bind_camera_buffer(ctx_, nullptr)) != OXC_OK) return fail(rc); // as render(): the camera comes from the argument
+  OxcDecodeTargets decode{};
+  decode.uv_normal = d_uv_normal_;
+  if ((rc = oxc_decode_visbuffer(ctx_, &camera, d_vis64_, nullptr, width_, height_, &decode, stream_)) != OXC_OK) return fail(rc);
+  if ((rc = oxc_resolve_visbuffer(ctx_, d_vis64_, width_, height_, nullptr, d_depth_, stream_)) != OXC_OK) return fail(rc);
+  rc = oxc_generate_ambient_occlusion(ctx_, &gtao_camera, &settings, d_depth_, d_uv_normal_, width_, height_, &targets, stream_);
+  if (rc == OXC_E_INVALID) return rc; // refused settings: nothing was launched, the frame state is intact
+  if (rc != OXC_OK) return fail(rc);
+  if (cudaMemcpyAsync(ao_host, targets.ambient_occlusion, px * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
+    return fail(OXC_E_CUDA);
   return OXC_OK;
 }
 
@@ -831,6 +879,12 @@ int oxr_decode_gbuffer(OxrRenderer* r, const OxcCullCamera* camera, float* albed
                        float* metallic_roughness_occlusion_host) {
   if (!r || !camera) return OXC_E_INVALID;
   return r->impl.decode_visbuffer(*camera, albedo_host, normal_host, emissive_host, metallic_roughness_occlusion_host);
+}
+
+int oxr_generate_ambient_occlusion(OxrRenderer* r, const OxcCullCamera* camera, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* settings,
+                                   float* ao_host) {
+  if (!r || !camera || !gtao_camera || !settings) return OXC_E_INVALID;
+  return r->impl.generate_ambient_occlusion(*camera, *gtao_camera, *settings, ao_host);
 }
 
 int oxr_render(OxrRenderer* r, const OxcCullCamera* camera, const float* occluder_depth_host, uint32_t* vis32_host,

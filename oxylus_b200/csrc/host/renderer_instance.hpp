@@ -81,6 +81,10 @@ public:
   // the vis decode pass (visbuffer_decode.slang:88-183) on the last rendered frame: albedo, normal, emissive and metallic / roughness /
   // occlusion planes (float4 per pixel; any host pointer may be null) with the table of the last set_materials
   auto decode_visbuffer(const OxcCullCamera& camera, float* albedo_host, float* normal_host, float* emissive_host, float* mro_host) -> int;
+  // generate_ambient_occlusion (PBR.cpp:143-311) on the last rendered frame: decode its normals into the plane resolve_shadowmap uses,
+  // then the three GTAO passes on its depth; width x height floats to the host
+  auto generate_ambient_occlusion(const OxcCullCamera& camera, const OxcGtaoCamera& gtao_camera, const OxcGtaoSettings& settings, float* ao_host)
+      -> int;
 
   // RendererInstance::render geometry section: run_geometry_pass(false) -> generate_hiz -> run_geometry_pass(true)
   auto render(const OxcCullCamera& camera, const float* occluder_depth_host, uint32_t* vis32_host, float* depth_host,
@@ -148,6 +152,10 @@ private:
   float* d_occluder_ = nullptr;
   uint32_t* d_overdraw_ = nullptr; // allocated by the first overdraw()
   float* d_gbuffer_ = nullptr;      // four float4 planes of decode_visbuffer, allocated by its first call
+  float* d_uv_normal_ = nullptr;    // uv_normal plane (float4 per pixel) the shadow resolve and the GTAO decode into, allocated by the
+                                    // first of them; kept for the renderer's lifetime
+  void* d_gtao_ = nullptr;          // generate_ambient_occlusion's planes (mips, edges, noisy and final occlusion), allocated by its first call
+  int uv_normal_plane();            // allocates d_uv_normal_ when missing: OXC_OK or OXC_E_CAPACITY
   bool has_external_depth_ = false;
   // transforms as the host last uploaded them, and on the device the values before the upload that last changed each of them
   // (TransformPrevious::previous_world, RendererInstance.cpp:1600-1609)
@@ -164,8 +172,7 @@ private:
     OxcVirtualClipmap clipmaps[10] = {}; // of the last update
     float inv_projection_view[16] = {};  // of the last update
     float resolution[2] = {};
-    float* d_normals = nullptr;          // uv_normal plane of the resolve's decode (float4 per pixel), allocated by its first call
-    float* d_shadow = nullptr;           // the resolve's output
+    float* d_shadow = nullptr;           // the resolve's output, allocated by its first call
   } vsm_;
   // the shadow draw's own context (same scene, transforms and materials as ctx_; max_views >= 10 for the clipmap cull)
   OxcContext* shadow_ctx_ = nullptr;

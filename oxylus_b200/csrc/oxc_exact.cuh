@@ -304,6 +304,73 @@ OXC_DI void canonical_sincos(float xf, float& s_out, float& c_out) {
 OXC_DI float canonical_sin(float x) { float s, c; canonical_sincos(x, s, c); return s; }
 OXC_DI float canonical_cos(float x) { float s, c; canonical_sincos(x, s, c); return c; }
 
+OXC_DI double ddiv64(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __ddiv_rn(a, b);
+#else
+  return a / b;
+#endif
+}
+
+// pow for the GTAO denoise, bit-identical to oracle/oxc_oracle_gtao.c orc_pow_canonical.  Binary64 throughout, one rounding to
+// binary32: x = m * 2^e with m in [sqrt(1/2), sqrt(2)] (taken from the binary32 bits), log m = 2 atanh(t), t = (m - 1) / (m + 1), by
+// its series to t^23; L = e * LN2_HI + (e * LN2_LO + log m); z = y * L clamped to +-1100; exp(z) = 2^k exp(r), k = rint(z / ln 2),
+// r = (z - k * LN2_HI) - k * LN2_LO (LN2_HI has 32 significant bits, so k * LN2_HI is exact), exp(r) by Taylor to r^13, ldexp.
+// Before the rounding the relative error is a few units of 2^-50, so the result is within 1 ulp of the correctly rounded binary32
+// power (it can differ from it only next to a rounding tie).  pow(1, y) = 1 and pow(x, 0) = 1 (NaN included); NaN or x < 0 gives
+// NaN; pow(+-0, y) = 0 for y > 0, +inf for y < 0; pow(inf, y) = inf for y > 0, else 0; y = +-inf by |x| against 1.
+OXC_DI float canonical_pow(float xf, float yf) {
+  if (xf == 1.0f || yf == 0.0f) return 1.0f;
+  if (xf != xf || yf != yf || xf < 0.0f) return __uint_as_float(0x7FC00000u);
+  if (xf == 0.0f) return yf > 0.0f ? 0.0f : __uint_as_float(0x7F800000u);
+  if (xf == __uint_as_float(0x7F800000u)) return yf > 0.0f ? xf : 0.0f;
+  if (fabsf(yf) == __uint_as_float(0x7F800000u)) return (xf < 1.0f) == (yf > 0.0f) ? 0.0f : __uint_as_float(0x7F800000u);
+  int e = 0;
+  float xm = xf;
+  if (xm < 1.17549435e-38f) { xm = fm(xm, 16777216.0f); e = -24; }
+  const uint32_t bits = __float_as_uint(xm);
+  e += (int)(bits >> 23) - 127;
+  float m = __uint_as_float((bits & 0x007FFFFFu) | 0x3F800000u);
+  if (m > 1.41421354f) { m = fm(m, 0.5f); e += 1; }
+  const double md = (double)m;
+  const double t = ddiv64(dadd64(md, -1.0), dadd64(md, 1.0));
+  const double s = dmul64(t, t);
+  double p = 1.0 / 23.0;
+  p = dadd64(1.0 / 21.0, dmul64(s, p));
+  p = dadd64(1.0 / 19.0, dmul64(s, p));
+  p = dadd64(1.0 / 17.0, dmul64(s, p));
+  p = dadd64(1.0 / 15.0, dmul64(s, p));
+  p = dadd64(1.0 / 13.0, dmul64(s, p));
+  p = dadd64(1.0 / 11.0, dmul64(s, p));
+  p = dadd64(1.0 / 9.0, dmul64(s, p));
+  p = dadd64(1.0 / 7.0, dmul64(s, p));
+  p = dadd64(1.0 / 5.0, dmul64(s, p));
+  p = dadd64(1.0 / 3.0, dmul64(s, p));
+  const double u = dmul64(t, 2.0);
+  const double lm = dadd64(u, dmul64(dmul64(u, s), p));
+  const double ed = (double)e;
+  const double L = dadd64(dmul64(ed, 6.93147180369123816490e-01), dadd64(dmul64(ed, 1.90821492927058770002e-10), lm));
+  double z = dmul64((double)yf, L);
+  z = z > 1100.0 ? 1100.0 : (z < -1100.0 ? -1100.0 : z);
+  const double k = rint(dmul64(z, 1.44269504088896338700e+00));
+  const double r = dadd64(dadd64(z, -dmul64(k, 6.93147180369123816490e-01)), -dmul64(k, 1.90821492927058770002e-10));
+  double q = 1.0 / 6227020800.0; // 1/13!
+  q = dadd64(1.0 / 479001600.0, dmul64(r, q));
+  q = dadd64(1.0 / 39916800.0, dmul64(r, q));
+  q = dadd64(1.0 / 3628800.0, dmul64(r, q));
+  q = dadd64(1.0 / 362880.0, dmul64(r, q));
+  q = dadd64(1.0 / 40320.0, dmul64(r, q));
+  q = dadd64(1.0 / 5040.0, dmul64(r, q));
+  q = dadd64(1.0 / 720.0, dmul64(r, q));
+  q = dadd64(1.0 / 120.0, dmul64(r, q));
+  q = dadd64(1.0 / 24.0, dmul64(r, q));
+  q = dadd64(1.0 / 6.0, dmul64(r, q));
+  q = dadd64(0.5, dmul64(r, q));
+  q = dadd64(1.0, dmul64(r, q));
+  const double er = dadd64(1.0, dmul64(r, q));
+  return d2f_rn(ldexp(er, (int)k));
+}
+
 // cull.slang:169-171: determinant(f32x3x3(c0.xyw, c1.xyw, c2.xyw)) >= 0.0001
 OXC_DI bool triangle_backface(float4 c0, float4 c1, float4 c2) {
   const float m00 = c0.x, m01 = c0.y, m02 = c0.w;

@@ -25,6 +25,7 @@
 #include "kernels_vsm.cuh"
 #include "kernels_vsm_draw.cuh"
 #include "kernels_vsm_resolve.cuh"
+#include "kernels_gtao.cuh"
 
 using namespace oxc;
 
@@ -1500,6 +1501,49 @@ int oxc_vsm_resolve_shadows(OxcContext* c, const OxcVsmContext* vsm, const float
   p.texel_length = vsm_first_texel_length(vsm); p.bias = vsm->clipmap_selection_bias; p.z_length = vsm->z_length;
   const dim3 grid((p.width + VSM_RESOLVE_TILE_X - 1) / VSM_RESOLVE_TILE_X, (p.height + VSM_RESOLVE_TILE_Y - 1) / VSM_RESOLVE_TILE_Y);
   k_vsm_resolve_shadows<<<grid, VSM_RESOLVE_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_generate_ambient_occlusion(OxcContext* c, const OxcGtaoCamera* cam, const OxcGtaoSettings* st, const float* depth_dev,
+                                   const float* normals_dev, uint32_t w, uint32_t h, const OxcGtaoTargets* t, void* stream) {
+  if (!c || !cam || !st || !depth_dev || !normals_dev || !t) return fail(OXC_E_INVALID, "null argument");
+  if (!t->depth_mips || !t->edges || !t->noisy_occlusion || !t->ambient_occlusion) return fail(OXC_E_INVALID, "null target");
+  if (w == 0 || h == 0) return fail(OXC_E_INVALID, "empty extent %u x %u", w, h);
+  if (w > 32768u || h > 32768u) return fail(OXC_E_INVALID, "extent %u x %u above 32768", w, h);
+  if (st->slice_count < 1u || st->slice_count > OXC_GTAO_MAX_SLICES)
+    return fail(OXC_E_INVALID, "slice_count %u outside 1..%u", st->slice_count, OXC_GTAO_MAX_SLICES);
+  if (st->samples_per_slice_side < 1u || st->samples_per_slice_side > OXC_GTAO_MAX_SAMPLES_PER_SIDE)
+    return fail(OXC_E_INVALID, "samples_per_slice_side %u outside 1..%u", st->samples_per_slice_side, OXC_GTAO_MAX_SAMPLES_PER_SIDE);
+  if (reinterpret_cast<uintptr_t>(normals_dev) & 15u) return fail(OXC_E_INVALID, "normals_dev is not 16-byte aligned (float4 per pixel)");
+  if ((reinterpret_cast<uintptr_t>(depth_dev) | reinterpret_cast<uintptr_t>(t->depth_mips) | reinterpret_cast<uintptr_t>(t->edges) |
+       reinterpret_cast<uintptr_t>(t->ambient_occlusion)) & 3u)
+    return fail(OXC_E_INVALID, "depth_dev, depth_mips, edges and ambient_occlusion must be 4-byte aligned");
+  if (reinterpret_cast<uintptr_t>(t->noisy_occlusion) & 1u) return fail(OXC_E_INVALID, "noisy_occlusion is not 2-byte aligned");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  GtaoParams p{};
+  p.depth = depth_dev; p.normals = reinterpret_cast<const float4*>(normals_dev);
+  p.mips = t->depth_mips; p.edges = t->edges; p.noisy = t->noisy_occlusion; p.ao = t->ambient_occlusion;
+  p.width = (int)w; p.height = (int)h;
+  long long off = 0;
+  for (int k = 0; k < GTAO_LEVELS; k++) {
+    p.mip_w[k] = (int)((w >> k) > 1u ? (w >> k) : 1u); p.mip_h[k] = (int)((h >> k) > 1u ? (h >> k) : 1u);
+    p.mip_off[k] = off;
+    off += (long long)p.mip_w[k] * p.mip_h[k];
+  }
+  p.m23 = cam->projection[14]; p.m22 = cam->projection[10]; p.p00 = cam->projection[0]; p.p11 = cam->projection[5];
+  for (int i = 0; i < 3; i++) p.view_row[i] = make_float4(cam->view[i], cam->view[4 + i], cam->view[8 + i], cam->view[12 + i]);
+  p.far_clip = cam->far_clip;
+  p.thickness = st->thickness; p.effect_radius = st->effect_radius; p.final_power = st->final_power;
+  p.slice_count = st->slice_count; p.samples_per_slice_side = st->samples_per_slice_side; p.noise_index = st->noise_index;
+  const dim3 pre((w + 2 * GTAO_PREFILTER_SIDE - 1) / (2 * GTAO_PREFILTER_SIDE), (h + 2 * GTAO_PREFILTER_SIDE - 1) / (2 * GTAO_PREFILTER_SIDE));
+  k_gtao_prefilter<<<pre, dim3(GTAO_PREFILTER_SIDE, GTAO_PREFILTER_SIDE), 0, s>>>(p);
+  LAUNCHED();
+  const dim3 grid((w + GTAO_TILE_X - 1) / GTAO_TILE_X, (h + GTAO_TILE_Y - 1) / GTAO_TILE_Y);
+  k_gtao_main<<<grid, GTAO_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  k_gtao_denoise<<<grid, GTAO_THREADS, 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }

@@ -86,13 +86,19 @@ def mat_mul_cm(a16, b16):
     return (a @ b).T.astype(np.float32).reshape(16)
 
 
-def make_camera(width, height, mesh_instance_count, yaw_deg=0.0, eye=(0.0, 0.0, 0.0), fov=60.0, near=0.1, far=1000.0):
-    """CullCamera as RendererInstance::render fills it (RendererInstance.cpp:783-790)."""
-    cam = np.zeros(1, dtype=abi.CULL_CAMERA_DT)
+def camera_matrices(width, height, yaw_deg=0.0, eye=(0.0, 0.0, 0.0), fov=60.0, near=0.1, far=1000.0):
+    """(projection, view), column-major 16 floats each: the two matrices make_camera multiplies into projection_view"""
     yaw = np.radians(yaw_deg)
     fwd = np.array([-np.sin(yaw), 0.0, -np.cos(yaw)])
     view = look_at(eye, np.asarray(eye) + fwd, (0.0, 1.0, 0.0))
     proj = perspective_reverse_z(fov, width / height, near, far)
+    return proj, view
+
+
+def make_camera(width, height, mesh_instance_count, yaw_deg=0.0, eye=(0.0, 0.0, 0.0), fov=60.0, near=0.1, far=1000.0):
+    """CullCamera as RendererInstance::render fills it (RendererInstance.cpp:783-790)."""
+    cam = np.zeros(1, dtype=abi.CULL_CAMERA_DT)
+    proj, view = camera_matrices(width, height, yaw_deg, eye, fov, near, far)
     cam["projection_view"][0] = mat_mul_cm(proj, view)
     cam["position"][0] = eye
     cam["acceptable_lod_error"] = 2.0  # RendererInstance.cpp:1394
