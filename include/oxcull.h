@@ -869,6 +869,97 @@ OXC_STATIC_ASSERT(sizeof(OxcGtaoTargets) == 32, "GtaoTargets");
 int oxc_generate_ambient_occlusion(OxcContext* ctx, const OxcGtaoCamera* camera, const OxcGtaoSettings* settings, const float* depth_dev,
                                    const float* normals_dev, uint32_t width, uint32_t height, const OxcGtaoTargets* targets, void* stream);
 
+/* Lighting: the pbr_apply_no_atmos variant of RendererInstance::apply_pbr (Passes/PBR.cpp:435-531, passes/pbr_apply_no_atmos.slang
+ * :23-127 with the pbr.slang:1-172 functions it calls).  One float4 (RGBA) per pixel of a width x height frame, row-major, into out_dev,
+ * from caller-owned device planes; no scratch, so the call is graph-capturable from its first call.  Inputs (OxcPbrInputs):
+ *   depth (D32F, reversed Z, 0 = sky); albedo, normal, emissive, metallic_roughness_occlusion: float4 per pixel as oxc_decode_gbuffer
+ *   writes them (normal = oct(normal-mapped normal) in .xy, oct(world normal) in .zw); optional, NULL reads as 1.0 (the reference clears
+ *   both attachments to White): ambient_occlusion (f32, as oxc_generate_ambient_occlusion writes it) and shadow (f32, as
+ *   oxc_vsm_resolve_shadows writes it); contact_shadow (f32), read only under OXC_SCENE_HAS_CONTACT_SHADOWS and then required.
+ * lights_dev: settings->light_count OxcLight records (the reference's lights buffer), 16-byte aligned, summed in index order.
+ * Refused with OXC_E_INVALID: a NULL required argument or plane, NULL lights with light_count > 0, a NULL contact plane under
+ * OXC_SCENE_HAS_CONTACT_SHADOWS, a zero extent or one above 32768, light_count > OXC_MAX_LIGHTS (the reference uploads at most 256),
+ * OXC_SCENE_HAS_ATMOSPHERE (that variant needs the sky LUTs), float4 planes, out_dev or lights_dev not 16-byte aligned, f32 planes not
+ * 4-byte aligned.  The other flag bits (bloom, FXAA, ...) are ignored, as the shader ignores them.
+ * SPECIFICATION (oracle/oxc_oracle_pbr.c orc_apply_pbr, bit for bit): IEEE binary32, no contraction, IEEE divide / sqrt, products and
+ * sums left to right as written, dot(a, b) = (a.x*b.x + a.y*b.y) + a.z*b.z, mul(M, v) row by row in the same order (+ M[i][3] * 1.0),
+ * normalize(v) = v / sqrt(dot(v, v)), length(v) = sqrt(dot(v, v)), lerp(a, b, t) = a + (b - a) * t, reflect(i, n) = i - (2 * n) *
+ * dot(i, n), max / min return the other operand for a NaN, clamp(x, a, b) = min(max(x, a), b), saturate(NaN) = 0, smoothstep(e0, e1, x)
+ * = (t * t) * (3 - 2 * t) with t = saturate((x - e0) / (e1 - e0)); constants are the binary32 roundings of the shader's literals;
+ * Fd_Lambert = fl(1 / fl(pi)).  Commitments where the shader leaves the outcome open:
+ *   1. pixel centre: tex_coord = ((x + 0.5) / W, (y + 0.5) / H); the albedo's SampleLevel at a pixel centre has bilinear weights of
+ *      exactly 0, so it is the pixel's own texel.
+ *   2. the normal plane's four components are rounded to binary16 (R16G16B16A16F, round to nearest even); both oct_to_vec3
+ *      (common/encoding.slang:7-15, which normalizes) follow the written order; N is normalized a second time, as written.
+ *   3. the ambient occlusion is rounded to binary16 (R16F); albedo, emissive, metallic / roughness / occlusion, shadow and contact
+ *      shadow are read as the binary32 values given (deviation: the reference stores the first three as RGBA8 sRGB, B10G11R11 and
+ *      RGBA8 unorm, conversions that are not bit-defined).
+ *   4. cos of the cone angles: canonical_sincos; exp2(-16 r - 1) = canonical_pow(2, .); pow(NoV + ao, .) = canonical_pow;
+ *      pow(., 5.0) of F_Schlick = canonical_pow5 (oxc_exact.cuh: binary64 x^2, (x^2 * x^2) * x, one rounding; within 1 ulp).
+ *   5. a light kind other than OXC_LIGHT_POINT / OXC_LIGHT_SPOT contributes nothing (the shader's if / else if).
+ *   6. early returns in shader order: OXC_SCENE_TRANSPARENT_BACKGROUND and depth == 0 gives (0, 0, 0, 0); then OXC_SCENE_HAS_SKY and
+ *      depth == 0 gives sky_has_texture ? (1, 1, 1, 1) : sky_solid_color; otherwise the full computation runs, also on sky pixels
+ *      without OXC_SCENE_HAS_SKY, with whatever non-finite values follow.
+ *   7. output: binary32 RGBA, the value before the reference's B10G11R11 / RGBA16F store (deviation); every NaN is written as
+ *      0x7FFFFFFF.  Hostile planes, lights and settings (NaN, Inf, denormals) do not fault and follow the same rules. */
+#define OXC_MAX_LIGHTS 256u                          /* GPU::MAX_LIGHTS */
+#define OXC_SCENE_HAS_DIRECTIONAL_LIGHT (1u << 0)     /* SceneFlags, SceneGPU.hpp:253-267 */
+#define OXC_SCENE_HAS_ATMOSPHERE (1u << 1)
+#define OXC_SCENE_HAS_EYE_ADAPTATION (1u << 2)
+#define OXC_SCENE_HAS_BLOOM (1u << 3)
+#define OXC_SCENE_HAS_FXAA (1u << 4)
+#define OXC_SCENE_HAS_GTAO (1u << 5)
+#define OXC_SCENE_HAS_FILM_GRAIN (1u << 6)
+#define OXC_SCENE_HAS_CHROMATIC_ABERRATION (1u << 7)
+#define OXC_SCENE_HAS_VIGNETTE (1u << 8)
+#define OXC_SCENE_HAS_CONTACT_SHADOWS (1u << 9)
+#define OXC_SCENE_HAS_SKY (1u << 10)
+#define OXC_SCENE_TRANSPARENT_BACKGROUND (1u << 11)
+#define OXC_LIGHT_DIRECTIONAL 0u                     /* LightKind */
+#define OXC_LIGHT_POINT 1u
+#define OXC_LIGHT_SPOT 2u
+typedef struct OxcLight {          /* GPU::Light, SceneGPU.hpp:241-251 */
+  float position[3];
+  float intensity;
+  float color[3];
+  float range;                     /* <= 0: no window, 1 / (d^2 + 0.1) */
+  float direction[3];              /* spot only, normalized by the pass */
+  float inner_cone_angle;          /* spot only, radians */
+  float outer_cone_angle;          /* spot only, radians */
+  uint32_t kind;                   /* OXC_LIGHT_* */
+  uint32_t pad[2];
+} OxcLight;
+typedef struct OxcPbrSettings {    /* the pass's specialization constant and push constants (PBR.cpp:436-486) */
+  uint32_t scene_flags;            /* OXC_SCENE_* */
+  float sun_direction[3];          /* L, used as given */
+  float sun_intensity;             /* Li */
+  float base_ambient_color[3];     /* the reference passes 0.03 */
+  float sky_solid_color[4];        /* Sky (scene.slang:236-240) */
+  float sky_ambient_color[3];
+  uint32_t sky_has_texture;
+  uint32_t light_count;            /* 0..OXC_MAX_LIGHTS */
+} OxcPbrSettings;
+typedef struct OxcPbrCamera {      /* the Camera fields the pass reads (scene.slang:162-188) */
+  float inv_projection_view[16];   /* column-major, as Camera::inv_projection_view */
+  float position[3];
+} OxcPbrCamera;
+typedef struct OxcPbrInputs {      /* device planes, W x H, row-major */
+  const float* depth;              /* required, f32 */
+  const float* albedo;             /* required, float4 */
+  const float* normal;             /* required, float4 */
+  const float* emissive;           /* required, float4 */
+  const float* metallic_roughness_occlusion; /* required, float4 */
+  const float* ambient_occlusion;  /* optional (NULL = 1.0), f32 rounded to binary16 */
+  const float* shadow;             /* optional (NULL = 1.0), f32, read under OXC_SCENE_HAS_DIRECTIONAL_LIGHT */
+  const float* contact_shadow;     /* f32, read (and required) only under OXC_SCENE_HAS_CONTACT_SHADOWS */
+} OxcPbrInputs;
+OXC_STATIC_ASSERT(sizeof(OxcLight) == 64, "Light");
+OXC_STATIC_ASSERT(sizeof(OxcPbrSettings) == 68, "PbrSettings");
+OXC_STATIC_ASSERT(sizeof(OxcPbrCamera) == 76, "PbrCamera");
+OXC_STATIC_ASSERT(sizeof(OxcPbrInputs) == 64, "PbrInputs");
+int oxc_apply_pbr(OxcContext* ctx, const OxcPbrCamera* camera, const OxcPbrSettings* settings, const OxcLight* lights_dev,
+                  const OxcPbrInputs* inputs, uint32_t width, uint32_t height, float* out_dev, void* stream);
+
 int oxc_get_outputs(OxcContext* ctx, OxcOutputs* out);
 /* Instrumentation hook: 128 u64 counters that builds with -DOXC_RASTER_STATS fill (tools/raster_stats.py); zero otherwise. */
 void* oxc_debug_stats_ptr(OxcContext* ctx);
@@ -994,6 +1085,21 @@ int oxr_decode_gbuffer(OxrRenderer* r, const OxcCullCamera* camera, float* albed
  * OXC_E_CAPACITY, with the camera path left usable, when the planes cannot be allocated. */
 int oxr_generate_ambient_occlusion(OxrRenderer* r, const OxcCullCamera* camera, const OxcGtaoCamera* gtao_camera,
                                    const OxcGtaoSettings* settings, float* ao_host);
+/* RendererInstance::apply_pbr (PBR.cpp:435-531, no atmosphere) with the passes before it, on the frame oxr_render / oxr_wait completed
+ * last, on the renderer's stream, synchronous:
+ *   1. the G-buffer decode with `camera` and the table of the last oxr_set_materials (as oxr_decode_gbuffer);
+ *   2. cast_shadows != 0: the shadow resolve with the state of the last oxr_vsm_update_pages / oxr_vsm_draw_shadows (OXC_E_STATE
+ *      without one); otherwise the shadow plane reads 1, as the reference's without cast_shadows;
+ *   3. OXC_SCENE_HAS_GTAO: oxc_generate_ambient_occlusion with gtao_camera and gtao_settings (both required then);
+ *   4. oxc_apply_pbr with pbr_camera, settings and settings->light_count records of lights_host, uploaded into a renderer-owned
+ *      OXC_MAX_LIGHTS-record buffer.
+ * The resolve and the GTAO read the G-buffer's normal plane (its .zw equals oxc_decode_visbuffer's uv_normal.zw).  width x height
+ * float4 to rgba_host.  OXC_SCENE_HAS_CONTACT_SHADOWS is refused (OXC_E_INVALID) until there is a contact-shadow pass.  The planes
+ * (G-buffer, resolve, GTAO, about 100 B / pixel, and 16 B / pixel of output) are allocated at the first call that needs them;
+ * OXC_E_CAPACITY, with the camera path left usable, when they cannot be.  The frame's outputs are left as they were. */
+int oxr_apply_pbr(OxrRenderer* r, const OxcCullCamera* camera, const OxcPbrCamera* pbr_camera, const OxcPbrSettings* settings,
+                  const OxcLight* lights_host, int cast_shadows, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* gtao_settings,
+                  float* rgba_host);
 
 /* ------------------------------------------------------------------------------------------------
  * oxb_* — mesh builder (SURVEY §8f.2): host-side producer of the blob layout above, mirroring build_gltf_mesh

@@ -361,6 +361,78 @@ def gtao_mip_layout(width, height):
     return out, off
 
 
+MAX_LIGHTS = 256  # GPU::MAX_LIGHTS
+# SceneFlags (SceneGPU.hpp:253-267)
+SCENE_HAS_DIRECTIONAL_LIGHT = 1 << 0
+SCENE_HAS_ATMOSPHERE = 1 << 1
+SCENE_HAS_EYE_ADAPTATION = 1 << 2
+SCENE_HAS_BLOOM = 1 << 3
+SCENE_HAS_FXAA = 1 << 4
+SCENE_HAS_GTAO = 1 << 5
+SCENE_HAS_FILM_GRAIN = 1 << 6
+SCENE_HAS_CHROMATIC_ABERRATION = 1 << 7
+SCENE_HAS_VIGNETTE = 1 << 8
+SCENE_HAS_CONTACT_SHADOWS = 1 << 9
+SCENE_HAS_SKY = 1 << 10
+SCENE_TRANSPARENT_BACKGROUND = 1 << 11
+# LightKind
+LIGHT_DIRECTIONAL, LIGHT_POINT, LIGHT_SPOT = 0, 1, 2
+
+
+class Light(C.Structure):
+    """OxcLight (GPU::Light, SceneGPU.hpp:241-251)"""
+
+    _fields_ = [("position", C.c_float * 3), ("intensity", C.c_float), ("color", C.c_float * 3), ("range", C.c_float), ("direction", C.c_float * 3),
+                ("inner_cone_angle", C.c_float), ("outer_cone_angle", C.c_float), ("kind", C.c_uint32), ("pad", C.c_uint32 * 2)]
+
+
+class PbrSettings(C.Structure):
+    """OxcPbrSettings: scene flags, sun direction and intensity, base ambient colour, the Sky record and the light count"""
+
+    _fields_ = [("scene_flags", C.c_uint32), ("sun_direction", C.c_float * 3), ("sun_intensity", C.c_float), ("base_ambient_color", C.c_float * 3),
+                ("sky_solid_color", C.c_float * 4), ("sky_ambient_color", C.c_float * 3), ("sky_has_texture", C.c_uint32), ("light_count", C.c_uint32)]
+
+
+class PbrCamera(C.Structure):
+    """OxcPbrCamera: Camera::inv_projection_view (column-major) and the camera position"""
+
+    _fields_ = [("inv_projection_view", C.c_float * 16), ("position", C.c_float * 3)]
+
+
+class PbrInputs(C.Structure):
+    """OxcPbrInputs: device pointers of depth, albedo, normal, emissive, metallic/roughness/occlusion, ambient occlusion, shadow and contact
+    shadow"""
+
+    _fields_ = [(k, C.c_void_p) for k in ("depth", "albedo", "normal", "emissive", "metallic_roughness_occlusion", "ambient_occlusion", "shadow",
+                                          "contact_shadow")]
+
+
+assert C.sizeof(Light) == 64 and C.sizeof(PbrSettings) == 68 and C.sizeof(PbrCamera) == 76 and C.sizeof(PbrInputs) == 64
+PBR_INPUTS = tuple(k for k, _ in PbrInputs._fields_)
+
+
+def pbr_settings(scene_flags=SCENE_HAS_DIRECTIONAL_LIGHT | SCENE_HAS_GTAO, sun_direction=(0.3, 0.8, 0.52), sun_intensity=10.0, base_ambient=0.03,
+                 sky_solid_color=(0.0, 0.0, 0.0, 1.0), sky_ambient_color=(0.0, 0.0, 0.0), sky_has_texture=False, light_count=0):
+    """PbrSettings as apply_pbr fills them (PBR.cpp:436-486: base ambient 0.03, DirectionalLight::intensity 10 by default)"""
+    s = PbrSettings()
+    s.scene_flags = int(scene_flags)
+    s.sun_direction[:] = [float(np.float32(v)) for v in sun_direction]
+    s.sun_intensity = float(sun_intensity)
+    s.base_ambient_color[:] = [float(np.float32(base_ambient))] * 3 if np.isscalar(base_ambient) else [float(v) for v in base_ambient]
+    s.sky_solid_color[:] = [float(v) for v in sky_solid_color]
+    s.sky_ambient_color[:] = [float(v) for v in sky_ambient_color]
+    s.sky_has_texture = int(bool(sky_has_texture))
+    s.light_count = int(light_count)
+    return s
+
+
+def pbr_camera(inv_projection_view, position):
+    c = PbrCamera()
+    c.inv_projection_view[:] = [float(x) for x in np.asarray(inv_projection_view, dtype=np.float32).reshape(16)]
+    c.position[:] = [float(x) for x in np.asarray(position, dtype=np.float32).reshape(3)]
+    return c
+
+
 MESH_MAX_LODS = 8
 
 

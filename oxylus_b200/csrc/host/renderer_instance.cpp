@@ -102,7 +102,7 @@ RendererInstance::RendererInstance(int device, const OxcCreateInfo& info, uint32
 RendererInstance::~RendererInstance() {
   if (stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(stream_));
   cudaFree(d_vis64_); cudaFree(d_vis32_); cudaFree(d_depth_); cudaFree(d_occluder_); cudaFree(d_overdraw_); cudaFree(d_gbuffer_);
-  cudaFree(d_uv_normal_); cudaFree(d_gtao_);
+  cudaFree(d_uv_normal_); cudaFree(d_gtao_); cudaFree(d_pbr_); cudaFree(d_lights_);
   if (h_pinned_) cudaFreeHost(h_pinned_);
   if (copy_stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(copy_stream_));
   for (auto& sl : slots_) {
@@ -296,23 +296,36 @@ auto RendererInstance::resolve_shadowmap(const OxcCullCamera& camera, float* sha
   const size_t px = (size_t)width_ * height_;
   // the resolve's own planes are an optional part, as the shadow draw's context is: without room for them the camera path stays
   // usable and this call returns OXC_E_CAPACITY (the sticky error is not set)
-  if (uv_normal_plane() != OXC_OK) return OXC_E_CAPACITY;
-  if (!vsm_.d_shadow && cudaMalloc(reinterpret_cast<void**>(&vsm_.d_shadow), px * 4) != cudaSuccess) {
-    cudaGetLastError(); // clear the allocation error so that the next launch check does not report it
-    vsm_.d_shadow = nullptr;
-    return OXC_E_CAPACITY;
-  }
-  const OxrVsmPages& v = vsm_.pages;
+  if (uv_normal_plane() != OXC_OK || shadow_plane() != OXC_OK) return OXC_E_CAPACITY;
   int rc;
   if ((rc = oxc_bind_camera_buffer(ctx_, nullptr)) != OXC_OK) return fail(rc); // as render(): the camera comes from the argument
   OxcDecodeTargets targets{};
   targets.uv_normal = d_uv_normal_;
   if ((rc = oxc_decode_visbuffer(ctx_, &camera, d_vis64_, nullptr, width_, height_, &targets, stream_)) != OXC_OK) return fail(rc);
-  if ((rc = oxc_resolve_visbuffer(ctx_, d_vis64_, width_, height_, nullptr, d_depth_, stream_)) != OXC_OK) return fail(rc);
-  if ((rc = oxc_vsm_resolve_shadows(ctx_, &vsm_.shape, vsm_.inv_projection_view, vsm_.resolution, vsm_.clipmaps, d_depth_, d_uv_normal_,
-                                    v.page_tables, v.physical_atlas, vsm_.d_shadow, stream_)) != OXC_OK) return fail(rc);
+  if ((rc = resolve_shadowmap_device(d_uv_normal_)) != OXC_OK) return rc;
   if (cudaMemcpyAsync(shadow_host, vsm_.d_shadow, px * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
     return fail(OXC_E_CUDA);
+  return OXC_OK;
+}
+
+int RendererInstance::shadow_plane() {
+  if (vsm_.d_shadow) return OXC_OK;
+  if (cudaMalloc(reinterpret_cast<void**>(&vsm_.d_shadow), (size_t)width_ * height_ * 4) != cudaSuccess) {
+    cudaGetLastError(); // clear the allocation error so that the next launch check does not report it
+    vsm_.d_shadow = nullptr;
+    return OXC_E_CAPACITY;
+  }
+  return OXC_OK;
+}
+
+// the frame's depth, then the fullscreen resolve into vsm_.d_shadow with the VSM state of the last update, from `normals` (float4 per
+// pixel, oct(world normal) in .zw), enqueued on stream_
+int RendererInstance::resolve_shadowmap_device(const float* normals) {
+  const OxrVsmPages& v = vsm_.pages;
+  int rc;
+  if ((rc = oxc_resolve_visbuffer(ctx_, d_vis64_, width_, height_, nullptr, d_depth_, stream_)) != OXC_OK) return fail(rc);
+  if ((rc = oxc_vsm_resolve_shadows(ctx_, &vsm_.shape, vsm_.inv_projection_view, vsm_.resolution, vsm_.clipmaps, d_depth_, normals,
+                                    v.page_tables, v.physical_atlas, vsm_.d_shadow, stream_)) != OXC_OK) return fail(rc);
   return OXC_OK;
 }
 
@@ -324,24 +337,38 @@ auto RendererInstance::decode_visbuffer(const OxcCullCamera& camera, float* albe
   cudaStream_t s = static_cast<cudaStream_t>(stream_);
   const size_t px = (size_t)width_ * height_;
   // the planes are an optional part, as the resolve's are: without room for them the camera path stays usable
-  if (!d_gbuffer_ && cudaMalloc(reinterpret_cast<void**>(&d_gbuffer_), px * 64) != cudaSuccess) {
-    cudaGetLastError(); // clear the allocation error so that the next launch check does not report it
-    d_gbuffer_ = nullptr;
-    return OXC_E_CAPACITY;
-  }
+  if (gbuffer_planes() != OXC_OK) return OXC_E_CAPACITY;
   float* const host[4] = {albedo_host, normal_host, emissive_host, mro_host};
   OxcGBufferTargets targets{};
   float** const dev[4] = {&targets.albedo, &targets.normal, &targets.emissive, &targets.metallic_roughness_occlusion};
   for (int k = 0; k < 4; k++) *dev[k] = host[k] ? d_gbuffer_ + (size_t)k * px * 4 : nullptr;
-  int rc;
-  if ((rc = oxc_bind_camera_buffer(ctx_, nullptr)) != OXC_OK) return fail(rc); // as render(): the camera comes from the argument
-  if (cudaMemsetAsync(d_gbuffer_, 0, px * 64, s) != cudaSuccess) return fail(OXC_E_CUDA); // discarded pixels: the cleared attachment
-  rc = oxc_decode_gbuffer(ctx_, &camera, d_vis64_, nullptr, width_, height_, &targets, stream_);
-  if (rc == OXC_E_STATE || rc == OXC_E_INVALID) return rc; // no or unreadable material table: the frame state is intact
-  if (rc != OXC_OK) return fail(rc);
+  const int rc = decode_gbuffer_device(camera, targets);
+  if (rc != OXC_OK) return rc;
   for (int k = 0; k < 4; k++)
     if (host[k] && cudaMemcpyAsync(host[k], *dev[k], px * 16, cudaMemcpyDeviceToHost, s) != cudaSuccess) return fail(OXC_E_CUDA);
   if (cudaStreamSynchronize(s) != cudaSuccess) return fail(OXC_E_CUDA);
+  return OXC_OK;
+}
+
+int RendererInstance::gbuffer_planes() {
+  if (d_gbuffer_) return OXC_OK;
+  if (cudaMalloc(reinterpret_cast<void**>(&d_gbuffer_), (size_t)width_ * height_ * 64) != cudaSuccess) {
+    cudaGetLastError(); // clear the allocation error so that the next launch check does not report it
+    d_gbuffer_ = nullptr;
+    return OXC_E_CAPACITY;
+  }
+  return OXC_OK;
+}
+
+// the cleared attachments, then the G-buffer decode of the last frame into `targets` (planes of d_gbuffer_), enqueued on stream_
+int RendererInstance::decode_gbuffer_device(const OxcCullCamera& camera, const OxcGBufferTargets& targets) {
+  int rc;
+  if ((rc = oxc_bind_camera_buffer(ctx_, nullptr)) != OXC_OK) return fail(rc); // as render(): the camera comes from the argument
+  if (cudaMemsetAsync(d_gbuffer_, 0, (size_t)width_ * height_ * 64, static_cast<cudaStream_t>(stream_)) != cudaSuccess)
+    return fail(OXC_E_CUDA); // discarded pixels: the cleared attachment
+  rc = oxc_decode_gbuffer(ctx_, &camera, d_vis64_, nullptr, width_, height_, &targets, stream_);
+  if (rc == OXC_E_STATE || rc == OXC_E_INVALID) return rc; // no or unreadable material table: the frame state is intact
+  if (rc != OXC_OK) return fail(rc);
   return OXC_OK;
 }
 
@@ -363,30 +390,98 @@ auto RendererInstance::generate_ambient_occlusion(const OxcCullCamera& camera, c
   if (!ao_host) return OXC_E_INVALID;
   cudaStream_t s = static_cast<cudaStream_t>(stream_);
   const size_t px = (size_t)width_ * height_;
-  size_t mip_texels = 0;
-  for (uint32_t k = 0; k < 5; k++) mip_texels += (size_t)std::max(1u, width_ >> k) * std::max(1u, height_ >> k);
   // the planes are an optional part, as the resolve's are: without room for them the camera path stays usable
-  if (uv_normal_plane() != OXC_OK) return OXC_E_CAPACITY;
-  if (!d_gtao_ && cudaMalloc(&d_gtao_, mip_texels * 4 + px * 10) != cudaSuccess) {
-    cudaGetLastError();
-    d_gtao_ = nullptr;
-    return OXC_E_CAPACITY;
-  }
-  OxcGtaoTargets targets{};
-  targets.depth_mips = static_cast<float*>(d_gtao_);
-  targets.edges = reinterpret_cast<uint32_t*>(targets.depth_mips + mip_texels);
-  targets.ambient_occlusion = reinterpret_cast<float*>(targets.edges + px);
-  targets.noisy_occlusion = reinterpret_cast<uint16_t*>(targets.ambient_occlusion + px);
+  if (uv_normal_plane() != OXC_OK || gtao_planes() != OXC_OK) return OXC_E_CAPACITY;
   int rc;
   if ((rc = oxc_bind_camera_buffer(ctx_, nullptr)) != OXC_OK) return fail(rc); // as render(): the camera comes from the argument
   OxcDecodeTargets decode{};
   decode.uv_normal = d_uv_normal_;
   if ((rc = oxc_decode_visbuffer(ctx_, &camera, d_vis64_, nullptr, width_, height_, &decode, stream_)) != OXC_OK) return fail(rc);
+  OxcGtaoTargets targets;
+  if ((rc = generate_ambient_occlusion_device(gtao_camera, settings, d_uv_normal_, &targets)) != OXC_OK) return rc;
+  if (cudaMemcpyAsync(ao_host, targets.ambient_occlusion, px * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
+    return fail(OXC_E_CUDA);
+  return OXC_OK;
+}
+
+size_t RendererInstance::gtao_mip_texels() const {
+  size_t mip_texels = 0;
+  for (uint32_t k = 0; k < 5; k++) mip_texels += (size_t)std::max(1u, width_ >> k) * std::max(1u, height_ >> k);
+  return mip_texels;
+}
+
+int RendererInstance::gtao_planes() {
+  if (d_gtao_) return OXC_OK;
+  if (cudaMalloc(&d_gtao_, gtao_mip_texels() * 4 + (size_t)width_ * height_ * 10) != cudaSuccess) {
+    cudaGetLastError();
+    d_gtao_ = nullptr;
+    return OXC_E_CAPACITY;
+  }
+  return OXC_OK;
+}
+
+// the frame's depth, then prefilter, sector pass and denoise into the renderer's own planes from `normals` (float4 per pixel, oct(world
+// normal) in .zw), enqueued on stream_; *targets receives the planes
+int RendererInstance::generate_ambient_occlusion_device(const OxcGtaoCamera& gtao_camera, const OxcGtaoSettings& settings, const float* normals,
+                                                        OxcGtaoTargets* targets) {
+  const size_t px = (size_t)width_ * height_;
+  *targets = OxcGtaoTargets{};
+  targets->depth_mips = static_cast<float*>(d_gtao_);
+  targets->edges = reinterpret_cast<uint32_t*>(targets->depth_mips + gtao_mip_texels());
+  targets->ambient_occlusion = reinterpret_cast<float*>(targets->edges + px);
+  targets->noisy_occlusion = reinterpret_cast<uint16_t*>(targets->ambient_occlusion + px);
+  int rc;
   if ((rc = oxc_resolve_visbuffer(ctx_, d_vis64_, width_, height_, nullptr, d_depth_, stream_)) != OXC_OK) return fail(rc);
-  rc = oxc_generate_ambient_occlusion(ctx_, &gtao_camera, &settings, d_depth_, d_uv_normal_, width_, height_, &targets, stream_);
+  rc = oxc_generate_ambient_occlusion(ctx_, &gtao_camera, &settings, d_depth_, normals, width_, height_, targets, stream_);
   if (rc == OXC_E_INVALID) return rc; // refused settings: nothing was launched, the frame state is intact
   if (rc != OXC_OK) return fail(rc);
-  if (cudaMemcpyAsync(ao_host, targets.ambient_occlusion, px * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
+  return OXC_OK;
+}
+
+// apply_pbr (PBR.cpp:435-531, no atmosphere) on stream_, synchronous, with the passes before it in RendererInstance::render: the
+// G-buffer of the last frame, the shadow resolve and the GTAO on its normal plane (whose .zw is the vis decode's uv_normal.zw), then
+// the lighting into the renderer's output plane
+auto RendererInstance::apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera& pbr_camera, const OxcPbrSettings& settings, const OxcLight* lights_host,
+                                 bool cast_shadows, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* gtao_settings, float* rgba_host) -> int {
+  if (!ctx_ || !error_.empty()) return OXC_E_STATE;
+  const bool gtao = (settings.scene_flags & OXC_SCENE_HAS_GTAO) != 0;
+  if (!rgba_host || (gtao && (!gtao_camera || !gtao_settings)) || (settings.light_count > 0 && !lights_host)) return OXC_E_INVALID;
+  if (settings.light_count > OXC_MAX_LIGHTS || (settings.scene_flags & (OXC_SCENE_HAS_ATMOSPHERE | OXC_SCENE_HAS_CONTACT_SHADOWS)))
+    return OXC_E_INVALID; // no atmosphere variant and no contact-shadow pass: refused before anything is enqueued
+  if (cast_shadows && !vsm_.updated) return OXC_E_STATE;
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  const size_t px = (size_t)width_ * height_;
+  // the planes are an optional part, as the other passes' are: without room for them the camera path stays usable
+  if (gbuffer_planes() != OXC_OK || (cast_shadows && shadow_plane() != OXC_OK) || (gtao && gtao_planes() != OXC_OK)) return OXC_E_CAPACITY;
+  if (!d_pbr_ && (cudaMalloc(reinterpret_cast<void**>(&d_pbr_), px * 16) != cudaSuccess ||
+                  cudaMalloc(reinterpret_cast<void**>(&d_lights_), OXC_MAX_LIGHTS * sizeof(OxcLight)) != cudaSuccess)) {
+    cudaGetLastError();
+    cudaFree(d_pbr_); d_pbr_ = nullptr;
+    return OXC_E_CAPACITY;
+  }
+  OxcGBufferTargets gb{};
+  gb.albedo = d_gbuffer_; gb.normal = d_gbuffer_ + px * 4; gb.emissive = d_gbuffer_ + px * 8; gb.metallic_roughness_occlusion = d_gbuffer_ + px * 12;
+  int rc;
+  if ((rc = decode_gbuffer_device(camera, gb)) != OXC_OK) return rc;
+  OxcPbrInputs in{};
+  in.albedo = gb.albedo; in.normal = gb.normal; in.emissive = gb.emissive; in.metallic_roughness_occlusion = gb.metallic_roughness_occlusion;
+  if (cast_shadows) {
+    if ((rc = resolve_shadowmap_device(gb.normal)) != OXC_OK) return rc;
+    in.shadow = vsm_.d_shadow;
+  }
+  if (gtao) {
+    OxcGtaoTargets t;
+    if ((rc = generate_ambient_occlusion_device(*gtao_camera, *gtao_settings, gb.normal, &t)) != OXC_OK) return rc;
+    in.ambient_occlusion = t.ambient_occlusion;
+  }
+  if ((rc = oxc_resolve_visbuffer(ctx_, d_vis64_, width_, height_, nullptr, d_depth_, stream_)) != OXC_OK) return fail(rc);
+  in.depth = d_depth_;
+  if (settings.light_count &&
+      cudaMemcpyAsync(d_lights_, lights_host, settings.light_count * sizeof(OxcLight), cudaMemcpyHostToDevice, s) != cudaSuccess)
+    return fail(OXC_E_CUDA);
+  rc = oxc_apply_pbr(ctx_, &pbr_camera, &settings, d_lights_, &in, width_, height_, d_pbr_, stream_);
+  if (rc != OXC_OK) return fail(rc);
+  if (cudaMemcpyAsync(rgba_host, d_pbr_, px * 16, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
     return fail(OXC_E_CUDA);
   return OXC_OK;
 }
@@ -885,6 +980,13 @@ int oxr_generate_ambient_occlusion(OxrRenderer* r, const OxcCullCamera* camera, 
                                    float* ao_host) {
   if (!r || !camera || !gtao_camera || !settings) return OXC_E_INVALID;
   return r->impl.generate_ambient_occlusion(*camera, *gtao_camera, *settings, ao_host);
+}
+
+int oxr_apply_pbr(OxrRenderer* r, const OxcCullCamera* camera, const OxcPbrCamera* pbr_camera, const OxcPbrSettings* settings,
+                  const OxcLight* lights_host, int cast_shadows, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* gtao_settings,
+                  float* rgba_host) {
+  if (!r || !camera || !pbr_camera || !settings) return OXC_E_INVALID;
+  return r->impl.apply_pbr(*camera, *pbr_camera, *settings, lights_host, cast_shadows != 0, gtao_camera, gtao_settings, rgba_host);
 }
 
 int oxr_render(OxrRenderer* r, const OxcCullCamera* camera, const float* occluder_depth_host, uint32_t* vis32_host,

@@ -85,6 +85,10 @@ public:
   // then the three GTAO passes on its depth; width x height floats to the host
   auto generate_ambient_occlusion(const OxcCullCamera& camera, const OxcGtaoCamera& gtao_camera, const OxcGtaoSettings& settings, float* ao_host)
       -> int;
+  // apply_pbr (PBR.cpp:435-531, no atmosphere) on the last rendered frame, with the G-buffer decode, the shadow resolve (cast_shadows)
+  // and the GTAO (HasGTAO) before it, all from the G-buffer's normal plane; width x height float4 to the host
+  auto apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera& pbr_camera, const OxcPbrSettings& settings, const OxcLight* lights_host,
+                 bool cast_shadows, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* gtao_settings, float* rgba_host) -> int;
 
   // RendererInstance::render geometry section: run_geometry_pass(false) -> generate_hiz -> run_geometry_pass(true)
   auto render(const OxcCullCamera& camera, const float* occluder_depth_host, uint32_t* vis32_host, float* depth_host,
@@ -156,6 +160,18 @@ private:
                                     // first of them; kept for the renderer's lifetime
   void* d_gtao_ = nullptr;          // generate_ambient_occlusion's planes (mips, edges, noisy and final occlusion), allocated by its first call
   int uv_normal_plane();            // allocates d_uv_normal_ when missing: OXC_OK or OXC_E_CAPACITY
+  int gbuffer_planes();             // allocates d_gbuffer_ when missing: OXC_OK or OXC_E_CAPACITY
+  int shadow_plane();               // allocates vsm_.d_shadow when missing: OXC_OK or OXC_E_CAPACITY
+  int gtao_planes();                // allocates d_gtao_ when missing: OXC_OK or OXC_E_CAPACITY
+  size_t gtao_mip_texels() const;   // texels of the five depth mips at the renderer's extent
+  // the device parts of decode_visbuffer, resolve_shadowmap and generate_ambient_occlusion, enqueued on stream_ without a copy; the
+  // two last read the given normal plane (oct(world normal) in .zw)
+  int decode_gbuffer_device(const OxcCullCamera& camera, const OxcGBufferTargets& targets);
+  int resolve_shadowmap_device(const float* normals);
+  int generate_ambient_occlusion_device(const OxcGtaoCamera& gtao_camera, const OxcGtaoSettings& settings, const float* normals,
+                                        OxcGtaoTargets* targets);
+  float* d_pbr_ = nullptr;          // apply_pbr's output plane (float4 per pixel), allocated by its first call
+  OxcLight* d_lights_ = nullptr;    // apply_pbr's lights buffer (OXC_MAX_LIGHTS records), allocated with d_pbr_
   bool has_external_depth_ = false;
   // transforms as the host last uploaded them, and on the device the values before the upload that last changed each of them
   // (TransformPrevious::previous_world, RendererInstance.cpp:1600-1609)

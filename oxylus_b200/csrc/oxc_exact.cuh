@@ -371,6 +371,20 @@ OXC_DI float canonical_pow(float xf, float yf) {
   return d2f_rn(ldexp(er, (int)k));
 }
 
+// pow(x, 5.0) for F_Schlick (PBR apply), bit-identical to oracle/oxc_oracle_pbr.c orc_pow5_canonical: x2 = x * x in binary64, then
+// (x2 * x2) * x in binary64, one rounding to binary32.  Within 1 ulp of the correctly rounded binary32 power: x has 24 significant
+// bits, so x2 (48 bits) is exact; x2 * x2 and the product with x each round once with relative error <= 2^-53, so the binary64 value
+// is x^5 (1 + d) with |d| < 2^-51.  No binary64 overflow or underflow can occur for finite binary32 x (|x^5| lies in [2^-745,
+// 2^640] or is 0), so the bound holds everywhere.  Half a binary32 ulp is at least 2^-25 relative (less only among binary32
+// subnormals, where the absolute spacing 2^-149 only widens it), so rounding x^5 (1 + d) gives RN(x^5) or, when x^5 lies within
+// 2^-51 relative of a rounding tie, its neighbour across that tie: in both cases |result - x^5| < 1 ulp.  NaN stays NaN, +-inf and
+// +-0 follow the sign of x.
+OXC_DI float canonical_pow5(float xf) {
+  const double x = (double)xf;
+  const double x2 = dmul64(x, x);
+  return d2f_rn(dmul64(dmul64(x2, x2), x));
+}
+
 // cull.slang:169-171: determinant(f32x3x3(c0.xyw, c1.xyw, c2.xyw)) >= 0.0001
 OXC_DI bool triangle_backface(float4 c0, float4 c1, float4 c2) {
   const float m00 = c0.x, m01 = c0.y, m02 = c0.w;

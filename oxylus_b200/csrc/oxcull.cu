@@ -26,6 +26,7 @@
 #include "kernels_vsm_draw.cuh"
 #include "kernels_vsm_resolve.cuh"
 #include "kernels_gtao.cuh"
+#include "kernels_pbr.cuh"
 
 using namespace oxc;
 
@@ -1544,6 +1545,34 @@ int oxc_generate_ambient_occlusion(OxcContext* c, const OxcGtaoCamera* cam, cons
   k_gtao_main<<<grid, GTAO_THREADS, 0, s>>>(p);
   LAUNCHED();
   k_gtao_denoise<<<grid, GTAO_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_apply_pbr(OxcContext* c, const OxcPbrCamera* cam, const OxcPbrSettings* st, const OxcLight* lights_dev, const OxcPbrInputs* in,
+                  uint32_t w, uint32_t h, float* out_dev, void* stream) {
+  if (!c || !cam || !st || !in || !out_dev) return fail(OXC_E_INVALID, "null argument");
+  if (!in->depth || !in->albedo || !in->normal || !in->emissive || !in->metallic_roughness_occlusion) return fail(OXC_E_INVALID, "null input plane");
+  if (st->light_count > OXC_MAX_LIGHTS) return fail(OXC_E_INVALID, "light_count %u above %u", st->light_count, OXC_MAX_LIGHTS);
+  if (st->light_count > 0 && !lights_dev) return fail(OXC_E_INVALID, "null lights with light_count %u", st->light_count);
+  if (st->scene_flags & OXC_SCENE_HAS_ATMOSPHERE) return fail(OXC_E_INVALID, "HasAtmosphere: the atmosphere variant is not available");
+  if ((st->scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS) && !in->contact_shadow)
+    return fail(OXC_E_INVALID, "null contact_shadow plane under HasContactShadows");
+  if (w == 0 || h == 0) return fail(OXC_E_INVALID, "empty extent %u x %u", w, h);
+  if (w > 32768u || h > 32768u) return fail(OXC_E_INVALID, "extent %u x %u above 32768", w, h);
+  if ((reinterpret_cast<uintptr_t>(in->albedo) | reinterpret_cast<uintptr_t>(in->normal) | reinterpret_cast<uintptr_t>(in->emissive) |
+       reinterpret_cast<uintptr_t>(in->metallic_roughness_occlusion) | reinterpret_cast<uintptr_t>(out_dev) |
+       reinterpret_cast<uintptr_t>(lights_dev)) & 15u)
+    return fail(OXC_E_INVALID, "float4 planes, out_dev and lights_dev must be 16-byte aligned");
+  if ((reinterpret_cast<uintptr_t>(in->depth) | reinterpret_cast<uintptr_t>(in->ambient_occlusion) | reinterpret_cast<uintptr_t>(in->shadow) |
+       reinterpret_cast<uintptr_t>(in->contact_shadow)) & 3u)
+    return fail(OXC_E_INVALID, "depth, ambient_occlusion, shadow and contact_shadow must be 4-byte aligned");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  PbrParams p = pbr_make_params(*cam, *st, lights_dev, *in, w, h, out_dev);
+  if (!(st->scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS)) p.contact = nullptr;
+  const dim3 grid((w + PBR_TILE_X - 1) / PBR_TILE_X, (h + PBR_TILE_Y - 1) / PBR_TILE_Y);
+  k_apply_pbr<<<grid, PBR_THREADS, 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }

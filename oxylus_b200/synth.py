@@ -108,6 +108,39 @@ def make_camera(width, height, mesh_instance_count, yaw_deg=0.0, eye=(0.0, 0.0, 
     return cam
 
 
+def pbr_camera(cull_camera):
+    """abi.PbrCamera of a make_camera camera: the binary64 inverse of its projection_view (column-major), rounded to binary32, and its
+    position"""
+    inv = np.linalg.inv(cull_camera["projection_view"][0].reshape(4, 4).T.astype(np.float64)).T.astype(np.float32).reshape(16)
+    return abi.pbr_camera(inv, cull_camera["position"][0])
+
+
+def make_lights(rng, n, eye=(0.0, 0.0, 0.0), yaw_deg=0.0, spot_fraction=0.5, distance=(3.0, 60.0), radius=(2.0, 25.0), intensity=(0.5, 40.0)):
+    """n seeded point and spot lights (abi.Light array) placed in front of a make_camera camera at `eye` / `yaw_deg`: positions up to
+    45 degrees off the view axis at `distance`, 0.5..6 m above the eye's height, ranges in `radius` (each lights part of the view),
+    colours in [0.2, 1], spots aimed at a point on the axis with cone angles of 0.1..0.9 rad (inner <= outer)"""
+    lights = (abi.Light * n)()
+    yaw = np.radians(yaw_deg)
+    for i in range(n):
+        d = rng.uniform(*distance)
+        a = yaw + rng.uniform(-np.pi / 4, np.pi / 4)
+        p = np.asarray(eye, np.float64) + (-np.sin(a) * d, rng.uniform(0.5, 6.0), -np.cos(a) * d)
+        L = lights[i]
+        L.position[:] = [float(np.float32(v)) for v in p]
+        L.intensity = float(np.float32(rng.uniform(*intensity)))
+        L.color[:] = [float(np.float32(v)) for v in rng.uniform(0.2, 1.0, 3)]
+        L.range = float(np.float32(rng.uniform(*radius)))
+        if rng.random() < spot_fraction:
+            L.kind = abi.LIGHT_SPOT
+            target = np.asarray(eye, np.float64) + (-np.sin(yaw) * rng.uniform(*distance), -2.0, -np.cos(yaw) * rng.uniform(*distance))
+            L.direction[:] = [float(np.float32(v)) for v in target - p]
+            inner = rng.uniform(0.1, 0.6)
+            L.inner_cone_angle, L.outer_cone_angle = float(np.float32(inner)), float(np.float32(inner + rng.uniform(0.0, 0.3)))
+        else:
+            L.kind = abi.LIGHT_POINT
+    return lights
+
+
 def make_ortho_view(direction, center, half_size, depth_range, mesh_instance_count, resolution=2048):
     """Orthographic reverse-Z shadow-cascade style view (Camera.cpp:44-52 shape) for the multi-view config.
     position carries the light direction (-dir), as the reference does for directional cone tests
