@@ -1,6 +1,7 @@
 """The GTAO on the device (oxc_generate_ambient_occlusion, oxr_generate_ambient_occlusion) against the CPU oracle
 (oracle/oxc_oracle_gtao.c orc_generate_ambient_occlusion): the depth mips, the edges, the noisy occlusion and the final occlusion
-compared bit for bit in every case, plus two checks without the oracle (an all-sky frame, a crease between two planes)."""
+compared bit for bit in every case, plus two checks without the oracle (an all-sky frame, a crease between two planes), and the device
+against the binary64 restatement of tests/test_oracle_gtao_f64.py on ray-cast scenes up to 4K."""
 import numpy as np
 import pytest
 
@@ -279,3 +280,48 @@ def test_renderer_frame(capi, go):
     for t, r in zip(tables, renderers):
         t.free()
         r.close()
+
+
+ANALYTIC = [("box", 211, 97, 3), ("turned", 1920, 1080, 2), ("spheres", 1920, 1080, 1), ("corridor", 3840, 2160, 0)]
+
+
+@pytest.mark.parametrize("name,w,h,preset", ANALYTIC, ids=[f"analytic_{n}_{w}x{h}" for n, w, h, _ in ANALYTIC])
+def test_analytic_against_restatement(ctx, name, w, h, preset):
+    """every plane of the device agrees with the binary64 restatement on a ray-cast scene, by the rules of test_oracle_gtao_f64"""
+    from tests import test_oracle_gtao_f64 as f64
+
+    cam, depth, normals = f64.scene(name, w, h)
+    settings = abi.gtao_settings(preset)
+    got = run_device(ctx, f64.gtao_camera(cam), settings, depth, normals)
+    f64.compare(got, f64.restate(cam, settings, depth, normals), settings, depth, f"{name} {w}x{h}")
+
+
+def test_renderer_frame_against_restatement(capi):
+    """oxr_generate_ambient_occlusion on a rendered frame agrees with the binary64 restatement over the frame's depth and the decode's
+    normal plane"""
+    from tests import test_oracle_gtao_f64 as f64
+    from tests.test_gpu_gbuffer import Table, scene_with_materials
+
+    sc = synth.with_ground_caster(scene_with_materials(20000, 48, 10, config_index=2, width=640, height=360, n_unique_meshes=16),
+                                  half_size=1200.0, center=(0.0, -2.0, -40.0))
+    sc.mesh_instances["material_index"][-1] = 0
+    cam0 = sc.camera(0.0)
+    proj, view = synth.camera_matrices(sc.width, sc.height, 0.0)
+    cam = f64.camera_dict(proj, view)
+    settings = abi.gtao_settings(3)
+    r = capi.Renderer(0, sc)
+    table = Table(r.ctx, 10)
+    r.set_materials(table.materials, table.dev_images, table.samplers)
+    depth = r.render(cam0, want_indices=False)["depth"].copy()
+    got = r.generate_ambient_occlusion(cam0, f64.gtao_camera(cam), settings)
+    normal_plane = r.decode_gbuffer(cam0)[1]
+    zw = normal_plane[..., 2:4]
+    finite = np.isfinite(zw).all(-1)
+    # the ground's normals are NaN (the NaN rules decide its occlusion) and some of the others are not binary16-exact
+    assert (~finite).mean() > 0.2 and (zw.astype(np.float16).astype(np.float32) != zw).any(-1)[finite].mean() > 0.01
+    stats = f64.compare(dict(ao=got), f64.restate(cam, settings, depth, normal_plane), settings, depth, "renderer frame")
+    print("renderer frame", stats)
+    held = depth != 0
+    assert held.mean() > 0.3 and (got[held] < 0.9).sum() > 1000
+    table.free()
+    r.close()
