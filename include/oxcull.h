@@ -960,6 +960,58 @@ OXC_STATIC_ASSERT(sizeof(OxcPbrInputs) == 64, "PbrInputs");
 int oxc_apply_pbr(OxcContext* ctx, const OxcPbrCamera* camera, const OxcPbrSettings* settings, const OxcLight* lights_dev,
                   const OxcPbrInputs* inputs, uint32_t width, uint32_t height, float* out_dev, void* stream);
 
+/* Contact shadows: RendererInstance's contact_shadows pass (RendererInstance.cpp:990-1020, passes/contact_shadows.slang:29-78 with the
+ * raymarch.slang DepthRayMarch / HybridRootFinder / DepthRaymarchDistanceFn code it calls).  One f32 per pixel of a width x height
+ * frame, row-major, into out_dev: 1 - shadow, the plane oxc_apply_pbr reads under OXC_SCENE_HAS_CONTACT_SHADOWS.  depth_dev (D32F,
+ * reversed Z, 0 = sky) is only read; no scratch, so the call is graph-capturable from its first call.  Sky pixels are marched like any
+ * other pixel, as the shader does; PBR apply's own early returns decide what they show.
+ * Refused with OXC_E_INVALID, before anything is launched: a NULL argument, a zero extent or one above 32768, steps outside
+ * 1..OXC_CONTACT_SHADOW_MAX_STEPS (the reference's editor range; the bound keeps the march at most 64 taps per pixel for any depth),
+ * depth_dev or out_dev not 4-byte aligned.  NaN or Inf thickness, length and sun direction are accepted and follow the rules below.
+ * SPECIFICATION (oracle/oxc_oracle_contact_shadows.c orc_contact_shadows, bit for bit): IEEE binary32, no contraction, IEEE divide /
+ * sqrt, sums and products in written order, dot(a, b) = (a.x*b.x + a.y*b.y) + a.z*b.z (two components: a.x*b.x + a.y*b.y), mul(M, v)
+ * row by row in the same order, normalize(v) = v / sqrt(dot(v, v)), length(v) = sqrt(dot(v, v)); sign(NaN) = 0, saturate(NaN) = 0,
+ * max / min return the other operand for a NaN, u32(x) truncates and saturates (NaN -> 0), pow(x, 1.0) = x, lerp(0, 1, t) = 0 + (1 -
+ * 0) * t, smoothstep(e0, e1, x) = (t * t) * (3 - 2 * t) with t = saturate((x - e0) / (e1 - e0)) (also for e0 > e1); constants are the
+ * binary32 roundings of the shader's literals, and (1.0 + bias) is fl(1 + fl(2e-6)) = 0x3F800011 (a Slang literal without suffix is a
+ * float; folding the sum in binary64 and rounding once gives the same bits).  For pixel (x, y):
+ *   1. uv = ((x + 0.5) / W, (y + 0.5) / H); depth = the nearest tap at uv; cs = (uv * 2 - 1, depth); h = mul(inv_projection_view,
+ *      (cs, 1)); ws = h.xyz / h.w.
+ *   2. end = ws + normalize(sun_direction) * length; end_cs = (mul(projection, mul(view, (end, 1)))).xyz / w (to_ws); dir = (end_cs -
+ *      cs, 0) * sign(end_cs.z) (to_cs); e = (cs, 1) + dir, e /= (e.w >= 0 ? 1 : -1) * max(1e-10, |e.w|), as written.
+ *   3. start clip: delta = e.xyz - cs, near = delta < 0 ? (1, 1, 1) : (-1, -1, 0) per component, k = max((near.x - cs.x) / delta.x,
+ *      (near.y - cs.y) / delta.y), start = cs + delta * max(0, k).  End clip: delta = e.xyz - start, far = delta >= 0 ? (1, 1, 1) :
+ *      (-1, -1, 0), m = min(min(fx, fy), fz) of (far - start) / delta, delta *= min(1, m), end = start + delta.
+ *   4. march: uv_s / uv_e = start.xy / end.xy * 0.5 + 0.5, n = max(2, min(steps, u32(floor(length((uv_e - uv_s) * (W, H)) / 1)))),
+ *      depth_thickness = thickness * (1 / near_clip).  Steps i = 0..n-1 at t = 0 + (1 - 0) * ((i + 1) / n): p = start + (end - start) *
+ *      t, uv = p.xy * 0.5 + 0.5, lin = 1 / bilinear(uv), unf = 1 / nearest(uv), distance = max(lin, unf) * (1 + bias) - 1 / p.z,
+ *      penetration = 1 / p.z - min(lin, unf).  The first step with distance < 0 is the candidate; the pixel is in contact when
+ *      penetration < depth_thickness and distance < depth_thickness, and then shadow = smoothstep(1, 0.3, penetration /
+ *      depth_thickness); otherwise shadow = 0.
+ *   5. nearest tap at uv: texel (floor(u * W), floor(v * H)) with NaN-safe saturating indices (oxc_alpha.cuh alpha_f2i), clamped to
+ *      the edge.  Bilinear tap at uv: x = u * W - 0.5, x0 = floor(x), wx = x - x0 (y likewise), texels x0, x0 + 1 / y0, y0 + 1 with the
+ *      same index rule, top = a00 + wx * (a10 - a00), bottom = a01 + wx * (a11 - a01), top + wy * (bottom - top): the GTAO's level tap
+ *      (oxc_generate_ambient_occlusion item 6).  Deviation: no 8-bit quantisation of the weights, as the alpha test's.
+ *   6. output: 1 - shadow as binary32 (the value of the reference's R32F store); it lies in [0, 1] and is never NaN.
+ * Hostile depth (NaN, Inf, denormal, negative) and settings do not fault and follow the same rules. */
+#define OXC_CONTACT_SHADOW_MAX_STEPS 64u
+typedef struct OxcContactShadowCamera { /* the Camera fields the pass reads (scene.slang:162-188), column-major */
+  float inv_projection_view[16];
+  float view[16];
+  float projection[16];
+  float near_clip;
+} OxcContactShadowCamera;
+typedef struct OxcContactShadowSettings { /* the pass's push constants (contact_shadows.slang:15-20, RendererCVar.cpp:30-34) */
+  float sun_direction[3];          /* DirectionalLight::direction, normalized by the pass */
+  uint32_t steps;                  /* 1..OXC_CONTACT_SHADOW_MAX_STEPS, the reference's default 8 */
+  float thickness;                 /* world units at the near plane, default 0.1 */
+  float length;                    /* world-space ray length, default 0.01 */
+} OxcContactShadowSettings;
+OXC_STATIC_ASSERT(sizeof(OxcContactShadowCamera) == 196, "ContactShadowCamera");
+OXC_STATIC_ASSERT(sizeof(OxcContactShadowSettings) == 24, "ContactShadowSettings");
+int oxc_contact_shadows(OxcContext* ctx, const OxcContactShadowCamera* camera, const OxcContactShadowSettings* settings, const float* depth_dev,
+                        uint32_t width, uint32_t height, float* out_dev, void* stream);
+
 int oxc_get_outputs(OxcContext* ctx, OxcOutputs* out);
 /* Instrumentation hook: 128 u64 counters that builds with -DOXC_RASTER_STATS fill (tools/raster_stats.py); zero otherwise. */
 void* oxc_debug_stats_ptr(OxcContext* ctx);
@@ -1094,12 +1146,26 @@ int oxr_generate_ambient_occlusion(OxrRenderer* r, const OxcCullCamera* camera, 
  *   4. oxc_apply_pbr with pbr_camera, settings and settings->light_count records of lights_host, uploaded into a renderer-owned
  *      OXC_MAX_LIGHTS-record buffer.
  * The resolve and the GTAO read the G-buffer's normal plane (its .zw equals oxc_decode_visbuffer's uv_normal.zw).  width x height
- * float4 to rgba_host.  OXC_SCENE_HAS_CONTACT_SHADOWS is refused (OXC_E_INVALID) until there is a contact-shadow pass.  The planes
- * (G-buffer, resolve, GTAO, about 100 B / pixel, and 16 B / pixel of output) are allocated at the first call that needs them;
- * OXC_E_CAPACITY, with the camera path left usable, when they cannot be.  The frame's outputs are left as they were. */
+ * float4 to rgba_host.  OXC_SCENE_HAS_CONTACT_SHADOWS is refused (OXC_E_INVALID): oxr_apply_pbr_with_contact_shadows below runs the
+ * contact-shadow pass and takes the flag.  The planes (G-buffer, resolve, GTAO, about 100 B / pixel, and 16 B / pixel of output) are
+ * allocated at the first call that needs them; OXC_E_CAPACITY, with the camera path left usable, when they cannot be.  The frame's
+ * outputs are left as they were. */
 int oxr_apply_pbr(OxrRenderer* r, const OxcCullCamera* camera, const OxcPbrCamera* pbr_camera, const OxcPbrSettings* settings,
                   const OxcLight* lights_host, int cast_shadows, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* gtao_settings,
                   float* rgba_host);
+/* The contact_shadows pass (RendererInstance.cpp:990-1020): oxc_contact_shadows on the depth of the frame oxr_render / oxr_wait
+ * completed last, into a 4 B / pixel plane the renderer allocates at the first call; width x height floats to contact_host.
+ * Synchronous.  The frame's outputs are left as they were.  OXC_E_CAPACITY, with the camera path left usable, when the plane cannot be
+ * allocated; OXC_E_INVALID for settings oxc_contact_shadows refuses. */
+int oxr_contact_shadows(OxrRenderer* r, const OxcContactShadowCamera* contact_camera, const OxcContactShadowSettings* settings,
+                        float* contact_host);
+/* oxr_apply_pbr with OXC_SCENE_HAS_CONTACT_SHADOWS accepted: under that flag the contact-shadow pass runs in the reference's place,
+ * after the shadow resolve and before the GTAO, with contact_camera and contact_settings (both required then), and oxc_apply_pbr reads
+ * its plane.  Without the flag it computes exactly what oxr_apply_pbr computes and the two contact arguments are not read. */
+int oxr_apply_pbr_with_contact_shadows(OxrRenderer* r, const OxcCullCamera* camera, const OxcPbrCamera* pbr_camera, const OxcPbrSettings* settings,
+                                       const OxcLight* lights_host, int cast_shadows, const OxcGtaoCamera* gtao_camera,
+                                       const OxcGtaoSettings* gtao_settings, const OxcContactShadowCamera* contact_camera,
+                                       const OxcContactShadowSettings* contact_settings, float* rgba_host);
 
 /* ------------------------------------------------------------------------------------------------
  * oxb_* — mesh builder (SURVEY §8f.2): host-side producer of the blob layout above, mirroring build_gltf_mesh

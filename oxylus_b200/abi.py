@@ -433,6 +433,40 @@ def pbr_camera(inv_projection_view, position):
     return c
 
 
+CONTACT_SHADOW_MAX_STEPS = 64  # the editor's range of the steps cvar (ViewportPanel.cpp:748)
+
+
+class ContactShadowCamera(C.Structure):
+    """OxcContactShadowCamera: Camera::inv_projection_view, view and projection (column-major) and near_clip"""
+
+    _fields_ = [("inv_projection_view", C.c_float * 16), ("view", C.c_float * 16), ("projection", C.c_float * 16), ("near_clip", C.c_float)]
+
+
+class ContactShadowSettings(C.Structure):
+    """OxcContactShadowSettings: the contact_shadows pass's push constants (sun direction, steps, thickness, length)"""
+
+    _fields_ = [("sun_direction", C.c_float * 3), ("steps", C.c_uint32), ("thickness", C.c_float), ("length", C.c_float)]
+
+
+assert C.sizeof(ContactShadowCamera) == 196 and C.sizeof(ContactShadowSettings) == 24
+
+
+def contact_shadow_camera(inv_projection_view, view, projection, near_clip):
+    c = ContactShadowCamera()
+    for name, m in (("inv_projection_view", inv_projection_view), ("view", view), ("projection", projection)):
+        getattr(c, name)[:] = [float(x) for x in np.asarray(m, dtype=np.float32).reshape(16)]
+    c.near_clip = float(np.float32(near_clip))
+    return c
+
+
+def contact_shadow_settings(sun_direction=(0.3, 0.8, 0.52), steps=8, thickness=0.1, length=0.01):
+    """ContactShadowSettings with the reference's cvar defaults (RendererCVar.cpp:30-34: 8 steps, thickness 0.1, length 0.01)"""
+    s = ContactShadowSettings()
+    s.sun_direction[:] = [float(np.float32(v)) for v in sun_direction]
+    s.steps, s.thickness, s.length = int(steps), float(np.float32(thickness)), float(np.float32(length))
+    return s
+
+
 MESH_MAX_LODS = 8
 
 

@@ -22,13 +22,14 @@ SYMBOLS = [
     "oxc_decode_visbuffer", "oxc_decode_gbuffer", "oxc_build_hpb", "oxc_mark_visible_pages",
     "oxc_vsm_begin_frame", "oxc_vsm_invalidate_pages", "oxc_vsm_allocate_pages", "oxc_vsm_clear_dirty_pages", "oxc_cull_meshlets_hpb_dirty_dev",
     "oxc_vsm_draw_pages", "oxc_vsm_draw_stats", "oxc_vsm_resolve_shadows", "oxc_generate_ambient_occlusion", "oxc_apply_pbr",
+    "oxc_contact_shadows",
     "oxc_get_outputs", "oxc_check_status", "oxc_mark_hiz_dirty", "oxc_bind_camera_buffer", "oxc_load_camera", "oxc_debug_stats_ptr",
     "oxc_mgpu_get_unique_id", "oxc_mgpu_init", "oxc_mgpu_init_with_comm", "oxc_mgpu_shutdown", "oxc_mgpu_info", "oxc_mgpu_exchange_hiz",
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
     "oxb_last_error", "oxb_build_mesh", "oxb_mesh_blob_size", "oxb_mesh_lod0_meshlet_count", "oxb_mesh_emit", "oxb_mesh_free", "oxb_simplify",
     "oxr_create", "oxr_destroy", "oxr_context", "oxr_update", "oxr_update_transforms", "oxr_set_external_depth", "oxr_set_materials", "oxr_overdraw", "oxr_render", "oxr_submit", "oxr_wait",
     "oxr_vsm_update_pages", "oxr_vsm_pages", "oxr_vsm_draw_shadows", "oxr_vsm_resolve_shadows", "oxr_decode_gbuffer",
-    "oxr_generate_ambient_occlusion", "oxr_apply_pbr",
+    "oxr_generate_ambient_occlusion", "oxr_apply_pbr", "oxr_contact_shadows", "oxr_apply_pbr_with_contact_shadows",
 ]
 
 
@@ -150,6 +151,10 @@ def load(build_if_missing=True):
     lib.oxr_generate_ambient_occlusion.argtypes = [vp, vp, C.POINTER(abi.GtaoCamera), C.POINTER(abi.GtaoSettings), vp]
     lib.oxc_apply_pbr.argtypes = [vp, C.POINTER(abi.PbrCamera), C.POINTER(abi.PbrSettings), vp, C.POINTER(abi.PbrInputs), u32, u32, vp, vp]
     lib.oxr_apply_pbr.argtypes = [vp, vp, C.POINTER(abi.PbrCamera), C.POINTER(abi.PbrSettings), vp, C.c_int, vp, vp, vp]
+    lib.oxc_contact_shadows.argtypes = [vp, C.POINTER(abi.ContactShadowCamera), C.POINTER(abi.ContactShadowSettings), vp, u32, u32, vp, vp]
+    lib.oxr_contact_shadows.argtypes = [vp, C.POINTER(abi.ContactShadowCamera), C.POINTER(abi.ContactShadowSettings), vp]
+    lib.oxr_apply_pbr_with_contact_shadows.argtypes = [vp, vp, C.POINTER(abi.PbrCamera), C.POINTER(abi.PbrSettings), vp, C.c_int, vp, vp,
+                                                       vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -504,6 +509,12 @@ class Context:
         _check(self.lib.oxc_apply_pbr(self.h, C.byref(pbr_camera), C.byref(settings), _ptr(lights_dev), C.byref(t), w, h, _ptr(out_dev),
                                       self.stream), "oxc_apply_pbr")
 
+    def contact_shadows(self, contact_camera, settings, depth_dev, w, h, out_dev):
+        """oxc_contact_shadows: 1 - the contact shadow (f32 per pixel) of a w x h frame into out_dev.  contact_camera / settings:
+        abi.ContactShadowCamera / abi.ContactShadowSettings"""
+        _check(self.lib.oxc_contact_shadows(self.h, C.byref(contact_camera), C.byref(settings), _ptr(depth_dev), w, h, _ptr(out_dev), self.stream),
+               "oxc_contact_shadows")
+
     def build_hpb(self, page_table_dev, size, layers, hpb_dev, levels):
         _check(self.lib.oxc_build_hpb(self.h, _ptr(page_table_dev), size, layers, _ptr(hpb_dev), levels, self.stream), "oxc_build_hpb")
 
@@ -760,11 +771,21 @@ class Renderer:
                "oxr_generate_ambient_occlusion")
         return out
 
-    def apply_pbr(self, cam, settings, lights=None, cast_shadows=False, gtao_camera=None, gtao_settings=None, pbr_camera=None):
+    def contact_shadows(self, contact_camera, settings):
+        """oxr_contact_shadows: 1 - the contact shadow (float32 [height, width]) over the depth of the frame rendered last
+        (contact_camera: abi.ContactShadowCamera of that frame's camera; settings: abi.ContactShadowSettings)"""
+        out = np.zeros((self.scene.height, self.scene.width), dtype=np.float32)
+        _check(self.lib.oxr_contact_shadows(self.h, C.byref(contact_camera), C.byref(settings), _ptr(out)), "oxr_contact_shadows")
+        return out
+
+    def apply_pbr(self, cam, settings, lights=None, cast_shadows=False, gtao_camera=None, gtao_settings=None, pbr_camera=None,
+                  contact_camera=None, contact_settings=None):
         """oxr_apply_pbr: the lit frame (float32 [height, width, 4]) of the frame rendered last with `cam`: G-buffer decode, the shadow
         resolve when cast_shadows (state of the last vsm_update_pages / vsm_draw_shadows), GTAO under SCENE_HAS_GTAO (gtao_camera,
         gtao_settings), then PBR apply with settings (abi.PbrSettings; light_count is set from `lights`, an abi.Light array).
-        pbr_camera defaults to synth.pbr_camera(cam)"""
+        pbr_camera defaults to synth.pbr_camera(cam).  Given contact_camera or contact_settings (abi.ContactShadowCamera /
+        abi.ContactShadowSettings), it calls oxr_apply_pbr_with_contact_shadows, which runs the contact-shadow pass under
+        SCENE_HAS_CONTACT_SHADOWS"""
         from oxylus_b200 import synth
 
         n = 0 if lights is None else len(lights)
@@ -772,9 +793,14 @@ class Renderer:
         settings.light_count = n
         pc = pbr_camera if pbr_camera is not None else synth.pbr_camera(cam)
         out = np.zeros((self.scene.height, self.scene.width, 4), dtype=np.float32)
-        _check(self.lib.oxr_apply_pbr(self.h, _ptr(cam), C.byref(pc), C.byref(settings), C.cast(lights, C.c_void_p) if n else None,
-                                      int(bool(cast_shadows)), C.byref(gtao_camera) if gtao_camera is not None else None,
-                                      C.byref(gtao_settings) if gtao_settings is not None else None, _ptr(out)), "oxr_apply_pbr")
+        args = [self.h, _ptr(cam), C.byref(pc), C.byref(settings), C.cast(lights, C.c_void_p) if n else None, int(bool(cast_shadows)),
+                C.byref(gtao_camera) if gtao_camera is not None else None, C.byref(gtao_settings) if gtao_settings is not None else None]
+        if contact_camera is None and contact_settings is None:
+            _check(self.lib.oxr_apply_pbr(*args, _ptr(out)), "oxr_apply_pbr")
+        else:
+            _check(self.lib.oxr_apply_pbr_with_contact_shadows(*args, C.byref(contact_camera) if contact_camera is not None else None,
+                                                               C.byref(contact_settings) if contact_settings is not None else None, _ptr(out)),
+                   "oxr_apply_pbr_with_contact_shadows")
         return out
 
     def vsm_pages(self):

@@ -102,7 +102,7 @@ RendererInstance::RendererInstance(int device, const OxcCreateInfo& info, uint32
 RendererInstance::~RendererInstance() {
   if (stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(stream_));
   cudaFree(d_vis64_); cudaFree(d_vis32_); cudaFree(d_depth_); cudaFree(d_occluder_); cudaFree(d_overdraw_); cudaFree(d_gbuffer_);
-  cudaFree(d_uv_normal_); cudaFree(d_gtao_); cudaFree(d_pbr_); cudaFree(d_lights_);
+  cudaFree(d_uv_normal_); cudaFree(d_gtao_); cudaFree(d_pbr_); cudaFree(d_lights_); cudaFree(d_contact_);
   if (h_pinned_) cudaFreeHost(h_pinned_);
   if (copy_stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(copy_stream_));
   for (auto& sl : slots_) {
@@ -442,17 +442,23 @@ int RendererInstance::generate_ambient_occlusion_device(const OxcGtaoCamera& gta
 // G-buffer of the last frame, the shadow resolve and the GTAO on its normal plane (whose .zw is the vis decode's uv_normal.zw), then
 // the lighting into the renderer's output plane
 auto RendererInstance::apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera& pbr_camera, const OxcPbrSettings& settings, const OxcLight* lights_host,
-                                 bool cast_shadows, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* gtao_settings, float* rgba_host) -> int {
+                                 bool cast_shadows, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* gtao_settings, float* rgba_host,
+                                 const OxcContactShadowCamera* contact_camera, const OxcContactShadowSettings* contact_settings) -> int {
   if (!ctx_ || !error_.empty()) return OXC_E_STATE;
   const bool gtao = (settings.scene_flags & OXC_SCENE_HAS_GTAO) != 0;
+  const bool contact = (settings.scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS) != 0;
   if (!rgba_host || (gtao && (!gtao_camera || !gtao_settings)) || (settings.light_count > 0 && !lights_host)) return OXC_E_INVALID;
-  if (settings.light_count > OXC_MAX_LIGHTS || (settings.scene_flags & (OXC_SCENE_HAS_ATMOSPHERE | OXC_SCENE_HAS_CONTACT_SHADOWS)))
-    return OXC_E_INVALID; // no atmosphere variant and no contact-shadow pass: refused before anything is enqueued
+  if (contact && (!contact_camera || !contact_settings || contact_settings->steps < 1u || contact_settings->steps > OXC_CONTACT_SHADOW_MAX_STEPS))
+    return OXC_E_INVALID; // refused before anything is enqueued
+  if (settings.light_count > OXC_MAX_LIGHTS || (settings.scene_flags & OXC_SCENE_HAS_ATMOSPHERE))
+    return OXC_E_INVALID; // no atmosphere variant: refused before anything is enqueued
   if (cast_shadows && !vsm_.updated) return OXC_E_STATE;
   cudaStream_t s = static_cast<cudaStream_t>(stream_);
   const size_t px = (size_t)width_ * height_;
   // the planes are an optional part, as the other passes' are: without room for them the camera path stays usable
-  if (gbuffer_planes() != OXC_OK || (cast_shadows && shadow_plane() != OXC_OK) || (gtao && gtao_planes() != OXC_OK)) return OXC_E_CAPACITY;
+  if (gbuffer_planes() != OXC_OK || (cast_shadows && shadow_plane() != OXC_OK) || (gtao && gtao_planes() != OXC_OK) ||
+      (contact && contact_plane() != OXC_OK))
+    return OXC_E_CAPACITY;
   if (!d_pbr_ && (cudaMalloc(reinterpret_cast<void**>(&d_pbr_), px * 16) != cudaSuccess ||
                   cudaMalloc(reinterpret_cast<void**>(&d_lights_), OXC_MAX_LIGHTS * sizeof(OxcLight)) != cudaSuccess)) {
     cudaGetLastError();
@@ -469,6 +475,10 @@ auto RendererInstance::apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera
     if ((rc = resolve_shadowmap_device(gb.normal)) != OXC_OK) return rc;
     in.shadow = vsm_.d_shadow;
   }
+  if (contact) { // RendererInstance.cpp:990-1020: after the shadow resolve, before the GTAO
+    if ((rc = contact_shadows_device(*contact_camera, *contact_settings)) != OXC_OK) return rc;
+    in.contact_shadow = d_contact_;
+  }
   if (gtao) {
     OxcGtaoTargets t;
     if ((rc = generate_ambient_occlusion_device(*gtao_camera, *gtao_settings, gb.normal, &t)) != OXC_OK) return rc;
@@ -483,6 +493,42 @@ auto RendererInstance::apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera
   if (rc != OXC_OK) return fail(rc);
   if (cudaMemcpyAsync(rgba_host, d_pbr_, px * 16, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
     return fail(OXC_E_CUDA);
+  return OXC_OK;
+}
+
+// the contact_shadows pass (RendererInstance.cpp:990-1020) on stream_, synchronous: the last frame's depth, the pass into the renderer's
+// own plane, width x height floats to the host
+auto RendererInstance::contact_shadows(const OxcContactShadowCamera& contact_camera, const OxcContactShadowSettings& settings, float* contact_host)
+    -> int {
+  if (!ctx_ || !error_.empty()) return OXC_E_STATE;
+  if (!contact_host) return OXC_E_INVALID;
+  // the plane is an optional part, as the other passes' are: without room for it the camera path stays usable
+  if (contact_plane() != OXC_OK) return OXC_E_CAPACITY;
+  int rc;
+  if ((rc = contact_shadows_device(contact_camera, settings)) != OXC_OK) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  if (cudaMemcpyAsync(contact_host, d_contact_, (size_t)width_ * height_ * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+      cudaStreamSynchronize(s) != cudaSuccess)
+    return fail(OXC_E_CUDA);
+  return OXC_OK;
+}
+
+int RendererInstance::contact_plane() {
+  if (d_contact_) return OXC_OK;
+  if (cudaMalloc(reinterpret_cast<void**>(&d_contact_), (size_t)width_ * height_ * 4) != cudaSuccess) {
+    cudaGetLastError();
+    d_contact_ = nullptr;
+    return OXC_E_CAPACITY;
+  }
+  return OXC_OK;
+}
+
+int RendererInstance::contact_shadows_device(const OxcContactShadowCamera& contact_camera, const OxcContactShadowSettings& settings) {
+  if (settings.steps < 1u || settings.steps > OXC_CONTACT_SHADOW_MAX_STEPS) return OXC_E_INVALID; // refused before anything is enqueued
+  int rc;
+  if ((rc = oxc_resolve_visbuffer(ctx_, d_vis64_, width_, height_, nullptr, d_depth_, stream_)) != OXC_OK) return fail(rc);
+  rc = oxc_contact_shadows(ctx_, &contact_camera, &settings, d_depth_, width_, height_, d_contact_, stream_);
+  if (rc != OXC_OK) return fail(rc);
   return OXC_OK;
 }
 
@@ -986,7 +1032,24 @@ int oxr_apply_pbr(OxrRenderer* r, const OxcCullCamera* camera, const OxcPbrCamer
                   const OxcLight* lights_host, int cast_shadows, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* gtao_settings,
                   float* rgba_host) {
   if (!r || !camera || !pbr_camera || !settings) return OXC_E_INVALID;
+  // HasContactShadows needs the contact-shadow pass's camera and settings: oxr_apply_pbr_with_contact_shadows takes them
+  if (settings->scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS) return OXC_E_INVALID;
   return r->impl.apply_pbr(*camera, *pbr_camera, *settings, lights_host, cast_shadows != 0, gtao_camera, gtao_settings, rgba_host);
+}
+
+int oxr_contact_shadows(OxrRenderer* r, const OxcContactShadowCamera* contact_camera, const OxcContactShadowSettings* settings,
+                        float* contact_host) {
+  if (!r || !contact_camera || !settings) return OXC_E_INVALID;
+  return r->impl.contact_shadows(*contact_camera, *settings, contact_host);
+}
+
+int oxr_apply_pbr_with_contact_shadows(OxrRenderer* r, const OxcCullCamera* camera, const OxcPbrCamera* pbr_camera, const OxcPbrSettings* settings,
+                                       const OxcLight* lights_host, int cast_shadows, const OxcGtaoCamera* gtao_camera,
+                                       const OxcGtaoSettings* gtao_settings, const OxcContactShadowCamera* contact_camera,
+                                       const OxcContactShadowSettings* contact_settings, float* rgba_host) {
+  if (!r || !camera || !pbr_camera || !settings) return OXC_E_INVALID;
+  return r->impl.apply_pbr(*camera, *pbr_camera, *settings, lights_host, cast_shadows != 0, gtao_camera, gtao_settings, rgba_host, contact_camera,
+                           contact_settings);
 }
 
 int oxr_render(OxrRenderer* r, const OxcCullCamera* camera, const float* occluder_depth_host, uint32_t* vis32_host,

@@ -86,9 +86,13 @@ public:
   auto generate_ambient_occlusion(const OxcCullCamera& camera, const OxcGtaoCamera& gtao_camera, const OxcGtaoSettings& settings, float* ao_host)
       -> int;
   // apply_pbr (PBR.cpp:435-531, no atmosphere) on the last rendered frame, with the G-buffer decode, the shadow resolve (cast_shadows)
-  // and the GTAO (HasGTAO) before it, all from the G-buffer's normal plane; width x height float4 to the host
+  // and the GTAO (HasGTAO) before it, all from the G-buffer's normal plane, and the contact shadows (HasContactShadows, both contact
+  // arguments required then) between the resolve and the GTAO, as the reference orders them; width x height float4 to the host
   auto apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera& pbr_camera, const OxcPbrSettings& settings, const OxcLight* lights_host,
-                 bool cast_shadows, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* gtao_settings, float* rgba_host) -> int;
+                 bool cast_shadows, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* gtao_settings, float* rgba_host,
+                 const OxcContactShadowCamera* contact_camera = nullptr, const OxcContactShadowSettings* contact_settings = nullptr) -> int;
+  // the contact_shadows pass (RendererInstance.cpp:990-1020) on the last rendered frame's depth; width x height floats to the host
+  auto contact_shadows(const OxcContactShadowCamera& contact_camera, const OxcContactShadowSettings& settings, float* contact_host) -> int;
 
   // RendererInstance::render geometry section: run_geometry_pass(false) -> generate_hiz -> run_geometry_pass(true)
   auto render(const OxcCullCamera& camera, const float* occluder_depth_host, uint32_t* vis32_host, float* depth_host,
@@ -171,6 +175,10 @@ private:
   int generate_ambient_occlusion_device(const OxcGtaoCamera& gtao_camera, const OxcGtaoSettings& settings, const float* normals,
                                         OxcGtaoTargets* targets);
   float* d_pbr_ = nullptr;          // apply_pbr's output plane (float4 per pixel), allocated by its first call
+  float* d_contact_ = nullptr;      // the contact-shadow plane (f32 per pixel), allocated by the first call that runs the pass
+  int contact_plane();              // allocates d_contact_ when missing: OXC_OK or OXC_E_CAPACITY
+  // the frame's depth, then the contact-shadow pass into d_contact_, enqueued on stream_ without a copy
+  int contact_shadows_device(const OxcContactShadowCamera& contact_camera, const OxcContactShadowSettings& settings);
   OxcLight* d_lights_ = nullptr;    // apply_pbr's lights buffer (OXC_MAX_LIGHTS records), allocated with d_pbr_
   bool has_external_depth_ = false;
   // transforms as the host last uploaded them, and on the device the values before the upload that last changed each of them

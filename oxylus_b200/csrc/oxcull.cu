@@ -27,6 +27,7 @@
 #include "kernels_vsm_resolve.cuh"
 #include "kernels_gtao.cuh"
 #include "kernels_pbr.cuh"
+#include "kernels_contact_shadows.cuh"
 
 using namespace oxc;
 
@@ -1573,6 +1574,34 @@ int oxc_apply_pbr(OxcContext* c, const OxcPbrCamera* cam, const OxcPbrSettings* 
   if (!(st->scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS)) p.contact = nullptr;
   const dim3 grid((w + PBR_TILE_X - 1) / PBR_TILE_X, (h + PBR_TILE_Y - 1) / PBR_TILE_Y);
   k_apply_pbr<<<grid, PBR_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_contact_shadows(OxcContext* c, const OxcContactShadowCamera* cam, const OxcContactShadowSettings* st, const float* depth_dev, uint32_t w,
+                        uint32_t h, float* out_dev, void* stream) {
+  if (!c || !cam || !st || !depth_dev || !out_dev) return fail(OXC_E_INVALID, "null argument");
+  if (w == 0 || h == 0) return fail(OXC_E_INVALID, "empty extent %u x %u", w, h);
+  if (w > 32768u || h > 32768u) return fail(OXC_E_INVALID, "extent %u x %u above 32768", w, h);
+  if (st->steps < 1u || st->steps > OXC_CONTACT_SHADOW_MAX_STEPS)
+    return fail(OXC_E_INVALID, "steps %u outside 1..%u", st->steps, OXC_CONTACT_SHADOW_MAX_STEPS);
+  if ((reinterpret_cast<uintptr_t>(depth_dev) | reinterpret_cast<uintptr_t>(out_dev)) & 3u)
+    return fail(OXC_E_INVALID, "depth_dev and out_dev must be 4-byte aligned");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  ContactShadowParams p{};
+  p.depth = depth_dev; p.out = out_dev; p.width = (int)w; p.height = (int)h;
+  for (int i = 0; i < 4; i++) {
+    p.inv_pv_row[i] = make_float4(cam->inv_projection_view[i], cam->inv_projection_view[4 + i], cam->inv_projection_view[8 + i],
+                                  cam->inv_projection_view[12 + i]);
+    p.view_row[i] = make_float4(cam->view[i], cam->view[4 + i], cam->view[8 + i], cam->view[12 + i]);
+    p.proj_row[i] = make_float4(cam->projection[i], cam->projection[4 + i], cam->projection[8 + i], cam->projection[12 + i]);
+  }
+  p.near_clip = cam->near_clip;
+  for (int i = 0; i < 3; i++) p.sun[i] = st->sun_direction[i];
+  p.thickness = st->thickness; p.length = st->length; p.steps = st->steps;
+  const dim3 grid((w + CONTACT_TILE_X - 1) / CONTACT_TILE_X, (h + CONTACT_TILE_Y - 1) / CONTACT_TILE_Y);
+  k_contact_shadows<<<grid, CONTACT_THREADS, 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }
