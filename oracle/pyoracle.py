@@ -17,13 +17,25 @@ from oxylus_b200 import abi  # noqa: E402  (ABI struct definitions only)
 _LIB = None
 
 
-def build(force=False):
-    so = os.path.join(_HERE, "liboxc_oracle.so")
-    srcs = [os.path.join(_HERE, f) for f in ("oxc_oracle.c", "oxc_oracle.h", "oxc_oracle_math.inc")]
-    srcs.append(os.path.join(os.path.dirname(_HERE), "include", "oxcull.h"))
+CFLAGS = ["-O2", "-std=c11", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-Wall", "-Wextra", "-Wno-unused-function", "-pthread"]
+
+
+def build_so(name, units, deps, force=False):
+    """compiles the C files `units` into oracle/<name> when it is missing or older than one of `deps` (every oracle file it is made
+    from) or include/oxcull.h.  The library is written under a per-process name and renamed into place, so concurrent test
+    processes never load a half-written one."""
+    so = os.path.join(_HERE, name)
+    srcs = [os.path.join(_HERE, f) for f in deps] + [os.path.join(os.path.dirname(_HERE), "include", "oxcull.h")]
     if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-B"])
+        tmp = so + f".{os.getpid()}.tmp"
+        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", tmp] + [os.path.join(_HERE, u) for u in units] +
+                              ["-lm", "-lpthread"])
+        os.replace(tmp, so)
     return so
+
+
+def build(force=False):
+    return build_so("liboxc_oracle.so", ["oxc_oracle.c"], ["oxc_oracle.c", "oxc_oracle.h", "oxc_oracle_math.inc"], force)
 
 
 def lib():

@@ -2,30 +2,20 @@
 sources it includes, built into oracle/liboxc_oracle_contact_shadows.so).  TEST INFRASTRUCTURE ONLY: tests/ and tools/ import it; the
 product package never does."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
+import pyoracle
 from pyoracle import _p
 from pyoracle_pbr import SOURCES as _PBR_SOURCES
-from pyoracle_vsm import CFLAGS
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 SOURCES = _PBR_SOURCES + ("oxc_oracle_contact_shadows.c", "oxc_oracle_contact_shadows.h")
 
 
 def build(force=False):
     """compiles liboxc_oracle_contact_shadows.so next to the sources when it is missing or older than them"""
-    so = os.path.join(_HERE, "liboxc_oracle_contact_shadows.so")
-    srcs = [os.path.join(_HERE, f) for f in SOURCES] + [os.path.join(os.path.dirname(_HERE), "include", "oxcull.h")]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        tmp = so + f".{os.getpid()}.tmp"
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", tmp, os.path.join(_HERE, "oxc_oracle_contact_shadows.c"),
-                                                                         "-lm", "-lpthread"])
-        os.replace(tmp, so)
-    return so
+    return pyoracle.build_so("liboxc_oracle_contact_shadows.so", ["oxc_oracle_contact_shadows.c"], SOURCES, force)
 
 
 def lib():

@@ -1,16 +1,12 @@
 """ctypes wrapper of the G-buffer decode oracle (oracle/oxc_oracle_gbuffer.c, one translation unit with oxc_oracle.c, built into
 oracle/liboxc_oracle_gbuffer.so).  TEST INFRASTRUCTURE ONLY: tests/ and tools/ import it; the product package never does."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 import pyoracle
 from pyoracle import _p
-from pyoracle_vsm import CFLAGS
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 SOURCES = ("oxc_oracle.c", "oxc_oracle.h", "oxc_oracle_math.inc", "oxc_oracle_gbuffer.c", "oxc_oracle_gbuffer.h")
 PLANES = ("albedo", "normal", "emissive", "metallic_roughness_occlusion")
@@ -18,13 +14,7 @@ PLANES = ("albedo", "normal", "emissive", "metallic_roughness_occlusion")
 
 def build(force=False):
     """compiles liboxc_oracle_gbuffer.so next to the sources when it is missing or older than them"""
-    so = os.path.join(_HERE, "liboxc_oracle_gbuffer.so")
-    srcs = [os.path.join(_HERE, f) for f in SOURCES] + [os.path.join(os.path.dirname(_HERE), "include", "oxcull.h")]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        tmp = so + f".{os.getpid()}.tmp"
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", tmp, os.path.join(_HERE, "oxc_oracle_gbuffer.c"), "-lm", "-lpthread"])
-        os.replace(tmp, so)
-    return so
+    return pyoracle.build_so("liboxc_oracle_gbuffer.so", ["oxc_oracle_gbuffer.c"], SOURCES, force)
 
 
 def lib():

@@ -3,29 +3,20 @@ oxc_oracle_vsm.c, built into oracle/liboxc_oracle_gtao.so).  TEST INFRASTRUCTURE
 package never does."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
+import pyoracle
 from pyoracle import _p
-from pyoracle_vsm import CFLAGS
 from pyoracle_vsm_resolve import SOURCES as _RESOLVE_SOURCES
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 SOURCES = _RESOLVE_SOURCES + ("oxc_oracle_gtao.c", "oxc_oracle_gtao.h")
 
 
 def build(force=False):
     """compiles liboxc_oracle_gtao.so next to the sources when it is missing or older than them"""
-    so = os.path.join(_HERE, "liboxc_oracle_gtao.so")
-    srcs = [os.path.join(_HERE, f) for f in SOURCES] + [os.path.join(os.path.dirname(_HERE), "include", "oxcull.h")]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        tmp = so + f".{os.getpid()}.tmp"
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", tmp, os.path.join(_HERE, "oxc_oracle_gtao.c"), "-lm",
-                                                                         "-lpthread"])
-        os.replace(tmp, so)
-    return so
+    return pyoracle.build_so("liboxc_oracle_gtao.so", ["oxc_oracle_gtao.c"], SOURCES, force)
 
 
 def lib():

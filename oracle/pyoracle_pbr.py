@@ -2,30 +2,20 @@
 includes, built into oracle/liboxc_oracle_pbr.so).  TEST INFRASTRUCTURE ONLY: tests/ and tools/ import it; the product package never
 does."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
+import pyoracle
 from pyoracle import _p
 from pyoracle_gtao import SOURCES as _GTAO_SOURCES
-from pyoracle_vsm import CFLAGS
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 SOURCES = _GTAO_SOURCES + ("oxc_oracle_pbr.c", "oxc_oracle_pbr.h")
 
 
 def build(force=False):
     """compiles liboxc_oracle_pbr.so next to the sources when it is missing or older than them"""
-    so = os.path.join(_HERE, "liboxc_oracle_pbr.so")
-    srcs = [os.path.join(_HERE, f) for f in SOURCES] + [os.path.join(os.path.dirname(_HERE), "include", "oxcull.h")]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        tmp = so + f".{os.getpid()}.tmp"
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", tmp, os.path.join(_HERE, "oxc_oracle_pbr.c"), "-lm",
-                                                                         "-lpthread"])
-        os.replace(tmp, so)
-    return so
+    return pyoracle.build_so("liboxc_oracle_pbr.so", ["oxc_oracle_pbr.c"], SOURCES, force)
 
 
 def lib():

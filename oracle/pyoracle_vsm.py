@@ -4,8 +4,6 @@ oracle/liboxc_oracle_vsm.so).  TEST INFRASTRUCTURE ONLY: tests/ import it; the p
 Page tables are (layers, size, size) u32 arrays and every other array is updated in place.  Scenes are pyoracle.HostScene
 objects (the same OrcScene layout)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
@@ -13,22 +11,13 @@ import pyoracle
 from pyoracle import HostScene, _p, hpb_layout  # noqa: F401  (HostScene: re-exported for the tests)
 from oxylus_b200 import abi
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 SOURCES = ("oxc_oracle.c", "oxc_oracle.h", "oxc_oracle_math.inc", "oxc_oracle_vsm.c", "oxc_oracle_vsm.h")
-CFLAGS = ["-O2", "-std=c11", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-Wall", "-Wextra", "-Wno-unused-function", "-pthread"]
 
 
 def build(force=False):
-    """compiles liboxc_oracle_vsm.so next to the sources (same flags as oracle/Makefile) when it is missing or older than them"""
-    so = os.path.join(_HERE, "liboxc_oracle_vsm.so")
-    srcs = [os.path.join(_HERE, f) for f in SOURCES] + [os.path.join(os.path.dirname(_HERE), "include", "oxcull.h")]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        tmp = so + f".{os.getpid()}.tmp"
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", tmp, os.path.join(_HERE, "oxc_oracle.c"),
-                                                                         os.path.join(_HERE, "oxc_oracle_vsm.c"), "-lm", "-lpthread"])
-        os.replace(tmp, so)
-    return so
+    """compiles liboxc_oracle_vsm.so next to the sources when it is missing or older than them"""
+    return pyoracle.build_so("liboxc_oracle_vsm.so", ["oxc_oracle.c", "oxc_oracle_vsm.c"], SOURCES, force)
 
 
 def lib():

@@ -2,16 +2,12 @@
 oxc_oracle_vsm.c, built into oracle/liboxc_oracle_vsm_resolve.so).  TEST INFRASTRUCTURE ONLY: tests/ and tools/ import it; the
 product package never does."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 import pyoracle
 from pyoracle import _p
-from pyoracle_vsm import CFLAGS
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 SOURCES = ("oxc_oracle.c", "oxc_oracle.h", "oxc_oracle_math.inc", "oxc_oracle_vsm.c", "oxc_oracle_vsm.h", "oxc_oracle_vsm_resolve.c",
            "oxc_oracle_vsm_resolve.h")
@@ -19,14 +15,7 @@ SOURCES = ("oxc_oracle.c", "oxc_oracle.h", "oxc_oracle_math.inc", "oxc_oracle_vs
 
 def build(force=False):
     """compiles liboxc_oracle_vsm_resolve.so next to the sources when it is missing or older than them"""
-    so = os.path.join(_HERE, "liboxc_oracle_vsm_resolve.so")
-    srcs = [os.path.join(_HERE, f) for f in SOURCES] + [os.path.join(os.path.dirname(_HERE), "include", "oxcull.h")]
-    if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        tmp = so + f".{os.getpid()}.tmp"
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", tmp, os.path.join(_HERE, "oxc_oracle_vsm_resolve.c"),
-                                                                         "-lm", "-lpthread"])
-        os.replace(tmp, so)
-    return so
+    return pyoracle.build_so("liboxc_oracle_vsm_resolve.so", ["oxc_oracle_vsm_resolve.c"], SOURCES, force)
 
 
 def lib():

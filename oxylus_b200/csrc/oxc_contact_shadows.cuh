@@ -22,6 +22,23 @@ struct ContactShadowParams {
   uint32_t steps;           // 1..OXC_CONTACT_SHADOW_MAX_STEPS
 };
 
+// the kernel's parameters from the C ABI's arguments (oxc_contact_shadows, and the host build of the tests)
+__host__ inline ContactShadowParams cs_make_params(const OxcContactShadowCamera& cam, const OxcContactShadowSettings& st, const float* depth,
+                                                   uint32_t w, uint32_t h, float* out) {
+  ContactShadowParams p{};
+  p.depth = depth; p.out = out; p.width = (int)w; p.height = (int)h;
+  for (int i = 0; i < 4; i++) {
+    p.inv_pv_row[i] = make_float4(cam.inv_projection_view[i], cam.inv_projection_view[4 + i], cam.inv_projection_view[8 + i],
+                                  cam.inv_projection_view[12 + i]);
+    p.view_row[i] = make_float4(cam.view[i], cam.view[4 + i], cam.view[8 + i], cam.view[12 + i]);
+    p.proj_row[i] = make_float4(cam.projection[i], cam.projection[4 + i], cam.projection[8 + i], cam.projection[12 + i]);
+  }
+  p.near_clip = cam.near_clip;
+  for (int i = 0; i < 3; i++) p.sun[i] = st.sun_direction[i];
+  p.thickness = st.thickness; p.length = st.length; p.steps = st.steps;
+  return p;
+}
+
 // the per-pass values every pixel derives from the settings: normalize(sun_dir) (contact_shadows.slang:60) and depth_thickness =
 // thickness * (1 / near_clip) (:57, raymarch.slang:597-598).  One function, so the bits do not depend on where they are computed.
 struct ContactShadowConstants {

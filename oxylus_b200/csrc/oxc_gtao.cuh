@@ -32,6 +32,33 @@ struct GtaoParams {
   uint32_t slice_count, samples_per_slice_side, noise_index;
 };
 
+// the packed pyramid (OxcGtaoTargets::depth_mips): level k is max(w >> k, 1) x max(h >> k, 1), the levels one after another.
+// gtao_mip_texels(w, h, k) is level k's offset, and with the default argument the plane's size.
+__host__ inline int gtao_mip_extent(uint32_t n, int k) { return (int)((n >> k) > 1u ? (n >> k) : 1u); }
+__host__ inline long long gtao_mip_texels(uint32_t w, uint32_t h, int levels = GTAO_LEVELS) {
+  long long n = 0;
+  for (int k = 0; k < levels; k++) n += (long long)gtao_mip_extent(w, k) * gtao_mip_extent(h, k);
+  return n;
+}
+
+// the kernels' parameters from the C ABI's arguments (oxc_generate_ambient_occlusion, and the host build of the tests)
+__host__ inline GtaoParams gtao_make_params(const OxcGtaoCamera& cam, const OxcGtaoSettings& st, const float* depth, const float* normals,
+                                            uint32_t w, uint32_t h, const OxcGtaoTargets& t) {
+  GtaoParams p{};
+  p.depth = depth; p.normals = reinterpret_cast<const float4*>(normals);
+  p.mips = t.depth_mips; p.edges = t.edges; p.noisy = t.noisy_occlusion; p.ao = t.ambient_occlusion;
+  p.width = (int)w; p.height = (int)h;
+  for (int k = 0; k < GTAO_LEVELS; k++) {
+    p.mip_w[k] = gtao_mip_extent(w, k); p.mip_h[k] = gtao_mip_extent(h, k); p.mip_off[k] = gtao_mip_texels(w, h, k);
+  }
+  p.m23 = cam.projection[14]; p.m22 = cam.projection[10]; p.p00 = cam.projection[0]; p.p11 = cam.projection[5];
+  for (int i = 0; i < 3; i++) p.view_row[i] = make_float4(cam.view[i], cam.view[4 + i], cam.view[8 + i], cam.view[12 + i]);
+  p.far_clip = cam.far_clip;
+  p.thickness = st.thickness; p.effect_radius = st.effect_radius; p.final_power = st.final_power;
+  p.slice_count = st.slice_count; p.samples_per_slice_side = st.samples_per_slice_side; p.noise_index = st.noise_index;
+  return p;
+}
+
 OXC_DI float gtao_sat(float x) { return vmin(vmax(x, 0.0f), 1.0f); }
 OXC_DI float gtao_sign(float x) { return x > 0.0f ? 1.0f : (x < 0.0f ? -1.0f : 0.0f); }
 OXC_DI uint32_t gtao_u32(float f) { return !(f > 0.0f) ? 0u : (f >= 4294967296.0f ? 0xFFFFFFFFu : (uint32_t)f); }

@@ -66,7 +66,8 @@ __host__ inline PbrParams pbr_make_params(const OxcPbrCamera& cam, const OxcPbrS
   p.flags = st.scene_flags; p.light_count = st.light_count;
   p.depth = in.depth; p.albedo = reinterpret_cast<const float4*>(in.albedo); p.normal = reinterpret_cast<const float4*>(in.normal);
   p.emissive = reinterpret_cast<const float4*>(in.emissive); p.mro = reinterpret_cast<const float4*>(in.metallic_roughness_occlusion);
-  p.ao = in.ambient_occlusion; p.shadow = in.shadow; p.contact = in.contact_shadow;
+  p.ao = in.ambient_occlusion; p.shadow = in.shadow;
+  p.contact = (st.scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS) ? in.contact_shadow : nullptr;
   p.lights = reinterpret_cast<const float4*>(lights); p.out = reinterpret_cast<float4*>(out);
   p.width = (int)w; p.height = (int)h;
   return p;

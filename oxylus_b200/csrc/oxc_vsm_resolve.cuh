@@ -60,6 +60,51 @@ struct VsmResolveParams {
   float texel_length, bias, z_length;
 };
 
+// rmvsm.slang:147-154 get_first_clipmap_texel_length with the oracle's operation order (host floats: IEEE, no contraction)
+__host__ inline float vsm_first_texel_length(const OxcVsmContext& vsm) {
+  volatile float scale_ratio = (float)(vsm.page_table_size - 1) / (float)vsm.page_table_size;
+  volatile float effective_width = vsm.first_clipmap_width * scale_ratio;
+  volatile float twice = effective_width * 2.0f;
+  return twice / vsm.virtual_extent;
+}
+
+// the camera and clipmap fields the page marking (VsmMarkParams) and the resolve (VsmResolveParams) share, from the C ABI's arguments
+template <class P>
+__host__ inline void vsm_fill_view(P& p, const float inv_pv[16], const float resolution[2], const OxcVirtualClipmap* clipmaps,
+                                   const OxcVsmContext& vsm) {
+  for (int i = 0; i < 4; i++) p.inv_pv_row[i] = make_float4(inv_pv[i], inv_pv[4 + i], inv_pv[8 + i], inv_pv[12 + i]);
+  // (1.0 / resolution) * 0.5 with the oracle's operation order (host floats: IEEE, no contraction)
+  p.inv_res_half[0] = (1.0f / resolution[0]) * 0.5f; p.inv_res_half[1] = (1.0f / resolution[1]) * 0.5f;
+  for (int k = 0; k < vsm.clipmap_count; k++) {
+    for (int i = 0; i < 4; i++)
+      for (int j = 0; j < 4; j++) p.clipmap_row[k][i][j] = clipmaps[k].projection_view_mat[j * 4 + i];
+    p.page_offset[k][0] = clipmaps[k].page_offset[0]; p.page_offset[k][1] = clipmaps[k].page_offset[1];
+  }
+  p.texel_length = vsm_first_texel_length(vsm);
+  p.bias = vsm.clipmap_selection_bias;
+}
+
+// the kernel's parameters from the C ABI's arguments (oxc_vsm_resolve_shadows, and the host build of the tests)
+__host__ inline VsmResolveParams vsm_resolve_make_params(const OxcVsmContext& vsm, const float inv_pv[16], const float resolution[2],
+                                                         const OxcVirtualClipmap* clipmaps, const float* depth, const float* normals,
+                                                         const uint32_t* page_tables, const float* atlas, float* shadow) {
+  VsmResolveParams p{};
+  vsm_fill_view(p, inv_pv, resolution, clipmaps, vsm);
+  for (int k = 0; k < vsm.clipmap_count; k++) {
+    const float* m = clipmaps[k].projection_view_mat;
+    p.ortho[k] = m[3] == 0.0f && m[7] == 0.0f && m[11] == 0.0f && m[15] == 1.0f;
+  }
+  for (int i = 0; i < VSM_RESOLVE_BLOCKER_SAMPLES; i++) vsm_hammersley((uint32_t)i, VSM_RESOLVE_BLOCKER_SAMPLES, p.ham[i][0], p.ham[i][1]);
+  for (int i = 0; i < VSM_RESOLVE_PCF_SAMPLES; i++)
+    vsm_hammersley((uint32_t)i, VSM_RESOLVE_PCF_SAMPLES, p.ham[VSM_RESOLVE_BLOCKER_SAMPLES + i][0], p.ham[VSM_RESOLVE_BLOCKER_SAMPLES + i][1]);
+  for (int i = 0; i < 3; i++) p.light[i] = vsm.directional_light_dir[i];
+  p.depth = depth; p.normals = reinterpret_cast<const float4*>(normals); p.page_tables = page_tables; p.atlas = atlas; p.shadow = shadow;
+  p.width = vsm.depth_extent[0]; p.height = vsm.depth_extent[1]; p.size = vsm.page_table_size; p.clipmap_count = vsm.clipmap_count;
+  p.page_size = vsm.page_size; p.atlas_size = vsm.physical_page_table_size; p.phys_per_row = vsm.physical_page_table_size / vsm.page_size;
+  p.z_length = vsm.z_length;
+  return p;
+}
+
 struct VsmBasis { float tx, ty, tz, bx, by, bz; };
 
 // resolve_shadowmaps.slang:77-82 perpendicular_basis: depends only on L

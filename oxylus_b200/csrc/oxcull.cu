@@ -1225,20 +1225,6 @@ int oxc_decode_gbuffer(OxcContext* c, const OxcCullCamera* cam, const uint64_t* 
   return OXC_OK;
 }
 
-} // extern "C"
-
-namespace {
-// rmvsm.slang:147-154 get_first_clipmap_texel_length with the oracle's operation order (host floats: IEEE, no contraction)
-float vsm_first_texel_length(const OxcVsmContext* vsm) {
-  volatile float scale_ratio = (float)(vsm->page_table_size - 1) / (float)vsm->page_table_size;
-  volatile float effective_width = vsm->first_clipmap_width * scale_ratio;
-  volatile float twice = effective_width * 2.0f;
-  return twice / vsm->virtual_extent;
-}
-} // namespace
-
-extern "C" {
-
 int oxc_mark_visible_pages(OxcContext* c, const float inv_pv[16], const float resolution[2], const OxcVirtualClipmap* clipmaps,
                            const OxcVsmContext* vsm, const float* depth_dev, uint32_t* page_tables_dev, uint32_t* page_occupancy_dev,
                            uint32_t* request_count_dev, int32_t* requests_dev, uint32_t request_capacity, void* stream) {
@@ -1249,19 +1235,10 @@ int oxc_mark_visible_pages(OxcContext* c, const float inv_pv[16], const float re
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
   VsmMarkParams p{};
-  for (int i = 0; i < 4; i++) p.inv_pv_row[i] = make_float4(inv_pv[i], inv_pv[4 + i], inv_pv[8 + i], inv_pv[12 + i]);
-  // (1.0 / resolution) * 0.5 and the texel length with the oracle's operation order (host floats: IEEE, no contraction)
-  p.inv_res_half[0] = (1.0f / resolution[0]) * 0.5f; p.inv_res_half[1] = (1.0f / resolution[1]) * 0.5f;
-  for (int k = 0; k < vsm->clipmap_count; k++) {
-    for (int i = 0; i < 4; i++)
-      for (int j = 0; j < 4; j++) p.clipmap_row[k][i][j] = clipmaps[k].projection_view_mat[j * 4 + i];
-    p.page_offset[k][0] = clipmaps[k].page_offset[0]; p.page_offset[k][1] = clipmaps[k].page_offset[1];
-  }
+  vsm_fill_view(p, inv_pv, resolution, clipmaps, *vsm);
   p.depth = depth_dev; p.page_tables = page_tables_dev; p.page_occupancy = page_occupancy_dev; p.request_count = request_count_dev;
   p.requests = requests_dev; p.request_capacity = request_capacity;
   p.width = vsm->depth_extent[0]; p.height = vsm->depth_extent[1]; p.size = vsm->page_table_size; p.clipmap_count = vsm->clipmap_count;
-  p.texel_length = vsm_first_texel_length(vsm);
-  p.bias = vsm->clipmap_selection_bias;
   const dim3 grid((p.width + 31) / 32, (p.height + 7) / 8);
   k_vsm_mark_visible_pages<<<grid, 256, 0, s>>>(p);
   LAUNCHED();
@@ -1482,25 +1459,8 @@ int oxc_vsm_resolve_shadows(OxcContext* c, const OxcVsmContext* vsm, const float
   if (reinterpret_cast<uintptr_t>(normals_dev) & 15u) return fail(OXC_E_INVALID, "normals_dev is not 16-byte aligned (float4 per pixel)");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
-  VsmResolveParams p{};
-  for (int i = 0; i < 4; i++) p.inv_pv_row[i] = make_float4(inv_pv[i], inv_pv[4 + i], inv_pv[8 + i], inv_pv[12 + i]);
-  p.inv_res_half[0] = (1.0f / resolution[0]) * 0.5f; p.inv_res_half[1] = (1.0f / resolution[1]) * 0.5f; // as oxc_mark_visible_pages
-  for (int k = 0; k < vsm->clipmap_count; k++) {
-    const float* m = clipmaps[k].projection_view_mat;
-    for (int i = 0; i < 4; i++)
-      for (int j = 0; j < 4; j++) p.clipmap_row[k][i][j] = m[j * 4 + i];
-    p.page_offset[k][0] = clipmaps[k].page_offset[0]; p.page_offset[k][1] = clipmaps[k].page_offset[1];
-    p.ortho[k] = m[3] == 0.0f && m[7] == 0.0f && m[11] == 0.0f && m[15] == 1.0f;
-  }
-  for (int i = 0; i < VSM_RESOLVE_BLOCKER_SAMPLES; i++) vsm_hammersley((uint32_t)i, VSM_RESOLVE_BLOCKER_SAMPLES, p.ham[i][0], p.ham[i][1]);
-  for (int i = 0; i < VSM_RESOLVE_PCF_SAMPLES; i++)
-    vsm_hammersley((uint32_t)i, VSM_RESOLVE_PCF_SAMPLES, p.ham[VSM_RESOLVE_BLOCKER_SAMPLES + i][0], p.ham[VSM_RESOLVE_BLOCKER_SAMPLES + i][1]);
-  for (int i = 0; i < 3; i++) p.light[i] = vsm->directional_light_dir[i];
-  p.depth = depth_dev; p.normals = reinterpret_cast<const float4*>(normals_dev); p.page_tables = page_tables_dev; p.atlas = physical_atlas_dev;
-  p.shadow = shadow_dev;
-  p.width = vsm->depth_extent[0]; p.height = vsm->depth_extent[1]; p.size = vsm->page_table_size; p.clipmap_count = vsm->clipmap_count;
-  p.page_size = vsm->page_size; p.atlas_size = vsm->physical_page_table_size; p.phys_per_row = vsm->physical_page_table_size / vsm->page_size;
-  p.texel_length = vsm_first_texel_length(vsm); p.bias = vsm->clipmap_selection_bias; p.z_length = vsm->z_length;
+  const VsmResolveParams p = vsm_resolve_make_params(*vsm, inv_pv, resolution, clipmaps, depth_dev, normals_dev, page_tables_dev,
+                                                      physical_atlas_dev, shadow_dev);
   const dim3 grid((p.width + VSM_RESOLVE_TILE_X - 1) / VSM_RESOLVE_TILE_X, (p.height + VSM_RESOLVE_TILE_Y - 1) / VSM_RESOLVE_TILE_Y);
   k_vsm_resolve_shadows<<<grid, VSM_RESOLVE_THREADS, 0, s>>>(p);
   LAUNCHED();
@@ -1524,21 +1484,7 @@ int oxc_generate_ambient_occlusion(OxcContext* c, const OxcGtaoCamera* cam, cons
   if (reinterpret_cast<uintptr_t>(t->noisy_occlusion) & 1u) return fail(OXC_E_INVALID, "noisy_occlusion is not 2-byte aligned");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
-  GtaoParams p{};
-  p.depth = depth_dev; p.normals = reinterpret_cast<const float4*>(normals_dev);
-  p.mips = t->depth_mips; p.edges = t->edges; p.noisy = t->noisy_occlusion; p.ao = t->ambient_occlusion;
-  p.width = (int)w; p.height = (int)h;
-  long long off = 0;
-  for (int k = 0; k < GTAO_LEVELS; k++) {
-    p.mip_w[k] = (int)((w >> k) > 1u ? (w >> k) : 1u); p.mip_h[k] = (int)((h >> k) > 1u ? (h >> k) : 1u);
-    p.mip_off[k] = off;
-    off += (long long)p.mip_w[k] * p.mip_h[k];
-  }
-  p.m23 = cam->projection[14]; p.m22 = cam->projection[10]; p.p00 = cam->projection[0]; p.p11 = cam->projection[5];
-  for (int i = 0; i < 3; i++) p.view_row[i] = make_float4(cam->view[i], cam->view[4 + i], cam->view[8 + i], cam->view[12 + i]);
-  p.far_clip = cam->far_clip;
-  p.thickness = st->thickness; p.effect_radius = st->effect_radius; p.final_power = st->final_power;
-  p.slice_count = st->slice_count; p.samples_per_slice_side = st->samples_per_slice_side; p.noise_index = st->noise_index;
+  const GtaoParams p = gtao_make_params(*cam, *st, depth_dev, normals_dev, w, h, *t);
   const dim3 pre((w + 2 * GTAO_PREFILTER_SIDE - 1) / (2 * GTAO_PREFILTER_SIDE), (h + 2 * GTAO_PREFILTER_SIDE - 1) / (2 * GTAO_PREFILTER_SIDE));
   k_gtao_prefilter<<<pre, dim3(GTAO_PREFILTER_SIDE, GTAO_PREFILTER_SIDE), 0, s>>>(p);
   LAUNCHED();
@@ -1570,8 +1516,7 @@ int oxc_apply_pbr(OxcContext* c, const OxcPbrCamera* cam, const OxcPbrSettings* 
     return fail(OXC_E_INVALID, "depth, ambient_occlusion, shadow and contact_shadow must be 4-byte aligned");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
-  PbrParams p = pbr_make_params(*cam, *st, lights_dev, *in, w, h, out_dev);
-  if (!(st->scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS)) p.contact = nullptr;
+  const PbrParams p = pbr_make_params(*cam, *st, lights_dev, *in, w, h, out_dev);
   const dim3 grid((w + PBR_TILE_X - 1) / PBR_TILE_X, (h + PBR_TILE_Y - 1) / PBR_TILE_Y);
   k_apply_pbr<<<grid, PBR_THREADS, 0, s>>>(p);
   LAUNCHED();
@@ -1589,17 +1534,7 @@ int oxc_contact_shadows(OxcContext* c, const OxcContactShadowCamera* cam, const 
     return fail(OXC_E_INVALID, "depth_dev and out_dev must be 4-byte aligned");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
-  ContactShadowParams p{};
-  p.depth = depth_dev; p.out = out_dev; p.width = (int)w; p.height = (int)h;
-  for (int i = 0; i < 4; i++) {
-    p.inv_pv_row[i] = make_float4(cam->inv_projection_view[i], cam->inv_projection_view[4 + i], cam->inv_projection_view[8 + i],
-                                  cam->inv_projection_view[12 + i]);
-    p.view_row[i] = make_float4(cam->view[i], cam->view[4 + i], cam->view[8 + i], cam->view[12 + i]);
-    p.proj_row[i] = make_float4(cam->projection[i], cam->projection[4 + i], cam->projection[8 + i], cam->projection[12 + i]);
-  }
-  p.near_clip = cam->near_clip;
-  for (int i = 0; i < 3; i++) p.sun[i] = st->sun_direction[i];
-  p.thickness = st->thickness; p.length = st->length; p.steps = st->steps;
+  const ContactShadowParams p = cs_make_params(*cam, *st, depth_dev, w, h, out_dev);
   const dim3 grid((w + CONTACT_TILE_X - 1) / CONTACT_TILE_X, (h + CONTACT_TILE_Y - 1) / CONTACT_TILE_Y);
   k_contact_shadows<<<grid, CONTACT_THREADS, 0, s>>>(p);
   LAUNCHED();

@@ -1,8 +1,8 @@
 // contact_shadows_vs_oracle.cpp — HOST run of the contact-shadow pass's per-pixel source (oxylus_b200/csrc/oxc_contact_shadows.cuh),
 // for the comparison with the oracle's specification (oracle/oxc_oracle_contact_shadows.c) that tests/test_contact_shadows_source_cpu.py
 // makes pixel for pixel, without a GPU.  The device header is compiled for the host through tests/host_shim/ (each __f*_rn intrinsic =
-// one IEEE binary32 operation under -ffp-contract=off).  The parameters are filled the way oxc_contact_shadows fills them.  Test
-// infrastructure only.
+// one IEEE binary32 operation under -ffp-contract=off).  The parameters come from the header's cs_make_params, as in
+// oxc_contact_shadows.  Test infrastructure only.
 //
 //   contact_shadows_vs_oracle <inputs.bin> <outputs.bin>
 // inputs.bin: OxcContactShadowCamera, OxcContactShadowSettings, width u32, height u32, depth[W*H] f32; outputs.bin receives out[W*H] f32.
@@ -27,18 +27,7 @@ int main(int argc, char** argv) {
   std::vector<float> depth((size_t)W * H), out((size_t)W * H);
   if (std::fread(depth.data(), 4, depth.size(), f) != depth.size()) return 2;
   std::fclose(f);
-  // oxcull.cu oxc_contact_shadows
-  ContactShadowParams p{};
-  p.depth = depth.data(); p.out = out.data(); p.width = (int)W; p.height = (int)H;
-  for (int i = 0; i < 4; i++) {
-    p.inv_pv_row[i] = make_float4(cam.inv_projection_view[i], cam.inv_projection_view[4 + i], cam.inv_projection_view[8 + i],
-                                  cam.inv_projection_view[12 + i]);
-    p.view_row[i] = make_float4(cam.view[i], cam.view[4 + i], cam.view[8 + i], cam.view[12 + i]);
-    p.proj_row[i] = make_float4(cam.projection[i], cam.projection[4 + i], cam.projection[8 + i], cam.projection[12 + i]);
-  }
-  p.near_clip = cam.near_clip;
-  for (int i = 0; i < 3; i++) p.sun[i] = st.sun_direction[i];
-  p.thickness = st.thickness; p.length = st.length; p.steps = st.steps;
+  const ContactShadowParams p = cs_make_params(cam, st, depth.data(), W, H, out.data());
   size_t shadowed = 0;
   for (int y = 0; y < (int)H; y++)
     for (int x = 0; x < (int)W; x++) {

@@ -1,8 +1,8 @@
 // gtao_vs_oracle.cpp — HOST run of the GTAO's per-pixel source (oxylus_b200/csrc/oxc_gtao.cuh), for the comparison with the oracle's
 // specification (oracle/oxc_oracle_gtao.c) that tests/test_gtao_source_cpu.py makes pixel for pixel, without a GPU.  The device header
 // is compiled for the host through tests/host_shim/ (each __f*_rn intrinsic = one IEEE binary32 operation under -ffp-contract=off; the
-// binary64 operations of canonical_sincos / canonical_pow are plain C++ operations under the same flag).  The parameters are filled
-// the way oxc_generate_ambient_occlusion fills them; the pyramid's stored texels come from the header's recursive virtual-pyramid
+// binary64 operations of canonical_sincos / canonical_pow are plain C++ operations under the same flag).  The parameters come
+// from the header's gtao_make_params, as in oxc_generate_ambient_occlusion; the pyramid's stored texels come from the header's recursive virtual-pyramid
 // rule (the prefilter kernel computes the same values in shared memory).  Test infrastructure only.
 //
 //   gtao_vs_oracle <inputs.bin> <outputs.bin>
@@ -29,28 +29,14 @@ int main(int argc, char** argv) {
   OxcGtaoSettings st;
   uint32_t W, H;
   if (!rd(f, &cam, 1) || !rd(f, &st, 1) || !rd(f, &W, 1) || !rd(f, &H, 1)) return 2;
-  std::vector<float> depth((size_t)W * H);
-  std::vector<float4> normals((size_t)W * H);
+  std::vector<float> depth((size_t)W * H), normals((size_t)W * H * 4);
   if (!rd(f, depth.data(), depth.size()) || !rd(f, normals.data(), normals.size())) return 2;
   std::fclose(f);
-  // oxcull.cu oxc_generate_ambient_occlusion
-  GtaoParams p{};
-  p.width = (int)W; p.height = (int)H;
-  long long off = 0;
-  for (int k = 0; k < GTAO_LEVELS; k++) {
-    p.mip_w[k] = (int)((W >> k) > 1u ? (W >> k) : 1u); p.mip_h[k] = (int)((H >> k) > 1u ? (H >> k) : 1u);
-    p.mip_off[k] = off;
-    off += (long long)p.mip_w[k] * p.mip_h[k];
-  }
-  std::vector<float> mips((size_t)off), ao((size_t)W * H);
+  std::vector<float> mips((size_t)gtao_mip_texels(W, H)), ao((size_t)W * H);
   std::vector<uint32_t> edges((size_t)W * H);
   std::vector<uint16_t> noisy((size_t)W * H);
-  p.depth = depth.data(); p.normals = normals.data(); p.mips = mips.data(); p.edges = edges.data(); p.noisy = noisy.data(); p.ao = ao.data();
-  p.m23 = cam.projection[14]; p.m22 = cam.projection[10]; p.p00 = cam.projection[0]; p.p11 = cam.projection[5];
-  for (int i = 0; i < 3; i++) p.view_row[i] = make_float4(cam.view[i], cam.view[4 + i], cam.view[8 + i], cam.view[12 + i]);
-  p.far_clip = cam.far_clip;
-  p.thickness = st.thickness; p.effect_radius = st.effect_radius; p.final_power = st.final_power;
-  p.slice_count = st.slice_count; p.samples_per_slice_side = st.samples_per_slice_side; p.noise_index = st.noise_index;
+  const OxcGtaoTargets t{mips.data(), edges.data(), noisy.data(), ao.data()};
+  const GtaoParams p = gtao_make_params(cam, st, depth.data(), normals.data(), W, H, t);
   float (*const level[GTAO_LEVELS])(const GtaoParams&, long long, long long) = {gtao_virtual_level<0>, gtao_virtual_level<1>, gtao_virtual_level<2>,
                                                                                  gtao_virtual_level<3>, gtao_virtual_level<4>};
   for (int k = 0; k < GTAO_LEVELS; k++)

@@ -44,8 +44,7 @@ int main(int argc, char** argv) {
   in.contact_shadow = (mask & 4u) ? contact.data() : nullptr;
   std::vector<float> out(px * 4);
   // oxcull.cu oxc_apply_pbr
-  PbrParams p = pbr_make_params(cam, st, lights.data(), in, W, H, out.data());
-  if (!(st.scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS)) p.contact = nullptr;
+  const PbrParams p = pbr_make_params(cam, st, lights.data(), in, W, H, out.data());
   // kernels_pbr.cuh k_apply_pbr: the staged lights, then every pixel
   std::vector<PbrLight> staged(st.light_count);
   for (uint32_t i = 0; i < st.light_count; i++) {

@@ -2,18 +2,13 @@
 the oracle (oracle/oxc_oracle_contact_shadows.c) on every pixel, without a GPU: random frames with sky, NaN / Inf / denormal / negative
 depth, steps 1 / 2 / 8 / 64, random and hostile settings, and odd sizes down to 1 x 1.  The nearest tap the header picks from the
 bilinear tap's four texels is covered by the hostile frames.  The GPU tier checks the same source as compiled by nvcc."""
-import os
 import subprocess
-import sys
 
 import numpy as np
 import pytest
 
+from tests.host_harness import compile_harness, skip_without_fma
 from tests.test_gpu_contact_shadows import box_on_plane, contact_camera_for, random_depth, random_settings
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
-
 
 @pytest.fixture(scope="module")
 def co():
@@ -21,14 +16,6 @@ def co():
 
     pyoracle_contact_shadows.build()
     return pyoracle_contact_shadows
-
-
-def _build(tmp_path, extra):
-    exe = str(tmp_path / ("contact_shadows_vs_oracle" + ("_fma" if extra else "")))
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-Wno-unknown-pragmas"] + (extra or ["-ffp-contract=off"]) +
-                          ["-I", os.path.join(ROOT, "tests", "host_shim"), "-I", os.path.join(ROOT, "oxylus_b200", "csrc"),
-                           os.path.join(ROOT, "tests", "contact_shadows_vs_oracle.cpp"), "-o", exe])
-    return exe
 
 
 def _cases():
@@ -68,7 +55,7 @@ def cases():
 
 
 def test_device_source_equals_the_oracle_on_the_host(co, cases, tmp_path):
-    exe = _build(tmp_path, None)
+    exe = compile_harness(tmp_path, "contact_shadows_vs_oracle")
     contact = 0
     for case in cases:
         got = _run(exe, tmp_path, case)
@@ -81,10 +68,8 @@ def test_device_source_equals_the_oracle_on_the_host(co, cases, tmp_path):
 
 def test_the_comparison_is_sensitive_to_contraction(co, cases, tmp_path):
     """the same source built WITH fma contraction disagrees with the oracle: fused multiply-adds break the canonical order"""
-    flags = subprocess.run(["grep", "-c", "fma", "/proc/cpuinfo"], capture_output=True, text=True).stdout.strip()
-    if flags in ("", "0"):
-        pytest.skip("host CPU has no FMA unit")
-    exe = _build(tmp_path, ["-mfma", "-ffp-contract=fast"])
+    skip_without_fma()
+    exe = compile_harness(tmp_path, "contact_shadows_vs_oracle", contract=True)
     differ = 0
     for case in cases:
         got = _run(exe, tmp_path, case)

@@ -5,36 +5,22 @@ operation) and links oracle/liboxc_oracle.so: dequantize_half (all 65 536 inputs
 planes + test, project_aabb, test_occlusion, canonical log2, ceil(log2), the backface determinant; tests/raster_core_vs_oracle.cpp
 does the same for the software raster's per-triangle core (csrc/oxc_raster_core.cuh).  The GPU tier checks the same source as
 compiled by nvcc; this is the CPU-tier half of that statement."""
-import os
 import subprocess
 
-import pytest
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _build(tmp_path, extra, source="device_vs_oracle"):
-    oracle_dir = os.path.join(ROOT, "oracle")
-    if not os.path.exists(os.path.join(oracle_dir, "liboxc_oracle.so")):
-        subprocess.check_call(["make", "-C", oracle_dir])
-    exe = str(tmp_path / (source + ("_x" if extra else "")))
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-Wno-unknown-pragmas"] + (extra or ["-ffp-contract=off"]) +
-                          ["-I", os.path.join(ROOT, "tests", "host_shim"), "-I", os.path.join(ROOT, "oxylus_b200", "csrc"),
-                           os.path.join(ROOT, "tests", source + ".cpp"), "-L", oracle_dir, "-loxc_oracle", f"-Wl,-rpath,{oracle_dir}", "-o", exe])
-    return exe
+from tests.host_harness import compile_harness, skip_without_fma
 
 
 def test_device_headers_equal_the_oracle_on_the_host(orc, tmp_path):
-    res = subprocess.run([_build(tmp_path, None), "300000"], capture_output=True, text=True, timeout=600)
+    exe = compile_harness(tmp_path, "device_vs_oracle", link_oracle=True)
+    res = subprocess.run([exe, "300000"], capture_output=True, text=True, timeout=600)
     assert res.returncode == 0 and res.stdout.strip().endswith("ok"), res.stdout + res.stderr
 
 
 def test_the_comparison_is_sensitive_to_contraction(orc, tmp_path):
     """the same program built WITH fma contraction must disagree: one fused multiply-add anywhere breaks the canonical order"""
-    flags = subprocess.run(["grep", "-c", "fma", "/proc/cpuinfo"], capture_output=True, text=True).stdout.strip()
-    if flags in ("", "0"):
-        pytest.skip("host CPU has no FMA unit")
-    res = subprocess.run([_build(tmp_path, ["-mfma", "-ffp-contract=fast"]), "50000"], capture_output=True, text=True, timeout=600)
+    skip_without_fma()
+    exe = compile_harness(tmp_path, "device_vs_oracle", contract=True, link_oracle=True)
+    res = subprocess.run([exe, "50000"], capture_output=True, text=True, timeout=600)
     assert res.returncode == 1 and "FAILED" in res.stdout
 
 
@@ -42,6 +28,7 @@ def test_raster_core_equals_the_oracle_on_the_host(orc, tmp_path):
     """csrc/oxc_raster_core.cuh (snapping, set-up, 32 / 64-bit stepped and direct edge functions, tie-break, depth, packed max,
     clipping) compiled for the host draws the same images as the oracle's raster specification, pixel for pixel: 300 000 random
     triangles from sub-pixel to screen-filling, shared edges, vertices behind the camera and outside the snap range"""
-    res = subprocess.run([_build(tmp_path, None, "raster_core_vs_oracle"), "300000"], capture_output=True, text=True, timeout=600)
+    exe = compile_harness(tmp_path, "raster_core_vs_oracle", link_oracle=True)
+    res = subprocess.run([exe, "300000"], capture_output=True, text=True, timeout=600)
     assert res.returncode == 0 and res.stdout.strip().endswith("ok"), res.stdout + res.stderr
     assert " 0 differ" in res.stdout and "(0 path disagreements)" in res.stdout and " 0 small-primitive disagreements" in res.stdout

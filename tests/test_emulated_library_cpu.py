@@ -87,39 +87,66 @@ def test_hostile_inputs_on_the_simt_emulator(emulated):
     assert res.returncode == 0 and res.stdout.strip().endswith("ok"), res.stdout[-2000:] + res.stderr[-2000:]
 
 
-def test_gpu_variants_on_the_simt_emulator(emulated):
-    """tests/test_gpu_variants.py: all nine k_cull_meshlets instantiations over three pyramid states, every flag subset and a second
-    camera, the occlusion toggle across frames, the mesh-level flags and the automatic shard id base, mixed cameras through the
-    raster and the triangle cull.  Its hostile frames are the torture script's, which test_hostile_inputs_on_the_simt_emulator runs."""
-    res = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", "test_gpu_variants.py"), "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider",
-                          "-k", "not hostile_frames"], cwd=ROOT, env=emulated, capture_output=True, text=True, timeout=900)
-    m = re.search(r"(\d+) passed", res.stdout)
-    assert res.returncode == 0 and m and int(m.group(1)) >= 18 and "skipped" not in res.stdout, res.stdout[-3000:] + res.stderr[-2000:]
+ORDERS = ("default", "shuffle")  # shuffle: OXC_SIMT_ORDER=shuffle, the emulator resumes the threads of a block in a shuffled order
+# Other GPU modules on the emulated library: (module, -k selection or a list of node ids, extra environment, orders, least passed tests
+# (None: every listed node id), timeout).  Each run reproduces the oracle bit for bit under an independent execution model; it says
+# nothing about GPU scheduling, memory ordering or speed.
+GPU_MODULES = [
+    # the VSM page kernels' scans, slot assignment and dirty-list compaction: begin-frame, invalidation, allocation, the 2048^2 dirty-page
+    # clear, the HPB cull on device flags and the refusals; the 8-frame renderer sequence, the 8192^2 clear and the CUDA graph stay on the GPU
+    ("test_gpu_vsm_pages", "not full_size and not graph and not 8192", {}, ORDERS, 10, 900),
+    # the shadow raster's bitmap, work-item split, two-sided set-up, clip path, alpha test and min sink over random tables, an uneven
+    # atlas and the refusals; the 8-frame renderer sequence at 8192^2, the CUDA graph and the renderer frame stay on the GPU
+    ("test_gpu_vsm_draw", "not full_size and not graph and not next_camera", {}, ORDERS, 7, 1800),
+    # the resolve's launch layout (8 x 4 pixel tiles per warp, the per-CTA basis in shared memory), parameters and refusals over all ten
+    # clipmaps in two atlas shapes; the full-size renderer chain, the CUDA graph and the renderer cases stay on the GPU
+    ("test_gpu_vsm_resolve", "random_cases or argument_refusals", {}, ORDERS, 3, 1800),
+    # k_decode_gbuffer's geometry and material halves, launch layout, table building and refusals: one random-table frame from both vis
+    # inputs, bad vertices and materials, the checker quad; the full-size frames, the CUDA graph and the renderer cases stay on the GPU
+    ("test_gpu_gbuffer", ["test_random_tables_bit_exact[1]", "test_bad_material_and_refusals", "test_bad_vertex_index_writes_zeros",
+                          "test_checker_quad_at_texel_centres"], {}, ORDERS, None, 2400),
+    # the three GTAO launches (the prefilter's shared-memory mips 2..4 across its barriers, 8 x 4 pixel tiles per warp), parameters,
+    # refusals and the binary64 restatement on a small ray-cast scene; the full-size cases, the CUDA graph and the renderer frame stay on
+    # the GPU
+    ("test_gpu_gtao", "1x1 or 17x9 or 640x360 or random_settings or all_sky or crease or argument_refusals or analytic_box_211x97", {},
+     ORDERS, 11, 3000),
+    # PBR apply's launch (the lights staged in shared memory across the barrier, 8 x 4 pixel tiles per warp), parameters and refusals
+    # with 0 / 1 / 256 lights; the full-size cases, the CUDA graph and the renderer chain stay on the GPU
+    ("test_gpu_pbr", "1x1 or 17x9 or flag_subsets or null_optional or hostile or emissive_only or out_of_range or sky_and_transparent "
+     "or argument_refusals", {}, ORDERS, 60, 3000),
+    # the contact shadows' launch (8 x 4 pixel tiles per warp, 32 x 8 per CTA), parameters and refusals at the small sizes, every step
+    # count and a box on a plane; the full-size cases, the CUDA graph and the renderer frames stay on the GPU
+    ("test_gpu_contact_shadows", "1x1 or 17x9 or test_steps or random_settings or box_on_plane or argument_refusals", {}, ORDERS, 14,
+     3000),
+    # all nine k_cull_meshlets instantiations over three pyramid states, every flag subset, the occlusion toggle, the mesh-level flags, the
+    # shard id base and mixed cameras through the raster; its hostile frames are the torture script's (test_hostile_inputs_...)
+    ("test_gpu_variants", "not hostile_frames", {}, ("default",), 18, 900),
+    # the shadow-clipmap, multi-view and terrain culls at every shape but the 512 x 512 terrain grid (the Renderer case runs eagerly here)
+    ("test_gpu_culls", "not 512x512", {}, ("default",), 17, 900),
+    # at the emulator's grid (2 SMs, one raster CTA each) 1024 survivors start a pass at 32-meshlet grabs: the stress scene's frames and
+    # variants, the triangle classes and the meshlet-run checks of oxc_set_scene
+    ("test_gpu_raster", None, {"OXC_TEST_RASTER_MIN_SURVIVORS": "1024"}, ORDERS, 9, 600),
+]
 
 
-def test_gpu_culls_on_the_simt_emulator(emulated):
-    """tests/test_gpu_culls.py: the shadow-clipmap cull at every pyramid shape, dirty mask, page offset and clipmap count, steered
-    page edges, shards, the engine's pass order with and without a bound device camera (the Renderer case runs eagerly here: no
-    graph capture), the multi-view cull at 1-16 views, the terrain cull at every grid but 512 x 512, flag subset and Hi-Z state.
-    All 17 of those cases must pass."""
-    res = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", "test_gpu_culls.py"), "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider",
-                          "-k", "not 512x512"], cwd=ROOT, env=emulated, capture_output=True, text=True, timeout=900)
-    m = re.search(r"(\d+) passed", res.stdout)
-    assert res.returncode == 0 and m and int(m.group(1)) >= 17 and "skipped" not in res.stdout, res.stdout[-3000:] + res.stderr[-2000:]
-
-
-@pytest.mark.parametrize("order", ["default", "shuffle"])
-def test_gpu_raster_on_the_simt_emulator(emulated, order):
-    """tests/test_gpu_raster.py at the emulator's grid (2 SMs, one raster CTA each: 1024 survivors start a pass at 32-meshlet
-    grabs): the stress scene's frames and variants against the oracle, the triangle classes and the meshlet-run checks of
-    oxc_set_scene.  Once more with OXC_SIMT_ORDER=shuffle (the emulator resumes the threads of a block in a shuffled order)."""
-    env = dict(emulated, OXC_TEST_RASTER_MIN_SURVIVORS="1024")
+@pytest.mark.parametrize("module,select,extra,order,least,timeout",
+                         [pytest.param(m, sel, extra, order, least, timeout, id=f"{m[len('test_gpu_'):]}-{order}")
+                          for m, sel, extra, orders, least, timeout in GPU_MODULES for order in orders])
+def test_gpu_module_on_the_simt_emulator(emulated, module, select, extra, order, least, timeout):
+    env = dict(emulated, **extra)
     if order == "shuffle":
         env["OXC_SIMT_ORDER"] = "shuffle"
-    res = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", "test_gpu_raster.py"), "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider"],
-                         cwd=ROOT, env=env, capture_output=True, text=True, timeout=600)
+    path = os.path.join(ROOT, "tests", module + ".py")
+    if isinstance(select, list):
+        args = [path + "::" + c for c in select]
+    else:
+        args = [path] + (["-k", select] if select else [])
+    res = subprocess.run([sys.executable, "-m", "pytest"] + args + ["-m", "gpu", "-q", "-x", "-p", "no:cacheprovider"], cwd=ROOT, env=env,
+                         capture_output=True, text=True, timeout=timeout)
     m = re.search(r"(\d+) passed", res.stdout)
-    assert res.returncode == 0 and m and int(m.group(1)) >= 9 and "skipped" not in res.stdout, res.stdout[-3000:] + res.stderr[-2000:]
+    passed = int(m.group(1)) if m else 0
+    enough = passed == len(select) if least is None else passed >= least
+    assert res.returncode == 0 and enough and "skipped" not in res.stdout, res.stdout[-3000:] + res.stderr[-2000:]
 
 
 def test_gpu_parity_suite_with_hostile_scenes_on_the_simt_emulator(emulated):

@@ -5,16 +5,12 @@ mode, mip chains, odd sizes and negative uv transforms.  The per-pixel geometry 
 tier and the emulated library check the device's geometry half."""
 import os
 import subprocess
-import sys
 
 import numpy as np
 import pytest
 
 from oxylus_b200 import abi, synth
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
-
+from tests.host_harness import compile_harness, skip_without_fma
 
 @pytest.fixture(scope="module")
 def gb():
@@ -22,14 +18,6 @@ def gb():
 
     pyoracle_gbuffer.build()
     return pyoracle_gbuffer
-
-
-def _build(tmp_path, extra):
-    exe = str(tmp_path / ("gbuffer_vs_oracle" + ("_fma" if extra else "")))
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-Wno-unknown-pragmas"] + (extra or ["-ffp-contract=off"]) +
-                          ["-I", os.path.join(ROOT, "tests", "host_shim"), "-I", os.path.join(ROOT, "oxylus_b200", "csrc"),
-                           os.path.join(ROOT, "tests", "gbuffer_vs_oracle.cpp"), "-o", exe])
-    return exe
 
 
 @pytest.fixture(scope="module")
@@ -80,7 +68,7 @@ def _run(exe, tmp_path, fr, name):
 
 
 def test_device_source_equals_the_oracle_on_the_host(frames, tmp_path):
-    exe = _build(tmp_path, None)
+    exe = compile_harness(tmp_path, "gbuffer_vs_oracle")
     for n, fr in enumerate(frames):
         got = _run(exe, tmp_path, fr, f"frame{n}")
         written = fr["mat"] != -1
@@ -95,10 +83,8 @@ def test_device_source_equals_the_oracle_on_the_host(frames, tmp_path):
 
 def test_the_comparison_is_sensitive_to_contraction(frames, tmp_path):
     """the same source built WITH fma contraction disagrees with the oracle: fused multiply-adds break the canonical order"""
-    flags = subprocess.run(["grep", "-c", "fma", "/proc/cpuinfo"], capture_output=True, text=True).stdout.strip()
-    if flags in ("", "0"):
-        pytest.skip("host CPU has no FMA unit")
-    exe = _build(tmp_path, ["-mfma", "-ffp-contract=fast"])
+    skip_without_fma()
+    exe = compile_harness(tmp_path, "gbuffer_vs_oracle", contract=True)
     differ = 0
     for n, fr in enumerate(frames):
         got = _run(exe, tmp_path, fr, f"fma{n}")

@@ -2,19 +2,14 @@
 (oracle/oxc_oracle_gtao.c) on every plane and every pixel, without a GPU: random frames with sky, NaN / Inf / denormal / negative depth,
 non-finite normals, all four presets, random and hostile settings, and odd sizes down to 1 x 1.  The GPU tier checks the same source as
 compiled by nvcc, with the prefilter's shared-memory tiling."""
-import os
 import subprocess
-import sys
 
 import numpy as np
 import pytest
 
 from oxylus_b200 import abi
+from tests.host_harness import compile_harness, skip_without_fma
 from tests.test_gpu_gtao import PLANES, assert_planes_equal, gtao_camera_for, random_frame, random_settings
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
-
 
 @pytest.fixture(scope="module")
 def go():
@@ -22,14 +17,6 @@ def go():
 
     pyoracle_gtao.build()
     return pyoracle_gtao
-
-
-def _build(tmp_path, extra):
-    exe = str(tmp_path / ("gtao_vs_oracle" + ("_fma" if extra else "")))
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-Wno-unknown-pragmas"] + (extra or ["-ffp-contract=off"]) +
-                          ["-I", os.path.join(ROOT, "tests", "host_shim"), "-I", os.path.join(ROOT, "oxylus_b200", "csrc"),
-                           os.path.join(ROOT, "tests", "gtao_vs_oracle.cpp"), "-o", exe])
-    return exe
 
 
 def _cases():
@@ -77,7 +64,7 @@ def cases():
 
 
 def test_device_source_equals_the_oracle_on_the_host(go, cases, tmp_path):
-    exe = _build(tmp_path, None)
+    exe = compile_harness(tmp_path, "gtao_vs_oracle")
     occluded = 0
     for case in cases:
         got, log = _run(exe, tmp_path, case)
@@ -89,10 +76,8 @@ def test_device_source_equals_the_oracle_on_the_host(go, cases, tmp_path):
 
 def test_the_comparison_is_sensitive_to_contraction(go, cases, tmp_path):
     """the same source built WITH fma contraction disagrees with the oracle: fused multiply-adds break the canonical order"""
-    flags = subprocess.run(["grep", "-c", "fma", "/proc/cpuinfo"], capture_output=True, text=True).stdout.strip()
-    if flags in ("", "0"):
-        pytest.skip("host CPU has no FMA unit")
-    exe = _build(tmp_path, ["-mfma", "-ffp-contract=fast"])
+    skip_without_fma()
+    exe = compile_harness(tmp_path, "gtao_vs_oracle", contract=True)
     differ = 0
     for case in cases[4:]:
         got, _ = _run(exe, tmp_path, case)

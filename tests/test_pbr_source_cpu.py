@@ -2,19 +2,14 @@
 (oracle/oxc_oracle_pbr.c) on every pixel, without a GPU: random frames with 0, 1, 17 and 256 mixed lights, every flag the pass reads,
 NULL optional planes and hostile values.  The GPU tier checks the same source as compiled by nvcc, with the lights staged in shared
 memory."""
-import os
 import subprocess
-import sys
 
 import numpy as np
 import pytest
 
 from oxylus_b200 import abi
+from tests.host_harness import compile_harness, skip_without_fma
 from tests.test_gpu_pbr import mixed_lights, random_planes, settings_for
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
-
 
 @pytest.fixture(scope="module")
 def po():
@@ -22,14 +17,6 @@ def po():
 
     pyoracle_pbr.build()
     return pyoracle_pbr
-
-
-def _build(tmp_path, extra):
-    exe = str(tmp_path / ("pbr_vs_oracle" + ("_fma" if extra else "")))
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-Wno-unknown-pragmas"] + (extra or ["-ffp-contract=off"]) +
-                          ["-I", os.path.join(ROOT, "tests", "host_shim"), "-I", os.path.join(ROOT, "oxylus_b200", "csrc"),
-                           os.path.join(ROOT, "tests", "pbr_vs_oracle.cpp"), "-o", exe])
-    return exe
 
 
 def _cases():
@@ -80,7 +67,7 @@ def cases():
 
 
 def test_device_source_equals_the_oracle_on_the_host(po, cases, tmp_path):
-    exe = _build(tmp_path, None)
+    exe = compile_harness(tmp_path, "pbr_vs_oracle")
     lit = 0
     for case in cases:
         got, want = _run(exe, tmp_path, case), _want(po, case)
@@ -92,10 +79,8 @@ def test_device_source_equals_the_oracle_on_the_host(po, cases, tmp_path):
 
 def test_the_comparison_is_sensitive_to_contraction(po, cases, tmp_path):
     """the same source built WITH fma contraction disagrees with the oracle: fused multiply-adds break the canonical order"""
-    flags = subprocess.run(["grep", "-c", "fma", "/proc/cpuinfo"], capture_output=True, text=True).stdout.strip()
-    if flags in ("", "0"):
-        pytest.skip("host CPU has no FMA unit")
-    exe = _build(tmp_path, ["-mfma", "-ffp-contract=fast"])
+    skip_without_fma()
+    exe = compile_harness(tmp_path, "pbr_vs_oracle", contract=True)
     differ = 0
     for case in cases[2:]:
         differ += int((_run(exe, tmp_path, case).view(np.uint32) != _want(po, case).view(np.uint32)).sum())

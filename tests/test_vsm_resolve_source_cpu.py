@@ -2,18 +2,13 @@
 oracle (oracle/oxc_oracle_vsm_resolve.c) pixel for pixel, without a GPU: over 10^6 pixels of random depth (sky, NaN, Inf and
 denormals included), random normals (hostile values included), random clipmaps with uneven page offsets (one not orthographic),
 random tables with addresses beyond the atlas, and random atlases.  The GPU tier checks the same source as compiled by nvcc."""
-import os
 import subprocess
-import sys
 
 import numpy as np
 import pytest
 
 from oxylus_b200 import abi, synth
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
-
+from tests.host_harness import compile_harness, skip_without_fma
 
 @pytest.fixture(scope="module")
 def vr():
@@ -21,14 +16,6 @@ def vr():
 
     pyoracle_vsm_resolve.build()
     return pyoracle_vsm_resolve
-
-
-def _build(tmp_path, extra):
-    exe = str(tmp_path / ("vsm_resolve_vs_oracle" + ("_fma" if extra else "")))
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-Wno-unknown-pragmas"] + (extra or ["-ffp-contract=off"]) +
-                          ["-I", os.path.join(ROOT, "tests", "host_shim"), "-I", os.path.join(ROOT, "oxylus_b200", "csrc"),
-                           os.path.join(ROOT, "tests", "vsm_resolve_vs_oracle.cpp"), "-o", exe])
-    return exe
 
 
 def _cases():
@@ -70,7 +57,7 @@ def cases():
 
 
 def test_device_source_equals_the_oracle_on_the_host(vr, cases, tmp_path):
-    exe = _build(tmp_path, None)
+    exe = compile_harness(tmp_path, "vsm_resolve_vs_oracle")
     pixels = 0
     for case in cases:
         shape, vsm, inv_pv, res, cm, depth, normals, pt, atlas = case
@@ -84,10 +71,8 @@ def test_device_source_equals_the_oracle_on_the_host(vr, cases, tmp_path):
 
 def test_the_comparison_is_sensitive_to_contraction(vr, cases, tmp_path):
     """the same source built WITH fma contraction disagrees with the oracle: fused multiply-adds break the canonical order"""
-    flags = subprocess.run(["grep", "-c", "fma", "/proc/cpuinfo"], capture_output=True, text=True).stdout.strip()
-    if flags in ("", "0"):
-        pytest.skip("host CPU has no FMA unit")
-    exe = _build(tmp_path, ["-mfma", "-ffp-contract=fast"])
+    skip_without_fma()
+    exe = compile_harness(tmp_path, "vsm_resolve_vs_oracle", contract=True)
     differ = 0
     for case in cases:
         shape, vsm, inv_pv, res, cm, depth, normals, pt, atlas = case
