@@ -1012,6 +1012,77 @@ OXC_STATIC_ASSERT(sizeof(OxcContactShadowSettings) == 24, "ContactShadowSettings
 int oxc_contact_shadows(OxcContext* ctx, const OxcContactShadowCamera* camera, const OxcContactShadowSettings* settings, const float* depth_dev,
                         uint32_t width, uint32_t height, float* out_dev, void* stream);
 
+/* Atmosphere lookup tables: the transmittance bake (RendererInstance.cpp:203-226, passes/sky_transmittance.slang) and the per-frame sky
+ * view and aerial perspective (Passes/PBR.cpp:11-50 and :96-140, passes/sky_view.slang and passes/sky_aerial_perspective.slang), with the
+ * sky.slang / common/math.slang functions they call, on the path the reference takes: no multiple-scattering LUT (eval_multiscattering is
+ * false at every call site, so the LUT the reference binds is never sampled), no ground bounce (eval_planet_luminance is false in all three
+ * passes).  Each plane holds binary16 RGBA texels (8 B), row-major, x fastest, then y, then z, at the sizes the record gives:
+ *   transmittance       transmittance_lut_size.xy: (exp(-optical_depth), 1), 1000 march steps per texel;
+ *   sky view            sky_view_lut_size.xy: (L / m, m), m = clamp(max(L.r, L.g, L.b), 2^-14, 65504), 48 steps;
+ *   aerial perspective  aerial_perspective_lut_size.xyz: (L, mean transmittance), 2 (z + 1) steps in slice z.
+ * oxc_atmosphere_sky_luts taps transmittance_dev (as oxc_atmosphere_transmittance wrote it) and writes both per-frame planes in one launch.
+ * No scratch, so both calls are graph-capturable from their first call.  The z sizes of the transmittance and sky-view LUTs and
+ * multiscattering_lut_size are not read; terrain_albedo, aerial_perspective_start_km and aerial_perspective_exposure are read only by the
+ * passes that consume the tables (the record is the engine's, kept whole).
+ * Refused with OXC_E_INVALID, before anything is launched: a NULL argument or plane, a plane not 8-byte aligned, a size the call reads that
+ * is 0 or above 4096 (transmittance x / y for both calls; sky view x / y and aerial perspective x / y / z for oxc_atmosphere_sky_luts), a
+ * sky-view dimension below 2 (from_sub_uvs_to_unit divides by res - 1), an aerial-perspective depth above 256 (so no thread marches more
+ * than 512 steps).  NaN, Inf and denormal atmosphere, camera and sun values are accepted and follow the rules below.
+ * SPECIFICATION (oracle/oxc_oracle_atmosphere.c, bit for bit): IEEE binary32, no contraction, IEEE divide / sqrt, sums and products in
+ * written order, dot(a, b) = (a.x*b.x + a.y*b.y) + a.z*b.z, mul(M, v) row by row in the same order, normalize(v) = v / sqrt(dot(v, v)),
+ * length(v) = sqrt(dot(v, v)), lerp(a, b, t) = a + (b - a) * t, max / min return the other operand for a NaN (equal operands give the
+ * second), clamp(x, a, b) = min(max(x, a), b), safe_sqrt(x) = sqrt(max(0, x)); constants are the binary32 roundings of the shaders'
+ * literals: PI 0x40490FDB, TAU 0x40C90FDB, CAMERA_SCALE_UNIT 0x3C23D70A, PLANET_RADIUS_OFFSET 0x3A83126F, HALF_MIN_NORMAL 0x38800000,
+ * HALF_MAX 0x477FE000, and the folded 1 / (4 PI) = fl(1 / fl(4 * PI)) = 0x3DA2F983, 3 / (16 PI) = 0x3D747645, 1.0 / 3.0 = 0x3EAAAAAB
+ * (4 * PI and 16 * PI are exact, so folding in binary32 or in binary64 with one rounding gives the same bits), 3.0 / 2.0 = 1.5.
+ * Commitments where the shaders leave the outcome open:
+ *   1. exp is canonical_exp (oxc_exact.cuh, binary32 Cody-Waite, within 1 ulp, exp(+-0) = 1, overflow to +inf, underflow through the
+ *      subnormals to +0); cos is canonical_cos; pow(x, 3/2) is canonical_pow; acos (beta, constant per call) is canonical_acos (binary64,
+ *      one rounding), and so are computed once per call: get_eye_pos, h = length((0, y, 0)) = sqrt(fl(y * y)) (not |y|), beta, PI - beta,
+ *      and the four exps of mie_asymmetry of henyey_greenstein_draine_phase.
+ *   2. the sky view divides the moved eye position by h before the move (so above the atmosphere the sun frame is per texel), as written.
+ *   3. Optional<f32>::value of `none` reads 0: the bake takes the exit distance without checking it, which only a record with atmos_radius
+ *      below planet_radius (or NaN) can miss; those texels march 1000 steps of length 0.
+ *   4. the MS * scattering_sum term of sun_luminance is kept with MS = 0, so an infinite or NaN sum gives NaN, as in the shader.
+ *   5. the transmittance tap: x = u * W - 0.5, x0 = floor(x), wx = x - x0 (y likewise), texels x0, x0 + 1 / y0, y0 + 1 with NaN-safe
+ *      saturating indices clamped to the edge, top = a00 + wx * (a10 - a00), bottom likewise, top + wy * (bottom - top), reading the
+ *      binary16 texels exactly: the GTAO's level tap without the 8-bit weight quantisation (deviation, as for the alpha test).
+ *   6. every texel is stored as binary16 RGBA, rounded to nearest even with subnormals kept, +-inf beyond 65504; every NaN as 0x7FFF.
+ *      The aerial perspective does not sanitize: an atmosphere with zero extinction stores 0 / 0 = NaN.
+ *   7. the sky view's max(L, 0) returns 0 for a NaN before sanitize replaces +-inf by 0.
+ *   8. the aerial perspective's per_slice_depth is f32(size.x / size.z) in integers (1 at 32^3, 0 when z > x); its start_depth,
+ *      start_pos and ray_pos are dead (view_height is reassigned before they are read) and not computed.
+ * Texel centres are ((x + 0.5) / W, (y + 0.5) / H).  The loops are bounded by 1000, 48 and 2 (z + 1) <= 512 whatever the values. */
+#define OXC_ATMOSPHERE_MAX_LUT_SIZE 4096u
+#define OXC_ATMOSPHERE_MAX_AERIAL_DEPTH 256u
+typedef struct OxcAtmosphere {      /* GPU::Atmosphere (SceneGPU.hpp:158-181), scalar layout */
+  float rayleigh_scatter[3];
+  float rayleigh_density;
+  float mie_scatter[3];
+  float mie_density;
+  float mie_extinction;
+  float mie_asymmetry;
+  float ozone_absorption[3];
+  float ozone_height;
+  float ozone_thickness;
+  float terrain_albedo[3];
+  float planet_radius;
+  float atmos_radius;
+  float aerial_perspective_start_km;
+  float aerial_perspective_exposure;
+  uint32_t transmittance_lut_size[3];
+  uint32_t sky_view_lut_size[3];
+  uint32_t multiscattering_lut_size[3];
+  uint32_t aerial_perspective_lut_size[3];
+} OxcAtmosphere;
+OXC_STATIC_ASSERT(sizeof(OxcAtmosphere) == 136, "Atmosphere");
+int oxc_atmosphere_transmittance(OxcContext* ctx, const OxcAtmosphere* atmosphere, uint16_t* lut_dev, void* stream);
+/* camera: inv_projection_view and position of the frame's camera (the aerial perspective's ray directions; both passes' eye height);
+ * sun_direction and sun_intensity: DirectionalLight::direction and ::intensity, as given. */
+int oxc_atmosphere_sky_luts(OxcContext* ctx, const OxcAtmosphere* atmosphere, const OxcPbrCamera* camera, const float sun_direction[3],
+                            float sun_intensity, const uint16_t* transmittance_dev, uint16_t* sky_view_dev, uint16_t* aerial_perspective_dev,
+                            void* stream);
+
 int oxc_get_outputs(OxcContext* ctx, OxcOutputs* out);
 /* Instrumentation hook: 128 u64 counters that builds with -DOXC_RASTER_STATS fill (tools/raster_stats.py); zero otherwise. */
 void* oxc_debug_stats_ptr(OxcContext* ctx);
@@ -1166,6 +1237,15 @@ int oxr_apply_pbr_with_contact_shadows(OxrRenderer* r, const OxcCullCamera* came
                                        const OxcLight* lights_host, int cast_shadows, const OxcGtaoCamera* gtao_camera,
                                        const OxcGtaoSettings* gtao_settings, const OxcContactShadowCamera* contact_camera,
                                        const OxcContactShadowSettings* contact_settings, float* rgba_host);
+/* The atmosphere's lookup tables as the reference makes them, on the renderer's stream, synchronous.  At its first call the renderer
+ * allocates its three planes at the reference's extents (transmittance 256 x 64, sky view 312 x 192, aerial perspective 32 x 32 x 32; about
+ * 0.7 MiB) and bakes the transmittance LUT once with the DEFAULT record (GPU::Atmosphere{} with those sizes), as the reference's init does:
+ * a scene's atmosphere never reaches the transmittance LUT.  Every call then runs oxc_atmosphere_sky_luts with a copy of the caller's
+ * record whose four size fields are replaced by the renderer's extents (RendererInstance.cpp:1456-1459), the camera and the sun.  Each
+ * non-NULL host pointer receives its plane (binary16 RGBA, 8 B per texel).  The frame's outputs are left as they were.  OXC_E_CAPACITY,
+ * with the camera path left usable, when the planes cannot be allocated. */
+int oxr_atmosphere_luts(OxrRenderer* r, const OxcAtmosphere* atmosphere, const OxcPbrCamera* camera, const float sun_direction[3],
+                        float sun_intensity, uint16_t* transmittance_host, uint16_t* sky_view_host, uint16_t* aerial_perspective_host);
 
 /* ------------------------------------------------------------------------------------------------
  * oxb_* — mesh builder (SURVEY §8f.2): host-side producer of the blob layout above, mirroring build_gltf_mesh

@@ -467,6 +467,47 @@ def contact_shadow_settings(sun_direction=(0.3, 0.8, 0.52), steps=8, thickness=0
     return s
 
 
+ATMOSPHERE_MAX_LUT_SIZE = 4096
+ATMOSPHERE_MAX_AERIAL_DEPTH = 256
+
+
+class Atmosphere(C.Structure):
+    """OxcAtmosphere (GPU::Atmosphere, SceneGPU.hpp:158-181, scalar layout)"""
+
+    _fields_ = [("rayleigh_scatter", C.c_float * 3), ("rayleigh_density", C.c_float), ("mie_scatter", C.c_float * 3), ("mie_density", C.c_float),
+                ("mie_extinction", C.c_float), ("mie_asymmetry", C.c_float), ("ozone_absorption", C.c_float * 3), ("ozone_height", C.c_float),
+                ("ozone_thickness", C.c_float), ("terrain_albedo", C.c_float * 3), ("planet_radius", C.c_float), ("atmos_radius", C.c_float),
+                ("aerial_perspective_start_km", C.c_float), ("aerial_perspective_exposure", C.c_float),
+                ("transmittance_lut_size", C.c_uint32 * 3), ("sky_view_lut_size", C.c_uint32 * 3), ("multiscattering_lut_size", C.c_uint32 * 3),
+                ("aerial_perspective_lut_size", C.c_uint32 * 3)]
+
+
+assert C.sizeof(Atmosphere) == 136
+
+# GPU::Atmosphere{} (SceneGPU.hpp:158-181) and the reference's LUT extents (RendererInstance.hpp: transmittance 256 x 64, sky view
+# 312 x 192, multiple scattering 32 x 32, aerial perspective 32 x 32 x 32)
+ATMOSPHERE_DEFAULTS = dict(rayleigh_scatter=(0.005802, 0.013558, 0.033100), rayleigh_density=8.0, mie_scatter=(0.003996, 0.003996, 0.003996),
+                           mie_density=1.2, mie_extinction=0.004440, mie_asymmetry=3.6, ozone_absorption=(0.000650, 0.001881, 0.000085),
+                           ozone_height=25.0, ozone_thickness=15.0, terrain_albedo=(0.3, 0.3, 0.3), planet_radius=6360.0, atmos_radius=6460.0,
+                           aerial_perspective_start_km=8.0, aerial_perspective_exposure=1.0, transmittance_lut_size=(256, 64, 1),
+                           sky_view_lut_size=(312, 192, 1), multiscattering_lut_size=(32, 32, 1), aerial_perspective_lut_size=(32, 32, 32))
+
+
+def atmosphere(**overrides):
+    """Atmosphere with the GPU::Atmosphere{} defaults and the reference's LUT sizes; any field may be overridden by name"""
+    a = Atmosphere()
+    for name, value in dict(ATMOSPHERE_DEFAULTS, **overrides).items():
+        if name not in ATMOSPHERE_DEFAULTS:
+            raise TypeError(f"Atmosphere has no field {name}")
+        if name.endswith("_size"):
+            getattr(a, name)[:] = [int(v) for v in value]
+        elif np.ndim(value):
+            getattr(a, name)[:] = [float(np.float32(v)) for v in value]
+        else:
+            setattr(a, name, float(np.float32(value)))
+    return a
+
+
 MESH_MAX_LODS = 8
 
 

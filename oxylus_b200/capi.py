@@ -22,7 +22,7 @@ SYMBOLS = [
     "oxc_decode_visbuffer", "oxc_decode_gbuffer", "oxc_build_hpb", "oxc_mark_visible_pages",
     "oxc_vsm_begin_frame", "oxc_vsm_invalidate_pages", "oxc_vsm_allocate_pages", "oxc_vsm_clear_dirty_pages", "oxc_cull_meshlets_hpb_dirty_dev",
     "oxc_vsm_draw_pages", "oxc_vsm_draw_stats", "oxc_vsm_resolve_shadows", "oxc_generate_ambient_occlusion", "oxc_apply_pbr",
-    "oxc_contact_shadows",
+    "oxc_contact_shadows", "oxc_atmosphere_transmittance", "oxc_atmosphere_sky_luts",
     "oxc_get_outputs", "oxc_check_status", "oxc_mark_hiz_dirty", "oxc_bind_camera_buffer", "oxc_load_camera", "oxc_debug_stats_ptr",
     "oxc_mgpu_get_unique_id", "oxc_mgpu_init", "oxc_mgpu_init_with_comm", "oxc_mgpu_shutdown", "oxc_mgpu_info", "oxc_mgpu_exchange_hiz",
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
@@ -30,6 +30,7 @@ SYMBOLS = [
     "oxr_create", "oxr_destroy", "oxr_context", "oxr_update", "oxr_update_transforms", "oxr_set_external_depth", "oxr_set_materials", "oxr_overdraw", "oxr_render", "oxr_submit", "oxr_wait",
     "oxr_vsm_update_pages", "oxr_vsm_pages", "oxr_vsm_draw_shadows", "oxr_vsm_resolve_shadows", "oxr_decode_gbuffer",
     "oxr_generate_ambient_occlusion", "oxr_apply_pbr", "oxr_contact_shadows", "oxr_apply_pbr_with_contact_shadows",
+    "oxr_atmosphere_luts",
 ]
 
 
@@ -155,6 +156,9 @@ def load(build_if_missing=True):
     lib.oxr_contact_shadows.argtypes = [vp, C.POINTER(abi.ContactShadowCamera), C.POINTER(abi.ContactShadowSettings), vp]
     lib.oxr_apply_pbr_with_contact_shadows.argtypes = [vp, vp, C.POINTER(abi.PbrCamera), C.POINTER(abi.PbrSettings), vp, C.c_int, vp, vp,
                                                        vp, vp, vp]
+    lib.oxc_atmosphere_transmittance.argtypes = [vp, C.POINTER(abi.Atmosphere), vp, vp]
+    lib.oxc_atmosphere_sky_luts.argtypes = [vp, C.POINTER(abi.Atmosphere), C.POINTER(abi.PbrCamera), vp, C.c_float, vp, vp, vp, vp]
+    lib.oxr_atmosphere_luts.argtypes = [vp, C.POINTER(abi.Atmosphere), C.POINTER(abi.PbrCamera), vp, C.c_float, vp, vp, vp]
     _LIB = lib
     return lib
 
@@ -509,6 +513,18 @@ class Context:
         _check(self.lib.oxc_apply_pbr(self.h, C.byref(pbr_camera), C.byref(settings), _ptr(lights_dev), C.byref(t), w, h, _ptr(out_dev),
                                       self.stream), "oxc_apply_pbr")
 
+    def atmosphere_transmittance(self, atmosphere, lut_dev):
+        """oxc_atmosphere_transmittance: the transmittance LUT (binary16 RGBA, atmosphere.transmittance_lut_size) into lut_dev"""
+        _check(self.lib.oxc_atmosphere_transmittance(self.h, C.byref(atmosphere), _ptr(lut_dev), self.stream), "oxc_atmosphere_transmittance")
+
+    def atmosphere_sky_luts(self, atmosphere, camera, sun_direction, sun_intensity, transmittance_dev, sky_view_dev, aerial_perspective_dev):
+        """oxc_atmosphere_sky_luts: the sky-view and aerial-perspective LUTs (binary16 RGBA) over the transmittance LUT.  camera:
+        abi.PbrCamera; sun_direction: 3 floats, as given"""
+        sun = (C.c_float * 3)(*[float(np.float32(v)) for v in sun_direction])
+        _check(self.lib.oxc_atmosphere_sky_luts(self.h, C.byref(atmosphere), C.byref(camera), sun, float(np.float32(sun_intensity)),
+                                                _ptr(transmittance_dev), _ptr(sky_view_dev), _ptr(aerial_perspective_dev), self.stream),
+               "oxc_atmosphere_sky_luts")
+
     def contact_shadows(self, contact_camera, settings, depth_dev, w, h, out_dev):
         """oxc_contact_shadows: 1 - the contact shadow (f32 per pixel) of a w x h frame into out_dev.  contact_camera / settings:
         abi.ContactShadowCamera / abi.ContactShadowSettings"""
@@ -777,6 +793,18 @@ class Renderer:
         out = np.zeros((self.scene.height, self.scene.width), dtype=np.float32)
         _check(self.lib.oxr_contact_shadows(self.h, C.byref(contact_camera), C.byref(settings), _ptr(out)), "oxr_contact_shadows")
         return out
+
+    def atmosphere_luts(self, atmosphere, camera, sun_direction, sun_intensity):
+        """oxr_atmosphere_luts: (transmittance [64, 256, 4], sky view [192, 312, 4], aerial perspective [32, 32, 32, 4]) as float16
+        arrays.  The transmittance LUT is the renderer's bake with the default record; the per-frame LUTs use `atmosphere` (abi.Atmosphere,
+        its sizes replaced by the renderer's), camera (abi.PbrCamera) and the sun"""
+        t = np.zeros((64, 256, 4), np.float16)
+        sv = np.zeros((192, 312, 4), np.float16)
+        ap = np.zeros((32, 32, 32, 4), np.float16)
+        sun = (C.c_float * 3)(*[float(np.float32(v)) for v in sun_direction])
+        _check(self.lib.oxr_atmosphere_luts(self.h, C.byref(atmosphere), C.byref(camera), sun, float(np.float32(sun_intensity)), _ptr(t),
+                                            _ptr(sv), _ptr(ap)), "oxr_atmosphere_luts")
+        return t, sv, ap
 
     def apply_pbr(self, cam, settings, lights=None, cast_shadows=False, gtao_camera=None, gtao_settings=None, pbr_camera=None,
                   contact_camera=None, contact_settings=None):

@@ -102,7 +102,7 @@ RendererInstance::RendererInstance(int device, const OxcCreateInfo& info, uint32
 RendererInstance::~RendererInstance() {
   if (stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(stream_));
   cudaFree(d_vis64_); cudaFree(d_vis32_); cudaFree(d_depth_); cudaFree(d_occluder_); cudaFree(d_overdraw_); cudaFree(d_gbuffer_);
-  cudaFree(d_uv_normal_); cudaFree(d_gtao_); cudaFree(d_pbr_); cudaFree(d_lights_); cudaFree(d_contact_);
+  cudaFree(d_uv_normal_); cudaFree(d_gtao_); cudaFree(d_pbr_); cudaFree(d_lights_); cudaFree(d_contact_); cudaFree(d_atmosphere_);
   if (h_pinned_) cudaFreeHost(h_pinned_);
   if (copy_stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(copy_stream_));
   for (auto& sl : slots_) {
@@ -508,6 +508,50 @@ auto RendererInstance::contact_shadows(const OxcContactShadowCamera& contact_cam
   if ((rc = contact_shadows_device(contact_camera, settings)) != OXC_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream_);
   if (cudaMemcpyAsync(contact_host, d_contact_, (size_t)width_ * height_ * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+      cudaStreamSynchronize(s) != cudaSuccess)
+    return fail(OXC_E_CUDA);
+  return OXC_OK;
+}
+
+// the atmosphere's LUTs on stream_, synchronous: the bake once with the default record (RendererInstance.cpp:203-226), then the two
+// per-frame LUTs with the caller's record at the renderer's extents (:1456-1459, PBR.cpp:11-50 and :96-140)
+auto RendererInstance::atmosphere_luts(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3],
+                                       float sun_intensity, uint16_t* transmittance_host, uint16_t* sky_view_host,
+                                       uint16_t* aerial_perspective_host) -> int {
+  if (!ctx_ || !error_.empty()) return OXC_E_STATE;
+  if (!sun_direction) return OXC_E_INVALID;
+  const size_t t_texels = (size_t)kTransmittanceLut[0] * kTransmittanceLut[1], sv_texels = (size_t)kSkyViewLut[0] * kSkyViewLut[1];
+  const size_t ap_texels = (size_t)kAerialLut[0] * kAerialLut[1] * kAerialLut[2];
+  if (!d_atmosphere_ && cudaMalloc(reinterpret_cast<void**>(&d_atmosphere_), (t_texels + sv_texels + ap_texels) * 8) != cudaSuccess) {
+    cudaGetLastError();
+    d_atmosphere_ = nullptr;
+    return OXC_E_CAPACITY; // an optional part: the camera path stays usable
+  }
+  uint16_t* d_t = d_atmosphere_;
+  uint16_t* d_sv = d_t + t_texels * 4;
+  uint16_t* d_ap = d_sv + sv_texels * 4;
+  OxcAtmosphere sized = atmosphere;
+  sized.transmittance_lut_size[0] = kTransmittanceLut[0]; sized.transmittance_lut_size[1] = kTransmittanceLut[1];
+  sized.transmittance_lut_size[2] = 1;
+  sized.sky_view_lut_size[0] = kSkyViewLut[0]; sized.sky_view_lut_size[1] = kSkyViewLut[1]; sized.sky_view_lut_size[2] = 1;
+  sized.multiscattering_lut_size[0] = kMultiscatteringLut[0]; sized.multiscattering_lut_size[1] = kMultiscatteringLut[1];
+  sized.multiscattering_lut_size[2] = 1;
+  for (int i = 0; i < 3; i++) sized.aerial_perspective_lut_size[i] = kAerialLut[i];
+  int rc;
+  if (!transmittance_baked_) {
+    // GPU::Atmosphere{} with only the transmittance and multiple-scattering sizes set, as the reference's init bakes it
+    OxcAtmosphere def = {{0.005802f, 0.013558f, 0.033100f}, 8.0f, {0.003996f, 0.003996f, 0.003996f}, 1.2f, 0.004440f, 3.6f,
+                         {0.000650f, 0.001881f, 0.000085f}, 25.0f, 15.0f, {0.3f, 0.3f, 0.3f}, 6360.0f, 6460.0f, 8.0f, 1.0f,
+                         {kTransmittanceLut[0], kTransmittanceLut[1], 1}, {0, 0, 0}, {kMultiscatteringLut[0], kMultiscatteringLut[1], 1},
+                         {0, 0, 0}};
+    if ((rc = oxc_atmosphere_transmittance(ctx_, &def, d_t, stream_)) != OXC_OK) return fail(rc);
+    transmittance_baked_ = true;
+  }
+  if ((rc = oxc_atmosphere_sky_luts(ctx_, &sized, &camera, sun_direction, sun_intensity, d_t, d_sv, d_ap, stream_)) != OXC_OK) return fail(rc);
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  if ((transmittance_host && cudaMemcpyAsync(transmittance_host, d_t, t_texels * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
+      (sky_view_host && cudaMemcpyAsync(sky_view_host, d_sv, sv_texels * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
+      (aerial_perspective_host && cudaMemcpyAsync(aerial_perspective_host, d_ap, ap_texels * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
       cudaStreamSynchronize(s) != cudaSuccess)
     return fail(OXC_E_CUDA);
   return OXC_OK;
@@ -1035,6 +1079,12 @@ int oxr_apply_pbr(OxrRenderer* r, const OxcCullCamera* camera, const OxcPbrCamer
   // HasContactShadows needs the contact-shadow pass's camera and settings: oxr_apply_pbr_with_contact_shadows takes them
   if (settings->scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS) return OXC_E_INVALID;
   return r->impl.apply_pbr(*camera, *pbr_camera, *settings, lights_host, cast_shadows != 0, gtao_camera, gtao_settings, rgba_host);
+}
+
+int oxr_atmosphere_luts(OxrRenderer* r, const OxcAtmosphere* atmosphere, const OxcPbrCamera* camera, const float sun_direction[3],
+                        float sun_intensity, uint16_t* transmittance_host, uint16_t* sky_view_host, uint16_t* aerial_perspective_host) {
+  if (!r || !atmosphere || !camera || !sun_direction) return OXC_E_INVALID;
+  return r->impl.atmosphere_luts(*atmosphere, *camera, sun_direction, sun_intensity, transmittance_host, sky_view_host, aerial_perspective_host);
 }
 
 int oxr_contact_shadows(OxrRenderer* r, const OxcContactShadowCamera* contact_camera, const OxcContactShadowSettings* settings,

@@ -93,6 +93,10 @@ public:
                  const OxcContactShadowCamera* contact_camera = nullptr, const OxcContactShadowSettings* contact_settings = nullptr) -> int;
   // the contact_shadows pass (RendererInstance.cpp:990-1020) on the last rendered frame's depth; width x height floats to the host
   auto contact_shadows(const OxcContactShadowCamera& contact_camera, const OxcContactShadowSettings& settings, float* contact_host) -> int;
+  // the atmosphere's LUTs (RendererInstance.cpp:203-226 bake with the default record, once; PBR.cpp:11-50 and :96-140 per call with
+  // the caller's record at the renderer's extents); each non-null host pointer receives its binary16 RGBA plane
+  auto atmosphere_luts(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3], float sun_intensity,
+                       uint16_t* transmittance_host, uint16_t* sky_view_host, uint16_t* aerial_perspective_host) -> int;
 
   // RendererInstance::render geometry section: run_geometry_pass(false) -> generate_hiz -> run_geometry_pass(true)
   auto render(const OxcCullCamera& camera, const float* occluder_depth_host, uint32_t* vis32_host, float* depth_host,
@@ -179,6 +183,12 @@ private:
   int contact_plane();              // allocates d_contact_ when missing: OXC_OK or OXC_E_CAPACITY
   // the frame's depth, then the contact-shadow pass into d_contact_, enqueued on stream_ without a copy
   int contact_shadows_device(const OxcContactShadowCamera& contact_camera, const OxcContactShadowSettings& settings);
+  // the atmosphere's LUTs at the reference's extents (RendererInstance.hpp: 256 x 64, 312 x 192, 32 x 32 x 32), binary16 RGBA, allocated
+  // by the first atmosphere_luts; the transmittance LUT is baked once, with the default record
+  static constexpr uint32_t kTransmittanceLut[2] = {256, 64}, kSkyViewLut[2] = {312, 192}, kMultiscatteringLut[2] = {32, 32},
+                            kAerialLut[3] = {32, 32, 32};
+  uint16_t* d_atmosphere_ = nullptr; // transmittance, then sky view, then aerial perspective
+  bool transmittance_baked_ = false;
   OxcLight* d_lights_ = nullptr;    // apply_pbr's lights buffer (OXC_MAX_LIGHTS records), allocated with d_pbr_
   bool has_external_depth_ = false;
   // transforms as the host last uploaded them, and on the device the values before the upload that last changed each of them

@@ -6,6 +6,7 @@
 // Reference lines: Oxylus/src/Render/Shaders/cull.slang, scene.slang, common/math.slang.
 #pragma once
 #include <cuda_fp16.h>
+#include <string.h>
 
 #include "oxc_types.cuh"
 
@@ -383,6 +384,93 @@ OXC_DI float canonical_pow5(float xf) {
   const double x = (double)xf;
   const double x2 = dmul64(x, x);
   return d2f_rn(dmul64(dmul64(x2, x2), x));
+}
+
+// binary32 operations for functions the parameter builders also call on the host: the device intrinsics, or one IEEE operation in the
+// host code (compiled with -ffp-contract=off, as the library's host code is)
+#define OXC_HD __host__ __device__ __forceinline__
+OXC_HD float hd_mul(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+OXC_HD float hd_add(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+OXC_HD float hd_sub(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fsub_rn(a, b);
+#else
+  return a - b;
+#endif
+}
+OXC_HD float hd_pow2(int k) { // 2^k for k in -126..127, from its bits
+  const uint32_t u = (uint32_t)(k + 127) << 23;
+#ifdef __CUDA_ARCH__
+  return __uint_as_float(u);
+#else
+  float f;
+  memcpy(&f, &u, 4);
+  return f;
+#endif
+}
+
+// exp in binary32 for the atmosphere's media (sky.slang:134-135, :231), bit-identical to oracle/oxc_oracle_atmosphere.c
+// orc_exp_canonical.  Cody-Waite: k = rint(x * fl(log2 e)), r = (x - k * LN2_HI) - k * LN2_LO with LN2_HI = 0.693359375 (9 significant
+// bits, so k * LN2_HI is exact for every k reached, and x - k * LN2_HI is exact by Sterbenz), exp(r) = 1 + (r + r^2 * q(r)) with q the
+// Taylor polynomial to r^8 / 8! by Horner, then the bits of 2^k: one multiplication for k in -126..127, two for k = 128 (the first
+// exact) and for k < -126 (the first exact, the second rounds once into the subnormals).  Error: at most 1 ulp against the exact
+// exp over all binary32 inputs (tests/test_oracle_atmosphere.py checks 10^7 inputs against binary64); exp(+-0) = 1 exactly, x > 89
+// and +inf give +inf, x < -104 and -inf give +0, NaN stays NaN (the input's bits).
+OXC_HD float canonical_exp(float x) {
+  if (x != x) return x;
+  if (x > 89.0f) return hd_mul(hd_pow2(127), hd_pow2(127)); // +inf
+  if (x < -104.0f) return 0.0f;
+  const float k = rintf(hd_mul(x, 1.44269502f));
+  const float r = hd_sub(hd_sub(x, hd_mul(k, 0.693359375f)), hd_mul(k, -2.12194440e-4f));
+  float q = 2.48015873e-05f;               // 1/8!
+  q = hd_add(1.98412701e-04f, hd_mul(r, q)); // 1/7!
+  q = hd_add(1.38888892e-03f, hd_mul(r, q)); // 1/6!
+  q = hd_add(8.33333377e-03f, hd_mul(r, q)); // 1/5!
+  q = hd_add(4.16666679e-02f, hd_mul(r, q)); // 1/4!
+  q = hd_add(1.66666672e-01f, hd_mul(r, q)); // 1/3!
+  q = hd_add(0.5f, hd_mul(r, q));
+  const float p = hd_add(1.0f, hd_add(r, hd_mul(hd_mul(r, r), q)));
+  const int ki = (int)k;
+  if (ki > 127) return hd_mul(hd_mul(p, hd_pow2(127)), hd_pow2(ki - 127));
+  if (ki < -126) return hd_mul(hd_mul(p, hd_pow2(ki + 100)), hd_pow2(-100));
+  return hd_mul(p, hd_pow2(ki));
+}
+
+// acos for the parameter builders (the sky view's beta, sky.slang:76), bit-identical to oracle/oxc_oracle_atmosphere.c
+// orc_acos_canonical.  Binary64 throughout, one rounding to binary32: for |x| <= 1/2, pi/2 - asin(x); above, 2 asin(sqrt((1 - |x|) / 2))
+// (x > 0) or pi - that (x < 0); asin(s) = s + s z P(z), z = s^2 <= 1/4, by its series to s^57 (coefficients by their recurrence in
+// binary64).  Before the rounding the error is a few units of 2^-53 relative, so the result is within 1 ulp of the exact acos.
+// |x| > 1 and NaN give NaN.  Host code only: the builders run it once per call.
+__host__ inline float canonical_acos(float xf) {
+  const double x = (double)xf;
+  if (!(x >= -1.0 && x <= 1.0)) return __builtin_nanf("");
+  const double a = x < 0.0 ? -x : x;
+  const double s = a <= 0.5 ? x : sqrt((1.0 - a) * 0.5);
+  double c[29];
+  double central = 1.0; // (2n)! / (4^n (n!)^2)
+  for (int n = 0; n < 29; n++) {
+    if (n > 0) central = central * (double)(2 * n - 1) / (double)(2 * n);
+    c[n] = central / (double)(2 * n + 1);
+  }
+  const double z = s * s;
+  double p = c[28];
+  for (int n = 27; n >= 1; n--) p = c[n] + z * p;
+  const double as = s + (s * z) * p;
+  const double PI_D = 3.141592653589793116;
+  if (a <= 0.5) return (float)(PI_D * 0.5 - as);
+  return (float)(x > 0.0 ? 2.0 * as : PI_D - 2.0 * as);
 }
 
 // cull.slang:169-171: determinant(f32x3x3(c0.xyw, c1.xyw, c2.xyw)) >= 0.0001

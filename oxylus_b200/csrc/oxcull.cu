@@ -28,6 +28,7 @@
 #include "kernels_gtao.cuh"
 #include "kernels_pbr.cuh"
 #include "kernels_contact_shadows.cuh"
+#include "kernels_atmosphere.cuh"
 
 using namespace oxc;
 
@@ -1537,6 +1538,61 @@ int oxc_contact_shadows(OxcContext* c, const OxcContactShadowCamera* cam, const 
   const ContactShadowParams p = cs_make_params(*cam, *st, depth_dev, w, h, out_dev);
   const dim3 grid((w + CONTACT_TILE_X - 1) / CONTACT_TILE_X, (h + CONTACT_TILE_Y - 1) / CONTACT_TILE_Y);
   k_contact_shadows<<<grid, CONTACT_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+// the sizes a call reads: 1..4096 (the transmittance LUT's x / y for both calls)
+static int atmosphere_check_sizes(const OxcAtmosphere& a, bool per_frame) {
+  const uint32_t* t = a.transmittance_lut_size;
+  if (t[0] == 0 || t[1] == 0 || t[0] > OXC_ATMOSPHERE_MAX_LUT_SIZE || t[1] > OXC_ATMOSPHERE_MAX_LUT_SIZE)
+    return fail(OXC_E_INVALID, "transmittance_lut_size %u x %u outside 1..%u", t[0], t[1], OXC_ATMOSPHERE_MAX_LUT_SIZE);
+  if (!per_frame) return OXC_OK;
+  const uint32_t* v = a.sky_view_lut_size;
+  if (v[0] < 2 || v[1] < 2 || v[0] > OXC_ATMOSPHERE_MAX_LUT_SIZE || v[1] > OXC_ATMOSPHERE_MAX_LUT_SIZE)
+    return fail(OXC_E_INVALID, "sky_view_lut_size %u x %u outside 2..%u", v[0], v[1], OXC_ATMOSPHERE_MAX_LUT_SIZE);
+  const uint32_t* ap = a.aerial_perspective_lut_size;
+  if (ap[0] == 0 || ap[1] == 0 || ap[2] == 0 || ap[0] > OXC_ATMOSPHERE_MAX_LUT_SIZE || ap[1] > OXC_ATMOSPHERE_MAX_LUT_SIZE ||
+      ap[2] > OXC_ATMOSPHERE_MAX_AERIAL_DEPTH)
+    return fail(OXC_E_INVALID, "aerial_perspective_lut_size %u x %u x %u outside 1..%u x 1..%u x 1..%u", ap[0], ap[1], ap[2],
+                OXC_ATMOSPHERE_MAX_LUT_SIZE, OXC_ATMOSPHERE_MAX_LUT_SIZE, OXC_ATMOSPHERE_MAX_AERIAL_DEPTH);
+  return OXC_OK;
+}
+
+int oxc_atmosphere_transmittance(OxcContext* c, const OxcAtmosphere* atmosphere, uint16_t* lut_dev, void* stream) {
+  if (!c || !atmosphere || !lut_dev) return fail(OXC_E_INVALID, "null argument");
+  if (reinterpret_cast<uintptr_t>(lut_dev) & 7u) return fail(OXC_E_INVALID, "lut_dev must be 8-byte aligned");
+  int rc;
+  if ((rc = atmosphere_check_sizes(*atmosphere, false)) != OXC_OK) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  const AtmosphereParams p = atmosphere_make_params(*atmosphere, nullptr, nullptr, 0.0f, nullptr, lut_dev, nullptr, nullptr, 0);
+  const size_t texels = (size_t)p.t_w * p.t_h;
+  k_atmosphere_transmittance<<<(unsigned)((texels + ATMOSPHERE_THREADS - 1) / ATMOSPHERE_THREADS), ATMOSPHERE_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_atmosphere_sky_luts(OxcContext* c, const OxcAtmosphere* atmosphere, const OxcPbrCamera* camera, const float sun_direction[3],
+                            float sun_intensity, const uint16_t* transmittance_dev, uint16_t* sky_view_dev, uint16_t* aerial_perspective_dev,
+                            void* stream) {
+  if (!c || !atmosphere || !camera || !sun_direction || !transmittance_dev || !sky_view_dev || !aerial_perspective_dev)
+    return fail(OXC_E_INVALID, "null argument");
+  if ((reinterpret_cast<uintptr_t>(transmittance_dev) | reinterpret_cast<uintptr_t>(sky_view_dev) |
+       reinterpret_cast<uintptr_t>(aerial_perspective_dev)) & 7u)
+    return fail(OXC_E_INVALID, "transmittance_dev, sky_view_dev and aerial_perspective_dev must be 8-byte aligned");
+  int rc;
+  if ((rc = atmosphere_check_sizes(*atmosphere, true)) != OXC_OK) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  const OxcAtmosphere& a = *atmosphere;
+  const size_t sky_texels = (size_t)a.sky_view_lut_size[0] * a.sky_view_lut_size[1];
+  const size_t aerial_texels = (size_t)a.aerial_perspective_lut_size[0] * a.aerial_perspective_lut_size[1] * a.aerial_perspective_lut_size[2];
+  const uint32_t sky_blocks = (uint32_t)((sky_texels + ATMOSPHERE_THREADS - 1) / ATMOSPHERE_THREADS);
+  const uint32_t aerial_blocks = (uint32_t)((aerial_texels + ATMOSPHERE_THREADS - 1) / ATMOSPHERE_THREADS);
+  const AtmosphereParams p = atmosphere_make_params(a, camera, sun_direction, sun_intensity, transmittance_dev, nullptr, sky_view_dev,
+                                                    aerial_perspective_dev, sky_blocks);
+  k_atmosphere_sky_luts<<<sky_blocks + aerial_blocks, ATMOSPHERE_THREADS, 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }
