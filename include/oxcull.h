@@ -248,7 +248,7 @@ enum {
                                            vertex index addresses records past the blob or whose micro index is >= its vertex count */
   OXC_STATUS_SURVIVOR_OVERFLOW = 1 << 2,/* oxc_mgpu_exchange_frame: a rank's survivor list exceeded the gather capacity (truncated) */
   OXC_STATUS_ID_OVERFLOW = 1 << 3,      /* a vis-buffer id did not fit the id bits of the packing (pixel skipped) */
-  OXC_STATUS_CLIP_OVERFLOW = 1 << 5,    /* more triangles crossed the near / guard-band planes than the clip queue holds (2^20): the rest was dropped */
+  OXC_STATUS_CLIP_OVERFLOW = 1 << 5,    /* a triangle across the near / guard-band planes found the raster's deferred queue (2^20 entries) full: the raster still drew it, by a slow second walk over the pass */
   OXC_STATUS_BAD_MATERIAL = 1 << 6,     /* a MeshInstance::material_index outside the table of oxc_set_materials (rasterised as opaque) */
   OXC_STATUS_PEER_TIMEOUT = 1 << 4      /* oxc_mgpu_exchange_hiz: a peer did not raise its flag within 30 s (OXC_MGPU_TIMEOUT_MS); that frame's pyramid is incomplete */
 };
@@ -462,8 +462,8 @@ int oxc_raster_overdraw(OxcContext* ctx, const OxcCullCamera* camera, uint32_t c
 int oxc_clear_overdraw(OxcContext* ctx, uint32_t* overdraw_dev, uint32_t width, uint32_t height, void* stream);
 
 /* Stand-alone clip pass: walks the pass's survivors again and clips / draws exactly the triangles described above.
- * oxc_raster_visbuffer does this by itself since round 2 (it queues those triangles while it rasterises), so a host only needs
- * this entry point after a raster that ran with the queue exhausted (OXC_STATUS_CLIP_OVERFLOW); drawing a triangle twice is
+ * oxc_raster_visbuffer does this by itself (it queues those triangles while it rasterises, and walks the pass again when the
+ * queue overflows), so a host only needs this entry point when it drives the plain raster itself; drawing a triangle twice is
  * harmless (same depth, same id). */
 int oxc_raster_visbuffer_clip_pass(OxcContext* ctx, const OxcCullCamera* camera, uint32_t cull_flags, uint32_t width,
                                    uint32_t height, uint64_t* vis_dev, void* stream);

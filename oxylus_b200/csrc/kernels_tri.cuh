@@ -39,9 +39,9 @@ struct TriParams {
   uint4* big_queue;          // BIG_WORDS/4 uint4 per entry
   uint32_t* big_counters;
   uint32_t big_capacity;
-  uint32_t* clip_queue;      // data words (id << prim_bits | triangle) of the triangles the plain rules drop: clipped by k_raster_clip_queue
-  uint32_t* clip_counter;    // entries pushed; zeroed before every raster launch
-  uint32_t clip_capacity;
+  uint32_t* deferred_queue;  // data words (id << prim_bits | triangle) of the triangles a lane does not draw itself: k_raster_deferred
+  uint32_t* deferred_counter; // entries pushed (keeps counting past the capacity); zeroed before every raster launch
+  uint32_t deferred_capacity;
   uint32_t prim_bits;        // triangle bits of the vis-buffer word: 8 (visbuffer.slang:9-14) or 6 (OxcCreateInfo::wide_ids)
   uint32_t small_primitive_cull; // 1: triangles whose snapped bounding box holds no sample centre are culled before they are counted
   uint32_t* status;          // sticky OXC_STATUS_* bits
@@ -155,8 +155,9 @@ __global__ void __launch_bounds__(TRI_THREADS) k_cull_triangles(const __grid_con
   }
 }
 
-// 3 CTAs / SM (80 registers) rather than 4 (64 registers, more spills in the pixel loop): on H100 SXM at 1 M meshlet
-// instances / 1080p the early raster takes 400-405 instead of 434-440 us, the late one 71-72 instead of 77 us (BASELINE.md 5.2)
+// 3 CTAs / SM: 76 registers without spills.  At 4 (64 registers) the early and late passes store 24 and 44 B of spills, and on an
+// H100 80GB HBM3 (700 W) at 1 M meshlet instances / 1080p the early raster takes 316-319 instead of 312-314 us and the late one
+// 74 instead of 68-70 us (BASELINE.md 5.16); at 5 (48 registers) they store 140 and 164 B of spills.
 #ifndef OXC_RASTER_MIN_BLOCKS
 #define OXC_RASTER_MIN_BLOCKS 3
 #endif
@@ -209,9 +210,17 @@ OXC_DI MeshletHeader bcast_header(const MeshletHeader& h, int src) {
   o.vertex_count = __shfl_sync(0xffffffffu, h.vertex_count, src);
   o.tri_offset = __shfl_sync(0xffffffffu, h.tri_offset, src); o.tri_count = __shfl_sync(0xffffffffu, h.tri_count, src);
   o.micro = reinterpret_cast<const uint32_t*>(__shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(h.micro), src));
-  o.vidx = reinterpret_cast<const uint32_t*>(__shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(h.vidx), src));
+  o.vidx = nullptr; // load_vertex_indices
   o.pos = reinterpret_cast<const uint2*>(__shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(h.pos), src));
   return o;
+}
+
+// the vertex indices of the meshlet whose header lane src holds: lane l loads indices l and l + 32
+OXC_DI void load_vertex_indices(const MeshletHeader& h, int src, uint32_t lane, uint32_t& vi0, uint32_t& vi1) {
+  const uint32_t n = __shfl_sync(0xffffffffu, h.vertex_count, src);
+  const uint32_t* vidx = reinterpret_cast<const uint32_t*>(__shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(h.vidx), src));
+  vi0 = lane < n ? __ldg(&vidx[lane]) : 0u;
+  vi1 = lane + 32u < n ? __ldg(&vidx[lane + 32u]) : 0u;
 }
 
 // ---- deferred large triangles ----
@@ -260,12 +269,7 @@ OXC_DI bool big_push(const TriParams& p, const TriSetup& s, uint32_t data) {
   return true;
 }
 
-constexpr uint32_t BIG_PUSH_ALONE = 4; // chunks a single lane may push by itself
-OXC_DI uint32_t big_chunk_count(const TriSetup& s) {
-  return ((uint32_t)(s.px1 - s.px0) / BIG_CHUNK_W + 1u) * ((uint32_t)(s.py1 - s.py0) / BIG_CHUNK_H + 1u);
-}
-
-// The same push done by a whole warp for ONE triangle (setup already broadcast to every lane): lane l writes chunks l, l + 32, ...
+// The same push done by a whole warp for ONE triangle (every lane holds its setup): lane l writes chunks l, l + 32, ...
 OXC_DI bool big_push_warp(const TriParams& p, const TriSetup& s, uint32_t data, uint32_t lane) {
   const uint32_t cw = (uint32_t)(s.px1 - s.px0) / BIG_CHUNK_W + 1u, ch = (uint32_t)(s.py1 - s.py0) / BIG_CHUNK_H + 1u;
   const uint32_t n = cw * ch;
@@ -285,24 +289,32 @@ OXC_DI bool big_push_warp(const TriParams& p, const TriSetup& s, uint32_t data, 
   return true;
 }
 
-// One warp per queued chunk; the chunk is covered in 8x4-pixel tiles (raster spec steps 5-6).  Chunks are dealt to the warps
-// of the grid round-robin: taking them from a counter costs every warp one same-address atomic, even just to learn that the
-// queue is empty.
+// The whole warp covers the box of one set-up triangle in 8x4-pixel tiles (raster spec steps 5-6).
+OXC_DI void raster_tiles(const TriParams& p, const TriSetup& b, uint32_t data, uint32_t lane) {
+  const int lx = lane & 7, ly = lane >> 3;
+  for (int ty = b.py0; ty <= b.py1; ty += 4)
+    for (int tx = b.px0; tx <= b.px1; tx += 8) {
+      const int px = tx + lx, py = ty + ly;
+      if (px <= b.px1 && py <= b.py1) raster_pixel(b, px, py, data, p.visbuf, p.width);
+    }
+}
+
+// One warp per queued chunk.  Chunks are dealt to the warps of the grid round-robin: taking them from a counter costs every
+// warp one same-address atomic, even just to learn that the queue is empty.
 __global__ void __launch_bounds__(256) k_raster_big(const __grid_constant__ TriParams p) {
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t total = min(p.big_counters[0], p.big_capacity);
-  const int lx = lane & 7, ly = lane >> 3;
   for (uint32_t i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < total; i += gridDim.x * (blockDim.x >> 5)) {
     TriSetup b;
     uint32_t data;
     big_entry_load(p.big_queue + (size_t)i * 4, b, data);
-    for (int ty = b.py0; ty <= b.py1; ty += 4)
-      for (int tx = b.px0; tx <= b.px1; tx += 8) {
-        const int px = tx + lx, py = ty + ly;
-        if (px <= b.px1 && py <= b.py1) raster_pixel(b, px, py, data, p.visbuf, p.width);
-      }
+    raster_tiles(p, b, data, lane);
   }
 }
+
+// A lane draws a set-up triangle itself when its edge functions fit 32 bits and its box holds at most RASTER_BIG_PIXELS
+// pixels; k_raster_deferred draws the others (and clips the triangles with an invalid vertex).
+OXC_DI bool lane_draws(const TriSetup& s) { return s.narrow && (s.px1 - s.px0 + 1) * (s.py1 - s.py0 + 1) <= RASTER_BIG_PIXELS; }
 
 #if defined(OXC_RASTER_STATS) && OXC_RASTER_STATS == 1
 // Statistics build only. Warp-wide, over every lane's v0 (when has0) and v1 (when has1): true when the snapped pixel box of the
@@ -400,15 +412,16 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
     mine.micro = nullptr; mine.vidx = nullptr; mine.pos = nullptr;
     if (lane < nb) mine = fetch_header(p, first + my_survivor, id_base);
     // vertex indices of the first meshlet, prefetched one meshlet ahead from here on
-    MeshletHeader cur = bcast_header(mine, 0);
-    uint32_t vi0 = lane < cur.vertex_count ? __ldg(&cur.vidx[lane]) : 0u;
-    uint32_t vi1 = lane + 32u < cur.vertex_count ? __ldg(&cur.vidx[lane + 32u]) : 0u;
+    uint32_t vi0, vi1;
+    load_vertex_indices(mine, 0, lane, vi0, vi1);
 #ifdef OXC_RASTER_STATS
     if (vi0 + vi1 == 0xFFFFFFFFu) kept++; // keep the loads ahead of the timer read
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_b));
 #endif
     for (uint32_t j = 0; j < nb; j++) {
-      const MeshletHeader w = cur;
+      // broadcast again from lane j rather than carried over from the previous meshlet: a header held across the pixel loops
+      // costs registers the loops need
+      const MeshletHeader w = bcast_header(mine, (int)j);
       {  // words [tri_offset / 4, ...) covering the run: two coalesced loads per warp, in flight during the vertex phase
         const uint32_t n_words = ((w.tri_offset & 3u) + w.tri_count * 3u + 3u) >> 2;
         const uint32_t* src = w.micro + (w.tri_offset >> 2);
@@ -421,11 +434,7 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
       const uint2 q0 = lane < w.vertex_count ? __ldg(&w.pos[vi0]) : make_uint2(0, 0);
       const uint2 q1 = lane + 32u < w.vertex_count ? __ldg(&w.pos[vi1]) : make_uint2(0, 0);
       // ... and the next meshlet's vertex indices, in flight while this one is rasterised
-      if (j + 1 < nb) {
-        cur = bcast_header(mine, (int)(j + 1));
-        vi0 = lane < cur.vertex_count ? __ldg(&cur.vidx[lane]) : 0u;
-        vi1 = lane + 32u < cur.vertex_count ? __ldg(&cur.vidx[lane + 32u]) : 0u;
-      }
+      if (j + 1 < nb) load_vertex_indices(mine, (int)(j + 1), lane, vi0, vi1);
       const InstCull* ic = p.inst + w.inst;
       const float4 r0 = __ldg(&ic->mvp_row[0]), r1 = __ldg(&ic->mvp_row[1]), r2 = __ldg(&ic->mvp_row[2]), r3 = __ldg(&ic->mvp_row[3]);
       // clip = mvp * (pos,1) once per vertex (visbuffer_encode_ms.slang:135-137), then the screen record
@@ -454,7 +463,7 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
         const uint32_t t = lane + 32u * k;
         bool pass = false;
         TriSetup s;
-        bool draw = false;
+        bool draw = false, defer = false, clip = false;
 #if defined(OXC_RASTER_STATS) && OXC_RASTER_STATS == 1
         int why_stat = -1;
 #endif
@@ -469,67 +478,59 @@ __global__ void __launch_bounds__(TRI_THREADS, OXC_RASTER_MIN_BLOCKS) k_raster_v
 #if defined(OXC_RASTER_STATS) && OXC_RASTER_STATS == 1
               why_stat = why;
 #endif
-              draw = why == TRI_DRAW;
+              draw = why == TRI_DRAW && lane_draws(s);
+              // a vertex at w <= 0 / beyond the snap range (clipped later, like a hardware rasteriser would,
+              // DrawGeometry.cpp:104-190), 64-bit edge functions or a large box: k_raster_deferred
+              clip = why == TRI_INVALID_VERTEX;
+              defer = clip || (why == TRI_DRAW && !draw);
               if (why == TRI_NO_SAMPLE && p.small_primitive_cull) pass = false; // north_star small-primitive cull (opt-in)
-              if (why == TRI_INVALID_VERTEX && p.clip_queue) { // a vertex at w <= 0 / beyond the snap range: clipped later, like a
-                const uint32_t slot = atomicAdd(p.clip_counter, 1u); // hardware rasteriser would (DrawGeometry.cpp:104-190)
-                if (slot < p.clip_capacity) p.clip_queue[slot] = (w.gid << p.prim_bits) | t;
-                else atomicOr(p.status, (uint32_t)OXC_STATUS_CLIP_OVERFLOW);
-              }
             }
           }
         }
         kept += pass ? 1u : 0u;
         const uint32_t data = (w.gid << p.prim_bits) | t;
-        const int bw = draw ? s.px1 - s.px0 + 1 : 0, bh = draw ? s.py1 - s.py0 + 1 : 0;
 #if defined(OXC_RASTER_STATS) && OXC_RASTER_STATS == 1
         {  // instrumentation build only: per round (32 triangles) histogram of the LARGEST per-lane pixel loop and the round's sums
-          const int area = (draw && bw * bh <= RASTER_BIG_PIXELS) ? bw * bh : 0;
+          const bool set_up = why_stat == TRI_DRAW;
+          const int bw = set_up ? s.px1 - s.px0 + 1 : 0, bh = set_up ? s.py1 - s.py0 + 1 : 0;
+          const int area = draw ? bw * bh : 0;
           const int mx = __reduce_max_sync(0xffffffffu, area), sm = __reduce_add_sync(0xffffffffu, area);
           const int nd = __popc(__ballot_sync(0xffffffffu, area > 0));
-          const int nbig = __popc(__ballot_sync(0xffffffffu, draw && bw * bh > RASTER_BIG_PIXELS));
+          const int nbig = __popc(__ballot_sync(0xffffffffu, bw * bh > RASTER_BIG_PIXELS));
+          const int nwide = __popc(__ballot_sync(0xffffffffu, set_up && !s.narrow));
+          const int nclip = __popc(__ballot_sync(0xffffffffu, clip));
+          const int ndefer = __popc(__ballot_sync(0xffffffffu, defer));
+          const int nsetup = __popc(__ballot_sync(0xffffffffu, set_up));
           const bool setup_round = __any_sync(0xffffffffu, why_stat == TRI_DRAW || why_stat == TRI_BACK_OR_DEGENERATE);
-          meshlet_draws |= __any_sync(0xffffffffu, draw);
+          meshlet_draws |= __any_sync(0xffffffffu, set_up);
           if (lane == 0) {
             unsigned long long* st = reinterpret_cast<unsigned long long*>(p.big_queue) + (size_t)p.big_capacity * 8 + (p.late ? 64 : 0);
             atomicAdd(&st[min(mx, 33)], 1ull);          // [0..33] histogram of max area
-            atomicAdd(&st[40], (unsigned long long)sm); // total candidate pixels (small path)
+            atomicAdd(&st[40], (unsigned long long)sm); // total candidate pixels (per-lane path)
             atomicAdd(&st[41], (unsigned long long)mx); // sum of per-round maxima
             atomicAdd(&st[42], (unsigned long long)nd); // drawing lanes
             atomicAdd(&st[43], 1ull);                   // rounds
             atomicAdd(&st[44], (unsigned long long)nbig);
             if (setup_round) atomicAdd(&st[47], 1ull); // rounds in which some lane runs the set-up past the bounding box
+            atomicAdd(&st[49], (unsigned long long)nwide);  // set-up triangles that fail narrow
+            atomicAdd(&st[50], (unsigned long long)nclip);  // TRI_INVALID_VERTEX triangles (clipped)
+            atomicAdd(&st[51], (unsigned long long)ndefer); // deferred-queue entries
+            atomicAdd(&st[52], (unsigned long long)nsetup); // set-up triangles (TRI_DRAW)
           }
         }
 #endif
-        bool big = draw && (bw * bh > RASTER_BIG_PIXELS);
-        if (draw && !big) raster_small(s, data, p.visbuf, p.width);
-        // a triangle of a few chunks is pushed by its own lane; one of many chunks (a screen-filling triangle is ~1000) is
-        // pushed by the whole warp below — a single lane writing them all becomes the tail of the raster launch
-        const bool few = big && big_chunk_count(s) <= BIG_PUSH_ALONE;
-        if (few && p.big_queue && big_push(p, s, data)) big = false; // deferred to k_raster_big
-        uint32_t big_mask = __ballot_sync(0xffffffffu, big);
-        while (big_mask) {
-          const int src = __ffs(big_mask) - 1;
-          big_mask &= big_mask - 1;
-          TriSetup b;
-          b.ax = __shfl_sync(0xffffffffu, s.ax, src); b.ay = __shfl_sync(0xffffffffu, s.ay, src);
-          b.bx = __shfl_sync(0xffffffffu, s.bx, src); b.by = __shfl_sync(0xffffffffu, s.by, src);
-          b.cx = __shfl_sync(0xffffffffu, s.cx, src); b.cy = __shfl_sync(0xffffffffu, s.cy, src);
-          b.za = __shfl_sync(0xffffffffu, s.za, src); b.dzb = __shfl_sync(0xffffffffu, s.dzb, src);
-          b.dzc = __shfl_sync(0xffffffffu, s.dzc, src);
-          b.px0 = __shfl_sync(0xffffffffu, s.px0, src); b.px1 = __shfl_sync(0xffffffffu, s.px1, src);
-          b.py0 = __shfl_sync(0xffffffffu, s.py0, src); b.py1 = __shfl_sync(0xffffffffu, s.py1, src);
-          b.bias = __shfl_sync(0xffffffffu, s.bias, src);
-          const uint32_t bdata = __shfl_sync(0xffffffffu, data, src);
-          if (p.big_queue && big_push_warp(p, b, bdata, lane)) continue; // chunks written by all 32 lanes
-          // the queue could not take it: the warp covers the bounding box in 8x4-pixel tiles right here
-          const int lx = lane & 7, ly = lane >> 3;
-          for (int ty = b.py0; ty <= b.py1; ty += 4)
-            for (int tx = b.px0; tx <= b.px1; tx += 8) {
-              const int px = tx + lx, py = ty + ly;
-              if (px <= b.px1 && py <= b.py1) raster_pixel(b, px, py, bdata, p.visbuf, p.width);
-            }
+        if (draw) raster_narrow(s, data, p.visbuf, p.width);
+        // the rest goes to the deferred queue, one atomic per round from the first deferring lane.  Past the capacity the counter
+        // keeps counting, and k_raster_deferred walks the pass again for the triangles the queue could not hold.  A clipped
+        // triangle past it also raises OXC_STATUS_CLIP_OVERFLOW: the queue is too small for the frame, and the walk is slow.
+        const uint32_t defer_mask = __ballot_sync(0xffffffffu, defer);
+        if (defer_mask) {
+          const int leader = __ffs(defer_mask) - 1;
+          uint32_t base = 0;
+          if (lane == (uint32_t)leader) base = atomicAdd(p.deferred_counter, (uint32_t)__popc(defer_mask));
+          const uint32_t slot = __shfl_sync(0xffffffffu, base, leader) + __popc(defer_mask & ((1u << lane) - 1u));
+          if (defer && slot < p.deferred_capacity) p.deferred_queue[slot] = data;
+          else if (clip) atomicOr(p.status, (uint32_t)OXC_STATUS_CLIP_OVERFLOW);
         }
       }
 #if defined(OXC_RASTER_STATS) && OXC_RASTER_STATS == 1
@@ -579,30 +580,72 @@ OXC_DI void clip_and_draw(const TriParams& p, float4 c0, float4 c1, float4 c2, u
   }
 }
 
-// One thread per queued triangle (k_raster_visbuffer queued its data word): the three clip-space corners are recomputed with
-// the canonical operation order (bit-identical to the ones the raster saw), then clipped and drawn.  Runs after every
-// k_raster_visbuffer and before k_raster_big; the queue is empty unless geometry crosses the near / guard-band planes.
-__global__ void __launch_bounds__(128) k_raster_clip_queue(const __grid_constant__ TriParams p) {
-  const uint32_t n = min(*p.clip_counter, p.clip_capacity);
-  const uint32_t id_base = p.id_base ? __ldg(p.id_base) : 0u;
-  for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
-    const uint32_t data = p.clip_queue[e];
-    const uint32_t gid = data >> p.prim_bits, t = data & ((1u << p.prim_bits) - 1u);
-    const uint2 mi = __ldg(reinterpret_cast<const uint2*>(p.meshlet_instances) + (gid - id_base));
-    const InstGeom* g = p.geom + mi.x;
-    const InstCull* ic = p.inst + mi.x;
-    const uint4 m = __ldg(reinterpret_cast<const uint4*>(g->meshlets + mi.y));
-    const float4 r0 = __ldg(&ic->mvp_row[0]), r1 = __ldg(&ic->mvp_row[1]), r2 = __ldg(&ic->mvp_row[2]), r3 = __ldg(&ic->mvp_row[3]);
-    float4 c[3];
+// The triangle behind a vis data word as k_raster_visbuffer sees it: the three clip-space corners recomputed with the canonical
+// operation order (bit-identical to the ones the raster saw), the same near-plane, backface and malformed-index tests and the
+// same set-up.  Returns the set-up's TRI_* result, or -1 for a triangle the raster culls or never reaches.
+OXC_DI int rebuild_triangle(const TriParams& p, uint32_t data, uint32_t id_base, float4 (&c)[3], TriSetup& s) {
+  const uint32_t gid = data >> p.prim_bits, t = data & ((1u << p.prim_bits) - 1u);
+  const uint2 mi = __ldg(reinterpret_cast<const uint2*>(p.meshlet_instances) + (gid - id_base));
+  const InstGeom* g = p.geom + mi.x;
+  const InstCull* ic = p.inst + mi.x;
+  const uint4 m = __ldg(reinterpret_cast<const uint4*>(g->meshlets + mi.y));
+  if (t >= min(m.w, (uint32_t)OXC_MESHLET_MAX_PRIMITIVES)) return -1;
+  const float4 r0 = __ldg(&ic->mvp_row[0]), r1 = __ldg(&ic->mvp_row[1]), r2 = __ldg(&ic->mvp_row[2]), r3 = __ldg(&ic->mvp_row[3]);
 #pragma unroll
-    for (int k = 0; k < 3; k++) {
-      const uint32_t li = micro_index(g->local_triangle_indices, m.y + t * 3u + k);
-      const uint32_t vi = __ldg(&g->indirect_vertex_indices[m.x + li]);
-      const uint2 q = __ldg(&g->vertex_positions[vi]);
-      const float x = dequantize_half_hw(q.x & 0xFFFFu), y = dequantize_half_hw(q.x >> 16), z = dequantize_half_hw(q.y & 0xFFFFu);
-      c[k] = make_float4(row_dot_p1(r0, x, y, z), row_dot_p1(r1, x, y, z), row_dot_p1(r2, x, y, z), row_dot_p1(r3, x, y, z));
+  for (int k = 0; k < 3; k++) {
+    const uint32_t li = micro_index(g->local_triangle_indices, m.y + t * 3u + k);
+    if (li >= min(m.z, (uint32_t)OXC_MESHLET_MAX_VERTICES)) return -1;
+    const uint32_t vi = __ldg(&g->indirect_vertex_indices[m.x + li]);
+    const uint2 q = __ldg(&g->vertex_positions[vi]);
+    const float x = dequantize_half_hw(q.x & 0xFFFFu), y = dequantize_half_hw(q.x >> 16), z = dequantize_half_hw(q.y & 0xFFFFu);
+    c[k] = make_float4(row_dot_p1(r0, x, y, z), row_dot_p1(r1, x, y, z), row_dot_p1(r2, x, y, z), row_dot_p1(r3, x, y, z));
+  }
+  if (!(c[0].z >= 0.0f && c[1].z >= 0.0f && c[2].z >= 0.0f) || triangle_backface(c[0], c[1], c[2])) return -1;
+  return tri_setup(to_screen(c[0], p.f_width, p.f_height), to_screen(c[1], p.f_width, p.f_height), to_screen(c[2], p.f_width, p.f_height),
+                   p.width, p.height, s);
+}
+
+// One deferred triangle, drawn by the whole warp (every lane passes the same data word): clipped by lane 0 if a vertex is
+// invalid; otherwise a box over RASTER_BIG_PIXELS goes to the chunk queue of k_raster_big, and a smaller box (64-bit edge
+// functions), or one the full chunk queue cannot take, is covered in 8x4-pixel tiles right here.
+OXC_DI void draw_deferred(const TriParams& p, uint32_t data, uint32_t id_base, uint32_t lane) {
+  float4 c[3];
+  TriSetup s;
+  const int why = rebuild_triangle(p, data, id_base, c, s);
+  if (why == TRI_INVALID_VERTEX) {
+    if (lane == 0) clip_and_draw(p, c[0], c[1], c[2], data, p.f_width, p.f_height);
+    return;
+  }
+  if (why != TRI_DRAW) return;
+  if ((s.px1 - s.px0 + 1) * (s.py1 - s.py0 + 1) > RASTER_BIG_PIXELS && big_push_warp(p, s, data, lane)) return;
+  raster_tiles(p, s, data, lane);
+}
+
+// One warp per entry of the deferred queue k_raster_visbuffer filled.  Runs after every k_raster_visbuffer and before
+// k_raster_big.  When the queue overflowed, the warps then walk the pass's survivors again and draw (or clip) every triangle a
+// lane would not draw itself; the queued ones are drawn twice, which the packed max
+// leaves unchanged.
+__global__ void __launch_bounds__(256) k_raster_deferred(const __grid_constant__ TriParams p) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t warp0 = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), warps = gridDim.x * (blockDim.x >> 5);
+  const uint32_t pushed = *p.deferred_counter;
+  const uint32_t n = min(pushed, p.deferred_capacity);
+  const uint32_t id_base = p.id_base ? __ldg(p.id_base) : 0u;
+  for (uint32_t e = warp0; e < n; e += warps) draw_deferred(p, p.deferred_queue[e], id_base, lane);
+  if (pushed <= p.deferred_capacity) return;
+  const uint32_t first = p.late ? p.vis->early_visible_meshlet_instances : 0u;
+  const uint32_t count = p.tri_cmd->x;
+  for (uint32_t g = warp0; g < count; g += warps) {
+    const uint32_t gid = __ldg(&p.visible_indices[first + g]);
+    for (uint32_t t = lane; t < OXC_MESHLET_MAX_PRIMITIVES; t += 32) {
+      const uint32_t data = (gid << p.prim_bits) | t;
+      float4 c[3];
+      TriSetup s;
+      const int why = rebuild_triangle(p, data, id_base, c, s);
+      const bool deferred = why == TRI_INVALID_VERTEX || (why == TRI_DRAW && !lane_draws(s));
+      for (uint32_t m = __ballot_sync(0xffffffffu, deferred); m; m &= m - 1)
+        draw_deferred(p, __shfl_sync(0xffffffffu, data, __ffs(m) - 1), id_base, lane);
     }
-    clip_and_draw(p, c[0], c[1], c[2], data, p.f_width, p.f_height);
   }
 }
 

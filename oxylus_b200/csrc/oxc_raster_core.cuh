@@ -145,36 +145,43 @@ OXC_DI void raster_pixel(const TriSetup& s, int px, int py, uint32_t data, unsig
 
 OXC_DI int orient2d_32(int ax, int ay, int bx, int by, int cx, int cy) { return (bx - ax) * (cy - ay) - (by - ay) * (cx - ax); }
 
-OXC_DI void shade_pixel_32(const TriSetup& s, int e0, int e1, int e2, int px, int py, uint32_t data, unsigned long long* vis,
-                           uint32_t W) {
-  if ((e0 - (s.bias & 1)) < 0 || (e1 - ((s.bias >> 1) & 1)) < 0 || (e2 - ((s.bias >> 2) & 1)) < 0) return;
-  const float zz = fa(fa(s.za, fm((float)e1, s.dzb)), fm((float)e2, s.dzc)); // (float)int32 == (float)int64 of the same value
-  if (!(zz >= 0.0f && zz <= 1.0f)) return;
-  uint32_t zb = __float_as_uint(zz);
-  zb = zb == 0x80000000u ? 0u : zb;
-  const unsigned long long v = ((unsigned long long)zb << 32) | data;
-  unsigned long long* ptr = vis + (size_t)py * W + px;
-  atomicMax(ptr, v); // fire-and-forget RED (see shade_pixel)
+// raster_small for a narrow triangle (32-bit edge functions), the per-lane loop of k_raster_visbuffer.  Each edge's bias is
+// folded into its start value, so a sample is covered when no stepped value is negative (one test of the three values' OR);
+// e1 and e2 get their bias back for the depth, which converts the same values as shade_pixel ((float)int32 == (float)int64 of
+// the same value).  The image pointer is stepped with the pixel instead of recomputed from (px, py).
+OXC_DI void raster_narrow(const TriSetup& s, uint32_t data, unsigned long long* vis, uint32_t W) {
+  const int sx0 = s.px0 * 256 + 128, sy0 = s.py0 * 256 + 128;
+  const int b1 = (s.bias >> 1) & 1, b2 = (s.bias >> 2) & 1;
+  int r0 = orient2d_32(s.bx, s.by, s.cx, s.cy, sx0, sy0) - (s.bias & 1), r1 = orient2d_32(s.cx, s.cy, s.ax, s.ay, sx0, sy0) - b1,
+      r2 = orient2d_32(s.ax, s.ay, s.bx, s.by, sx0, sy0) - b2;
+  const int dx0 = -(s.cy - s.by) * 256, dy0 = (s.cx - s.bx) * 256, dx1 = -(s.ay - s.cy) * 256, dy1 = (s.ax - s.cx) * 256,
+            dx2 = -(s.by - s.ay) * 256, dy2 = (s.bx - s.ax) * 256;
+  const int nx = s.px1 - s.px0;
+  unsigned long long* row = vis + (size_t)s.py0 * W + s.px0;
+  for (int py = s.py0; py <= s.py1; py++, row += W) {
+    int e0 = r0, e1 = r1, e2 = r2;
+    for (int i = 0; i <= nx; i++) {
+      if ((e0 | e1 | e2) >= 0) {
+        const float zz = fa(fa(s.za, fm((float)(e1 + b1), s.dzb)), fm((float)(e2 + b2), s.dzc));
+        if (zz >= 0.0f && zz <= 1.0f) {
+          uint32_t zb = __float_as_uint(zz);
+          zb = zb == 0x80000000u ? 0u : zb;
+          atomicMax(row + i, ((unsigned long long)zb << 32) | data); // fire-and-forget RED (see shade_pixel)
+        }
+      }
+      e0 += dx0; e1 += dx1; e2 += dx2;
+    }
+    r0 += dy0; r1 += dy1; r2 += dy2;
+  }
 }
 
 // one lane walks the (small) bounding box with incrementally stepped edge functions (adds only)
 OXC_DI void raster_small(const TriSetup& s, uint32_t data, unsigned long long* vis, uint32_t W) {
-  const int sx0 = s.px0 * 256 + 128, sy0 = s.py0 * 256 + 128;
   if (s.narrow) {
-    int r0 = orient2d_32(s.bx, s.by, s.cx, s.cy, sx0, sy0), r1 = orient2d_32(s.cx, s.cy, s.ax, s.ay, sx0, sy0),
-        r2 = orient2d_32(s.ax, s.ay, s.bx, s.by, sx0, sy0);
-    const int dx0 = -(s.cy - s.by) * 256, dy0 = (s.cx - s.bx) * 256, dx1 = -(s.ay - s.cy) * 256, dy1 = (s.ax - s.cx) * 256,
-              dx2 = -(s.by - s.ay) * 256, dy2 = (s.bx - s.ax) * 256;
-    for (int py = s.py0; py <= s.py1; py++) {
-      int e0 = r0, e1 = r1, e2 = r2;
-      for (int px = s.px0; px <= s.px1; px++) {
-        shade_pixel_32(s, e0, e1, e2, px, py, data, vis, W);
-        e0 += dx0; e1 += dx1; e2 += dx2;
-      }
-      r0 += dy0; r1 += dy1; r2 += dy2;
-    }
+    raster_narrow(s, data, vis, W);
     return;
   }
+  const int sx0 = s.px0 * 256 + 128, sy0 = s.py0 * 256 + 128;
   long long r0 = orient2d(s.bx, s.by, s.cx, s.cy, sx0, sy0);
   long long r1 = orient2d(s.cx, s.cy, s.ax, s.ay, sx0, sy0);
   long long r2 = orient2d(s.ax, s.ay, s.bx, s.by, sx0, sy0);

@@ -134,9 +134,9 @@ struct OxcContext {
   uint4* d_big_queue = nullptr;      // deferred large triangles of the raster (kernels_tri.cuh)
   uint32_t* d_big_counters = nullptr;
   uint32_t big_capacity = 0;
-  uint32_t* d_clip_queue = nullptr;  // triangles the plain raster rules drop (clipped by k_raster_clip_queue)
-  uint32_t* d_clip_counter = nullptr;
-  uint32_t clip_capacity = 1u << 20;
+  uint32_t* d_deferred_queue = nullptr;  // triangles a raster lane does not draw itself (k_raster_deferred)
+  uint32_t* d_deferred_counter = nullptr;
+  uint32_t deferred_capacity = 1u << 20;
   // hiz
   float* d_hiz = nullptr;
   HizDesc hiz{};
@@ -338,7 +338,7 @@ int oxc_create(int device, const OxcCreateInfo* info, OxcContext** out_ctx) {
   TRY(dalloc(&c->d_cull_triangles_cmd, 1));
   TRY(dalloc(&c->d_draw_cmd, 1));
   TRY(dalloc(&c->d_tri_counter, 1));
-  TRY(dalloc(&c->d_raster_work, 4)); // work counter | chunk-queue counters (2) | clip-queue counter: one 16-byte memset per raster call
+  TRY(dalloc(&c->d_raster_work, 4)); // work counter | chunk-queue counters (2) | deferred-queue counter: one 16-byte memset per raster call
   c->big_capacity = 1u << 18; // 262144 chunks x 64 B = 16 MB; overflow falls back to inline rasterisation
   if (const char* e = getenv("OXC_BIG_CAPACITY")) { // test hook: force the overflow paths
     const long v = atol(e);
@@ -351,16 +351,16 @@ int oxc_create(int device, const OxcCreateInfo* info, OxcContext** out_ctx) {
 #endif
   CK(cudaMemset(c->d_big_queue + (size_t)c->big_capacity * 4, 0, 1024));
   c->d_big_counters = c->d_raster_work + 1;
-  if (const char* e = getenv("OXC_CLIP_CAPACITY")) { // test hook: force the overflow path
+  if (const char* e = getenv("OXC_CLIP_CAPACITY")) { // test hook: force the deferred queue's overflow paths
     const long v = atol(e);
-    if (v >= 1 && v <= (1l << 24)) c->clip_capacity = (uint32_t)v;
+    if (v >= 1 && v <= (1l << 24)) c->deferred_capacity = (uint32_t)v;
   }
-  TRY(dalloc(&c->d_clip_queue, (size_t)c->clip_capacity));
+  TRY(dalloc(&c->d_deferred_queue, (size_t)c->deferred_capacity));
   if (const char* e = getenv("OXC_VSM_DRAW_CAPACITY")) { // test hook: force the VSM draw's inline path
     const long v = atol(e);
     if (v >= 1 && v <= (1l << 24)) c->vsm_queue_capacity = (uint32_t)v;
   }
-  c->d_clip_counter = c->d_raster_work + 3;
+  c->d_deferred_counter = c->d_raster_work + 3;
   TRY(dalloc(&c->d_id_base_auto, 1));
   TRY(dalloc(&c->d_status, 1));
   c->prim_bits = info->wide_ids ? OXC_VIS_WIDE_PRIMITIVE_BITS : OXC_VIS_PRIMITIVE_BITS;
@@ -428,7 +428,7 @@ void oxc_destroy(OxcContext* c) {
   cudaFree(c->d_lod_aabb); cudaFree(c->d_inst); cudaFree(c->d_geom); cudaFree(c->d_counts); cudaFree(c->d_block_sums);
   cudaFree(c->d_meshlet_instances); cudaFree(c->d_slabs); cudaFree(c->d_visible); cudaFree(c->d_mask); cudaFree(c->d_vis);
   cudaFree(c->d_cull_meshlets_cmd); cudaFree(c->d_cull_triangles_cmd); cudaFree(c->d_draw_cmd);
-  cudaFree(c->d_reordered); cudaFree(c->d_tri_counter); cudaFree(c->d_raster_work); cudaFree(c->d_big_queue); cudaFree(c->d_clip_queue); cudaFree(c->d_id_base_auto); cudaFree(c->d_status); cudaFree(c->d_hiz);
+  cudaFree(c->d_reordered); cudaFree(c->d_tri_counter); cudaFree(c->d_raster_work); cudaFree(c->d_big_queue); cudaFree(c->d_deferred_queue); cudaFree(c->d_id_base_auto); cudaFree(c->d_status); cudaFree(c->d_hiz);
   cudaFree(c->d_view_planes); cudaFree(c->d_view_bits); cudaFree(c->d_view_counts); cudaFree(c->d_inst_views);
   cudaFree(c->d_alpha_materials); cudaFree(c->d_alpha_lists); cudaFree(c->d_alpha_cmd); cudaFree(c->d_gbuf_table);
   cudaFree(c->d_vsm_bitmap); cudaFree(c->d_vsm_first_px); cudaFree(c->d_vsm_queue); cudaFree(c->d_vsm_counters);
@@ -842,9 +842,9 @@ int oxc_raster_visbuffer(OxcContext* c, const OxcCullCamera* cam, uint32_t flags
   raster_target(c, vis, w, h, &p);
   p.small_primitive_cull = small_primitive_cull ? 1u : 0u;
   p.work_counter = c->d_raster_work;
-  CK(cudaMemsetAsync(c->d_raster_work, 0, 16, s)); // work counter, chunk-queue counters, clip-queue counter
+  CK(cudaMemsetAsync(c->d_raster_work, 0, 16, s)); // work counter, chunk-queue counters, deferred-queue counter
   const uint32_t grid = persistent_grid(c, TRI_WARPS, c->occ_raster);
-  p.clip_queue = c->d_clip_queue; p.clip_counter = c->d_clip_counter; p.clip_capacity = c->clip_capacity;
+  p.deferred_queue = c->d_deferred_queue; p.deferred_counter = c->d_deferred_counter; p.deferred_capacity = c->deferred_capacity;
   TriParams pm = p; // what the plain raster kernel walks: the pass's survivors, or their opaque part
   AlphaParams ap{};
   if (c->alpha_active) {
@@ -854,7 +854,9 @@ int oxc_raster_visbuffer(OxcContext* c, const OxcCullCamera* cam, uint32_t flags
   if (p.late) k_raster_visbuffer<true><<<grid, TRI_THREADS, 0, s>>>(pm);
   else k_raster_visbuffer<false><<<grid, TRI_THREADS, 0, s>>>(pm);
   LAUNCHED();
-  k_raster_clip_queue<<<c->sm_count, 128, 0, s>>>(p); // the triangles the plain rules drop (usually none: exits at once)
+  // the triangles a raster lane does not draw itself (clipped, 64-bit edge functions, large boxes), one warp each; with the
+  // survivors the raster walked, for the walk after an overflow
+  k_raster_deferred<<<c->sm_count * 8, 256, 0, s>>>(pm);
   LAUNCHED();
   if (c->alpha_active) {
     k_raster_alpha<false><<<c->sm_count * 8, ALPHA_THREADS, 0, s>>>(p, ap); // the alpha-tested meshlets, one warp each
@@ -1611,7 +1613,7 @@ int oxc_check_status(OxcContext* c, void* stream, uint32_t* flags_out) {
     return fail(OXC_E_CAPACITY, "device status 0x%x:%s%s%s%s%s", f, (f & OXC_STATUS_MESHLET_OVERFLOW) ? " cull_meshes exceeded max_meshlet_instances (clamped)" : "",
                 (f & OXC_STATUS_SURVIVOR_OVERFLOW) ? " a survivor list exceeded the gather capacity (truncated)" : "",
                 (f & OXC_STATUS_ID_OVERFLOW) ? " a meshlet-instance id overflowed the vis-buffer id bits" : "",
-                (f & OXC_STATUS_CLIP_OVERFLOW) ? " the clip queue overflowed (run oxc_raster_visbuffer_clip_pass)" : "",
+                (f & OXC_STATUS_CLIP_OVERFLOW) ? " the raster's deferred queue overflowed (every triangle was drawn, the overflowing ones by a slow second walk over the pass)" : "",
                 (f & OXC_STATUS_PEER_TIMEOUT) ? " a peer GPU did not signal its Hi-Z exchange in time" : "");
   if (f & OXC_STATUS_BAD_MATERIAL)
     return fail(OXC_E_INVALID, "device status 0x%x: a MeshInstance::material_index lies outside the table of oxc_set_materials (rasterised as opaque)", f);

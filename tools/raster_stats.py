@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Instrumentation run (variant library built with -DOXC_RASTER_STATS): per round of 32 triangles, how long is the longest
 per-lane pixel loop, how many rounds run the triangle set-up, how many meshlets draw anything, and how many could be settled
-once per meshlet (footprint box without a sample centre, no invalid vertex)?  Usage:  OXC_LIB_PATH=$PWD/oxylus_b200/liboxcull_stats.so python tools/raster_stats.py"""
+once per meshlet (footprint box without a sample centre, no invalid vertex), and how many triangles go to the deferred queue
+(not narrow, box over RASTER_BIG_PIXELS, invalid vertex)?  Usage:  OXC_LIB_PATH=$PWD/oxylus_b200/liboxcull_stats.so python tools/raster_stats.py"""
 import os
 import sys
 
@@ -33,6 +34,11 @@ for name, o in (("early", 0), ("late", 64)):
           f"deferred big tris/frame {st[o + 44] / frames:.0f}")
     print(f"   meshlets with a drawing triangle/frame {st[o + 46] / frames:.0f}  set-up rounds/frame {st[o + 47] / frames:.0f}")
     print(f"   meshlets whose footprint holds no sample centre and that have no invalid vertex/frame {st[o + 48] / frames:.0f}")
+    setup = max(1, int(st[o + 52]))
+    print(f"   set-up triangles/frame {st[o + 52] / frames:.0f}; per frame, and per million set-up triangles: not narrow "
+          f"{st[o + 49] / frames:.0f} ({st[o + 49] * 1e6 / setup:.1f}), box over RASTER_BIG_PIXELS {st[o + 44] / frames:.0f} "
+          f"({st[o + 44] * 1e6 / setup:.1f}), invalid vertex (clipped) {st[o + 50] / frames:.0f} ({st[o + 50] * 1e6 / setup:.1f}); "
+          f"deferred-queue entries {st[o + 51] / frames:.0f} ({st[o + 51] * 1e6 / setup:.1f})")
     print("   histogram of max per-lane bbox area per round (0..32, 33+):")
     print("   " + " ".join(f"{int(x / frames)}" for x in h))
     cost_serial = float((h * np.arange(34)).sum())
