@@ -1083,6 +1083,56 @@ int oxc_atmosphere_sky_luts(OxcContext* ctx, const OxcAtmosphere* atmosphere, co
                             float sun_intensity, const uint16_t* transmittance_dev, uint16_t* sky_view_dev, uint16_t* aerial_perspective_dev,
                             void* stream);
 
+/* The sky IBL cube (Passes/PBR.cpp:52-94, passes/sky_ibl.slang, RendererInstance.cpp:187-201 and :1022): the sky light of each of 6
+ * faces x 32 x 32 texels, 64 cosine-weighted taps of the sky-view LUT per texel around the texel's direction (sky.slang:296-322
+ * get_atmosphere_illuminance_along_ray), plus a sun term, accumulated frame to frame.  The reference runs it every frame under
+ * HasAtmosphere && HasDirectionalLight, after the sky view, with sun_ambient_strength 0.15 and frame_index = the engine's frame counter.
+ * cube_dev: 6 x 32 x 32 binary16 RGBA texels (48 KiB), face-major, then y, then x fastest; faces 0..5 look along +X, -X, +Y, -Y, +Z, -Z.
+ * It is read and written in place: a texel with a > 0 and finite rgb is history, so a zeroed cube (the reference clears it to black)
+ * means no history.  transmittance_dev and sky_view_dev are the LUTs oxc_atmosphere_transmittance and oxc_atmosphere_sky_luts wrote,
+ * at the record's transmittance_lut_size.xy and sky_view_lut_size.xy; of the camera only the position is read.  No scratch, so the
+ * call is graph-capturable; a captured graph replays the frame_index it was captured with.
+ * Refused with OXC_E_INVALID, before anything is launched: a NULL argument or plane, a plane not 8-byte aligned, a transmittance size
+ * 0 or above 4096, a sky-view size below 2 or above 4096, a cube that shares a byte with either LUT.  NaN, Inf and denormal values in
+ * the record, camera, sun, intensities and cube are accepted and follow the rules below.
+ * SPECIFICATION (oracle/oxc_oracle_sky_ibl.c, bit for bit): the atmosphere rules above (binary32, no contraction, written order, dot,
+ * normalize, length, lerp, max / min with NaN, clamp, safe_sqrt, saturate(x) = min(max(x, 0), 1), its constants and its items 1, 5 and 6),
+ * cross(a, b) = (a.y*b.z - a.z*b.y, a.z*b.x - a.x*b.z, a.x*b.y - a.y*b.x), frac(x) = x - floor(x), sanitize(x) = isfinite(x) ? x : 0,
+ * f32(u32) rounds to nearest even; constants 0.999 0x3F7FBE77, IGN's 0.06711056 0x3D897143, 0.00583715 0x3BBF4590, 52.9829189
+ * 0x4253EE82, 0.61803398875 0x3F1E377A, 2.3283064365386963e-10 0x2F800000, alpha 0.02 0x3CA3D70A, 1e-20 0x1E3CE508, 1e-5 0x3727C5AC,
+ * 2.0 * PI = TAU.  For texel (x, y) of face f:
+ *   1. uv = (f32(x, y) + 0.5) / 32, dir = normalize(mul(M_f, (uv * 2 - 1, -1))), M_f the shader's mat3 literals read by rows and
+ *      mul(M, v) row by row; up = |dir.y| < 0.999 ? (0, 1, 0) : (1, 0, 0), tangent = normalize(cross(up, dir)), bitangent =
+ *      cross(dir, tangent).
+ *   2. history = the texel as stored, binary16 read exactly; has_history = a > 0 && all(isfinite(rgb)) (NaN, +-inf, a <= 0 or a NaN alpha
+ *      mean none).  base = IGN(f32(x, y) + f32(f) * (37, 17)), IGN(p) = frac(52.9829189 * frac(p.x * 0.06711056 + p.y * 0.00583715));
+ *      rotation = has_history ? frac(base + f32(frame_index) * 0.61803398875) : base.
+ *   3. sample i of 64: u1 = (f32(i) + 0.5) / 64, u2 = frac(radical_inverse_vdc(i) + rotation) (exact for i < 64), phi = TAU * u2, cos and
+ *      sin of phi by canonical_sincos, local = (sqrt(u1) cos, sqrt(u1) sin, sqrt(max(0, 1 - u1))), input = normalize((x * tangent +
+ *      y * bitangent) + z * dir).  Its value is sanitize(get_atmosphere_illuminance_along_ray(sun, eye, input)) with eye = (0, eye_y, 0):
+ *      height = eye_h, up = eye / height and the normalized sun once per call; side = length(cross(up, input)) > 1e-5 ? normalize(that)
+ *      : (1, 0, 0); forward = normalize(cross(side, up)); light_on_plane = safe_normalize((dot(sun, forward), dot(sun, side)), (1, 0)),
+ *      safe_normalize(v, f) = len2 > 1e-20 ? v * rsqrt(len2) : f with rsqrt(x) = fl(1 / fl(sqrt(x))) (two roundings, where the shader's
+ *      rsqrt is approximate); intersect_planet = ray_sphere_intersect_nearest(eye, input, planet_radius).hasValue; then
+ *      sky_view_params_to_lut_uv with the per-call beta and PI - beta, acos(dot(input, up)) by canonical_acos (binary64, the same bits on
+ *      the device and the host) and atan2(-l.y, -l.x) by canonical_atan2 (binary64, one rounding, within 1 ulp, C99 special cases), and
+ *      from_unit_to_sub_uvs; the tap (atmosphere item 5, all four channels) of the sky-view LUT; sanitize(rgb * a).  For a finite
+ *      height up is exactly (0, 1, 0) (sqrt(fl(y * y)) = |y|), so the view-zenith cosine is input.y and rounding cannot push it past 1;
+ *      an acos argument past +-1 or NaN (a NaN up, from an infinite or NaN height) gives NaN, which reaches safe_sqrt: max(0, NaN) = 0,
+ *      so v = 0.5, the horizon row, in both branches.
+ *   4. estimate = (((0 + s_0) + s_1) + ... + s_63) / 64 per channel, in index order.  sun term = (((0.15 * T) * sun_intensity) *
+ *      saturate(dot(dir, sun))) / PI with the sun as given (not normalized) and T the transmittance tap at
+ *      transmittance_params_to_lut_uv(atmos_radius, planet_radius, (eye_y, dot(sun, (0, 1, 0)))); sun_ambient_strength for 0.15.
+ *   5. result = min(max(sanitize(estimate + sun term), 0), 65504); stored = has_history ? lerp(history.rgb, result, 0.02) : result, as
+ *      (stored, 1) in binary16 (atmosphere item 6).  A finite history and a result in [0, 65504] keep the stored rgb finite: it is never
+ *      NaN; a negative finite history decays toward the result. */
+#define OXC_SKY_IBL_CUBE_RES 32u
+#define OXC_SKY_IBL_SAMPLES 64u
+#define OXC_SKY_IBL_CUBE_BYTES (6u * OXC_SKY_IBL_CUBE_RES * OXC_SKY_IBL_CUBE_RES * 8u)
+int oxc_atmosphere_sky_ibl(OxcContext* ctx, const OxcAtmosphere* atmosphere, const OxcPbrCamera* camera, const float sun_direction[3],
+                           float sun_intensity, float sun_ambient_strength, uint32_t frame_index, const uint16_t* transmittance_dev,
+                           const uint16_t* sky_view_dev, uint16_t* cube_dev, void* stream);
+
 int oxc_get_outputs(OxcContext* ctx, OxcOutputs* out);
 /* Instrumentation hook: 128 u64 counters that builds with -DOXC_RASTER_STATS fill (tools/raster_stats.py); zero otherwise. */
 void* oxc_debug_stats_ptr(OxcContext* ctx);
@@ -1246,6 +1296,15 @@ int oxr_apply_pbr_with_contact_shadows(OxrRenderer* r, const OxcCullCamera* came
  * with the camera path left usable, when the planes cannot be allocated. */
 int oxr_atmosphere_luts(OxrRenderer* r, const OxcAtmosphere* atmosphere, const OxcPbrCamera* camera, const float sun_direction[3],
                         float sun_intensity, uint16_t* transmittance_host, uint16_t* sky_view_host, uint16_t* aerial_perspective_host);
+/* The sky IBL cube as the reference makes it each frame, on the renderer's stream, synchronous: the per-frame LUTs exactly as
+ * oxr_atmosphere_luts makes them (the same planes, the bake at the first call), then oxc_atmosphere_sky_ibl over them into a cube the
+ * renderer owns (allocated and zeroed at the first call, as the reference clears its cube to black) with sun_ambient_strength 0.15 and
+ * frame_index = the number of earlier oxr_atmosphere_sky_ibl calls on this renderer (0 at the first).  That count equals the reference's
+ * frame counter when the call runs once per frame from the engine's first frame.  cube_host (may be NULL) receives the cube, 6 x 32 x 32
+ * binary16 RGBA (48 KiB).  The frame's outputs are left as they were.  OXC_E_CAPACITY, with the camera path left usable, when the
+ * planes cannot be allocated; a failed call does not advance the count. */
+int oxr_atmosphere_sky_ibl(OxrRenderer* r, const OxcAtmosphere* atmosphere, const OxcPbrCamera* camera, const float sun_direction[3],
+                           float sun_intensity, uint16_t* cube_host);
 
 /* ------------------------------------------------------------------------------------------------
  * oxb_* — mesh builder (SURVEY §8f.2): host-side producer of the blob layout above, mirroring build_gltf_mesh

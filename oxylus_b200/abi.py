@@ -493,6 +493,15 @@ ATMOSPHERE_DEFAULTS = dict(rayleigh_scatter=(0.005802, 0.013558, 0.033100), rayl
                            sky_view_lut_size=(312, 192, 1), multiscattering_lut_size=(32, 32, 1), aerial_perspective_lut_size=(32, 32, 32))
 
 
+# the sky IBL cube (oxc_atmosphere_sky_ibl): 6 faces x 32 x 32 binary16 RGBA texels, 64 sky-view samples per texel per call
+SKY_IBL_CUBE_RES = 32
+SKY_IBL_SAMPLES = 64
+SKY_IBL_CUBE_SHAPE = (6, SKY_IBL_CUBE_RES, SKY_IBL_CUBE_RES, 4)
+SKY_IBL_CUBE_BYTES = 6 * SKY_IBL_CUBE_RES * SKY_IBL_CUBE_RES * 8
+# the sun_ambient_strength the reference passes (Passes/PBR.cpp:56)
+SKY_IBL_SUN_AMBIENT_STRENGTH = 0.15
+
+
 def atmosphere(**overrides):
     """Atmosphere with the GPU::Atmosphere{} defaults and the reference's LUT sizes; any field may be overridden by name"""
     a = Atmosphere()

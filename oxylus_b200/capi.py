@@ -22,7 +22,7 @@ SYMBOLS = [
     "oxc_decode_visbuffer", "oxc_decode_gbuffer", "oxc_build_hpb", "oxc_mark_visible_pages",
     "oxc_vsm_begin_frame", "oxc_vsm_invalidate_pages", "oxc_vsm_allocate_pages", "oxc_vsm_clear_dirty_pages", "oxc_cull_meshlets_hpb_dirty_dev",
     "oxc_vsm_draw_pages", "oxc_vsm_draw_stats", "oxc_vsm_resolve_shadows", "oxc_generate_ambient_occlusion", "oxc_apply_pbr",
-    "oxc_contact_shadows", "oxc_atmosphere_transmittance", "oxc_atmosphere_sky_luts",
+    "oxc_contact_shadows", "oxc_atmosphere_transmittance", "oxc_atmosphere_sky_luts", "oxc_atmosphere_sky_ibl",
     "oxc_get_outputs", "oxc_check_status", "oxc_mark_hiz_dirty", "oxc_bind_camera_buffer", "oxc_load_camera", "oxc_debug_stats_ptr",
     "oxc_mgpu_get_unique_id", "oxc_mgpu_init", "oxc_mgpu_init_with_comm", "oxc_mgpu_shutdown", "oxc_mgpu_info", "oxc_mgpu_exchange_hiz",
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
@@ -30,7 +30,7 @@ SYMBOLS = [
     "oxr_create", "oxr_destroy", "oxr_context", "oxr_update", "oxr_update_transforms", "oxr_set_external_depth", "oxr_set_materials", "oxr_overdraw", "oxr_render", "oxr_submit", "oxr_wait",
     "oxr_vsm_update_pages", "oxr_vsm_pages", "oxr_vsm_draw_shadows", "oxr_vsm_resolve_shadows", "oxr_decode_gbuffer",
     "oxr_generate_ambient_occlusion", "oxr_apply_pbr", "oxr_contact_shadows", "oxr_apply_pbr_with_contact_shadows",
-    "oxr_atmosphere_luts",
+    "oxr_atmosphere_luts", "oxr_atmosphere_sky_ibl",
 ]
 
 
@@ -159,6 +159,9 @@ def load(build_if_missing=True):
     lib.oxc_atmosphere_transmittance.argtypes = [vp, C.POINTER(abi.Atmosphere), vp, vp]
     lib.oxc_atmosphere_sky_luts.argtypes = [vp, C.POINTER(abi.Atmosphere), C.POINTER(abi.PbrCamera), vp, C.c_float, vp, vp, vp, vp]
     lib.oxr_atmosphere_luts.argtypes = [vp, C.POINTER(abi.Atmosphere), C.POINTER(abi.PbrCamera), vp, C.c_float, vp, vp, vp]
+    lib.oxc_atmosphere_sky_ibl.argtypes = [vp, C.POINTER(abi.Atmosphere), C.POINTER(abi.PbrCamera), vp, C.c_float, C.c_float, u32, vp, vp, vp,
+                                           vp]
+    lib.oxr_atmosphere_sky_ibl.argtypes = [vp, C.POINTER(abi.Atmosphere), C.POINTER(abi.PbrCamera), vp, C.c_float, vp]
     _LIB = lib
     return lib
 
@@ -525,6 +528,16 @@ class Context:
                                                 _ptr(transmittance_dev), _ptr(sky_view_dev), _ptr(aerial_perspective_dev), self.stream),
                "oxc_atmosphere_sky_luts")
 
+    def atmosphere_sky_ibl(self, atmosphere, camera, sun_direction, sun_intensity, sun_ambient_strength, frame_index, transmittance_dev,
+                           sky_view_dev, cube_dev):
+        """oxc_atmosphere_sky_ibl: the next sky IBL cube (6 x 32 x 32 binary16 RGBA, read and written in place at cube_dev; zeroed = no
+        history) over the transmittance and sky-view LUTs.  camera: abi.PbrCamera (only its position is read); sun_direction: 3 floats,
+        as given; the reference passes sun_ambient_strength 0.15 and its frame counter as frame_index"""
+        sun = (C.c_float * 3)(*[float(np.float32(v)) for v in sun_direction])
+        _check(self.lib.oxc_atmosphere_sky_ibl(self.h, C.byref(atmosphere), C.byref(camera), sun, float(np.float32(sun_intensity)),
+                                               float(np.float32(sun_ambient_strength)), int(frame_index) & 0xFFFFFFFF, _ptr(transmittance_dev),
+                                               _ptr(sky_view_dev), _ptr(cube_dev), self.stream), "oxc_atmosphere_sky_ibl")
+
     def contact_shadows(self, contact_camera, settings, depth_dev, w, h, out_dev):
         """oxc_contact_shadows: 1 - the contact shadow (f32 per pixel) of a w x h frame into out_dev.  contact_camera / settings:
         abi.ContactShadowCamera / abi.ContactShadowSettings"""
@@ -805,6 +818,16 @@ class Renderer:
         _check(self.lib.oxr_atmosphere_luts(self.h, C.byref(atmosphere), C.byref(camera), sun, float(np.float32(sun_intensity)), _ptr(t),
                                             _ptr(sv), _ptr(ap)), "oxr_atmosphere_luts")
         return t, sv, ap
+
+    def atmosphere_sky_ibl(self, atmosphere, camera, sun_direction, sun_intensity):
+        """oxr_atmosphere_sky_ibl: the renderer's sky IBL cube after this call, float16 [6, 32, 32, 4].  The per-frame LUTs are made as
+        atmosphere_luts makes them; the cube persists across calls (zeroed at the first) and the call's frame_index is the number of
+        earlier calls on this renderer"""
+        cube = np.zeros(abi.SKY_IBL_CUBE_SHAPE, np.float16)
+        sun = (C.c_float * 3)(*[float(np.float32(v)) for v in sun_direction])
+        _check(self.lib.oxr_atmosphere_sky_ibl(self.h, C.byref(atmosphere), C.byref(camera), sun, float(np.float32(sun_intensity)), _ptr(cube)),
+               "oxr_atmosphere_sky_ibl")
+        return cube
 
     def apply_pbr(self, cam, settings, lights=None, cast_shadows=False, gtao_camera=None, gtao_settings=None, pbr_camera=None,
                   contact_camera=None, contact_settings=None):

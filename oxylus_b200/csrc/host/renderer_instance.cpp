@@ -102,7 +102,7 @@ RendererInstance::RendererInstance(int device, const OxcCreateInfo& info, uint32
 RendererInstance::~RendererInstance() {
   if (stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(stream_));
   cudaFree(d_vis64_); cudaFree(d_vis32_); cudaFree(d_depth_); cudaFree(d_occluder_); cudaFree(d_overdraw_); cudaFree(d_gbuffer_);
-  cudaFree(d_uv_normal_); cudaFree(d_gtao_); cudaFree(d_pbr_); cudaFree(d_lights_); cudaFree(d_contact_); cudaFree(d_atmosphere_);
+  cudaFree(d_uv_normal_); cudaFree(d_gtao_); cudaFree(d_pbr_); cudaFree(d_lights_); cudaFree(d_contact_); cudaFree(d_atmosphere_); cudaFree(d_sky_ibl_cube_);
   if (h_pinned_) cudaFreeHost(h_pinned_);
   if (copy_stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(copy_stream_));
   for (auto& sl : slots_) {
@@ -513,11 +513,10 @@ auto RendererInstance::contact_shadows(const OxcContactShadowCamera& contact_cam
   return OXC_OK;
 }
 
-// the atmosphere's LUTs on stream_, synchronous: the bake once with the default record (RendererInstance.cpp:203-226), then the two
-// per-frame LUTs with the caller's record at the renderer's extents (:1456-1459, PBR.cpp:11-50 and :96-140)
-auto RendererInstance::atmosphere_luts(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3],
-                                       float sun_intensity, uint16_t* transmittance_host, uint16_t* sky_view_host,
-                                       uint16_t* aerial_perspective_host) -> int {
+// the atmosphere's LUTs on stream_, without a copy: the bake once with the default record (RendererInstance.cpp:203-226), then the two
+// per-frame LUTs with the caller's record at the renderer's extents (:1456-1459, PBR.cpp:11-50 and :96-140); *sized receives that record
+int RendererInstance::atmosphere_luts_device(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3],
+                                             float sun_intensity, OxcAtmosphere* sized_out) {
   if (!ctx_ || !error_.empty()) return OXC_E_STATE;
   if (!sun_direction) return OXC_E_INVALID;
   const size_t t_texels = (size_t)kTransmittanceLut[0] * kTransmittanceLut[1], sv_texels = (size_t)kSkyViewLut[0] * kSkyViewLut[1];
@@ -548,10 +547,55 @@ auto RendererInstance::atmosphere_luts(const OxcAtmosphere& atmosphere, const Ox
     transmittance_baked_ = true;
   }
   if ((rc = oxc_atmosphere_sky_luts(ctx_, &sized, &camera, sun_direction, sun_intensity, d_t, d_sv, d_ap, stream_)) != OXC_OK) return fail(rc);
+  if (sized_out) *sized_out = sized;
+  return OXC_OK;
+}
+
+// atmosphere_luts_device, then the copies to the host, synchronous
+auto RendererInstance::atmosphere_luts(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3],
+                                       float sun_intensity, uint16_t* transmittance_host, uint16_t* sky_view_host,
+                                       uint16_t* aerial_perspective_host) -> int {
+  int rc;
+  if ((rc = atmosphere_luts_device(atmosphere, camera, sun_direction, sun_intensity, nullptr)) != OXC_OK) return rc;
+  const size_t t_texels = (size_t)kTransmittanceLut[0] * kTransmittanceLut[1], sv_texels = (size_t)kSkyViewLut[0] * kSkyViewLut[1];
+  const size_t ap_texels = (size_t)kAerialLut[0] * kAerialLut[1] * kAerialLut[2];
+  uint16_t* d_t = d_atmosphere_;
+  uint16_t* d_sv = d_t + t_texels * 4;
+  uint16_t* d_ap = d_sv + sv_texels * 4;
   cudaStream_t s = static_cast<cudaStream_t>(stream_);
   if ((transmittance_host && cudaMemcpyAsync(transmittance_host, d_t, t_texels * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
       (sky_view_host && cudaMemcpyAsync(sky_view_host, d_sv, sv_texels * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
       (aerial_perspective_host && cudaMemcpyAsync(aerial_perspective_host, d_ap, ap_texels * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
+      cudaStreamSynchronize(s) != cudaSuccess)
+    return fail(OXC_E_CUDA);
+  return OXC_OK;
+}
+
+// the per-frame LUTs as atmosphere_luts makes them, then the sky IBL cube (PBR.cpp:52-94) into the renderer's cube with
+// sun_ambient_strength 0.15 and frame_index = the count of earlier calls, synchronous
+auto RendererInstance::atmosphere_sky_ibl(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3],
+                                          float sun_intensity, uint16_t* cube_host) -> int {
+  OxcAtmosphere sized;
+  int rc;
+  if ((rc = atmosphere_luts_device(atmosphere, camera, sun_direction, sun_intensity, &sized)) != OXC_OK) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  if (!d_sky_ibl_cube_) {
+    if (cudaMalloc(reinterpret_cast<void**>(&d_sky_ibl_cube_), OXC_SKY_IBL_CUBE_BYTES) != cudaSuccess) {
+      cudaGetLastError();
+      d_sky_ibl_cube_ = nullptr;
+      return OXC_E_CAPACITY; // an optional part: the camera path stays usable
+    }
+    // cleared to black, as RendererInstance.cpp:197-201 clears the reference's: no texel has history
+    if (cudaMemsetAsync(d_sky_ibl_cube_, 0, OXC_SKY_IBL_CUBE_BYTES, s) != cudaSuccess) return fail(OXC_E_CUDA);
+  }
+  const size_t t_texels = (size_t)kTransmittanceLut[0] * kTransmittanceLut[1];
+  const uint16_t* d_t = d_atmosphere_;
+  const uint16_t* d_sv = d_t + t_texels * 4;
+  if ((rc = oxc_atmosphere_sky_ibl(ctx_, &sized, &camera, sun_direction, sun_intensity, 0.15f, sky_ibl_calls_, d_t, d_sv, d_sky_ibl_cube_,
+                                   stream_)) != OXC_OK)
+    return fail(rc);
+  sky_ibl_calls_++;
+  if ((cube_host && cudaMemcpyAsync(cube_host, d_sky_ibl_cube_, OXC_SKY_IBL_CUBE_BYTES, cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
       cudaStreamSynchronize(s) != cudaSuccess)
     return fail(OXC_E_CUDA);
   return OXC_OK;
@@ -1085,6 +1129,12 @@ int oxr_atmosphere_luts(OxrRenderer* r, const OxcAtmosphere* atmosphere, const O
                         float sun_intensity, uint16_t* transmittance_host, uint16_t* sky_view_host, uint16_t* aerial_perspective_host) {
   if (!r || !atmosphere || !camera || !sun_direction) return OXC_E_INVALID;
   return r->impl.atmosphere_luts(*atmosphere, *camera, sun_direction, sun_intensity, transmittance_host, sky_view_host, aerial_perspective_host);
+}
+
+int oxr_atmosphere_sky_ibl(OxrRenderer* r, const OxcAtmosphere* atmosphere, const OxcPbrCamera* camera, const float sun_direction[3],
+                           float sun_intensity, uint16_t* cube_host) {
+  if (!r || !atmosphere || !camera || !sun_direction) return OXC_E_INVALID;
+  return r->impl.atmosphere_sky_ibl(*atmosphere, *camera, sun_direction, sun_intensity, cube_host);
 }
 
 int oxr_contact_shadows(OxrRenderer* r, const OxcContactShadowCamera* contact_camera, const OxcContactShadowSettings* settings,

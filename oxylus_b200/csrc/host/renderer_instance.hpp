@@ -97,6 +97,10 @@ public:
   // the caller's record at the renderer's extents); each non-null host pointer receives its binary16 RGBA plane
   auto atmosphere_luts(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3], float sun_intensity,
                        uint16_t* transmittance_host, uint16_t* sky_view_host, uint16_t* aerial_perspective_host) -> int;
+  // the per-frame LUTs as atmosphere_luts makes them, then the sky IBL cube (PBR.cpp:52-94) into the renderer's persistent cube with
+  // sun_ambient_strength 0.15 and frame_index = the number of earlier calls; the cube (binary16 RGBA, 48 KiB) to the host when non-null
+  auto atmosphere_sky_ibl(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3], float sun_intensity,
+                          uint16_t* cube_host) -> int;
 
   // RendererInstance::render geometry section: run_geometry_pass(false) -> generate_hiz -> run_geometry_pass(true)
   auto render(const OxcCullCamera& camera, const float* occluder_depth_host, uint32_t* vis32_host, float* depth_host,
@@ -189,6 +193,11 @@ private:
                             kAerialLut[3] = {32, 32, 32};
   uint16_t* d_atmosphere_ = nullptr; // transmittance, then sky view, then aerial perspective
   bool transmittance_baked_ = false;
+  // the bake when missing and the per-frame LUTs on stream_, without a copy; sized_out (may be null) receives the record they used
+  int atmosphere_luts_device(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3], float sun_intensity,
+                             OxcAtmosphere* sized_out);
+  uint16_t* d_sky_ibl_cube_ = nullptr; // the sky IBL cube, allocated and zeroed by the first atmosphere_sky_ibl
+  uint32_t sky_ibl_calls_ = 0;         // atmosphere_sky_ibl calls so far: the frame_index of the next one
   OxcLight* d_lights_ = nullptr;    // apply_pbr's lights buffer (OXC_MAX_LIGHTS records), allocated with d_pbr_
   bool has_external_depth_ = false;
   // transforms as the host last uploaded them, and on the device the values before the upload that last changed each of them

@@ -245,22 +245,26 @@ OXC_DI float canonical_log2(float x) {
   return fa((float)e, fm(t, p));
 }
 
-// binary64 operations of canonical_sincos: the device intrinsics are never contracted; the host build runs -ffp-contract=off
-OXC_DI double dmul64(double a, double b) {
+// functions the parameter builders also call on the host
+#define OXC_HD __host__ __device__ __forceinline__
+
+// binary64 operations of canonical_sincos, canonical_acos and canonical_atan2: the device intrinsics are never contracted; the host
+// build runs -ffp-contract=off
+OXC_HD double dmul64(double a, double b) {
 #ifdef __CUDA_ARCH__
   return __dmul_rn(a, b);
 #else
   return a * b;
 #endif
 }
-OXC_DI double dadd64(double a, double b) {
+OXC_HD double dadd64(double a, double b) {
 #ifdef __CUDA_ARCH__
   return __dadd_rn(a, b);
 #else
   return a + b;
 #endif
 }
-OXC_DI float d2f_rn(double a) {
+OXC_HD float d2f_rn(double a) {
 #ifdef __CUDA_ARCH__
   return __double2float_rn(a);
 #else
@@ -305,7 +309,7 @@ OXC_DI void canonical_sincos(float xf, float& s_out, float& c_out) {
 OXC_DI float canonical_sin(float x) { float s, c; canonical_sincos(x, s, c); return s; }
 OXC_DI float canonical_cos(float x) { float s, c; canonical_sincos(x, s, c); return c; }
 
-OXC_DI double ddiv64(double a, double b) {
+OXC_HD double ddiv64(double a, double b) {
 #ifdef __CUDA_ARCH__
   return __ddiv_rn(a, b);
 #else
@@ -388,7 +392,6 @@ OXC_DI float canonical_pow5(float xf) {
 
 // binary32 operations for functions the parameter builders also call on the host: the device intrinsics, or one IEEE operation in the
 // host code (compiled with -ffp-contract=off, as the library's host code is)
-#define OXC_HD __host__ __device__ __forceinline__
 OXC_HD float hd_mul(float a, float b) {
 #ifdef __CUDA_ARCH__
   return __fmul_rn(a, b);
@@ -448,29 +451,123 @@ OXC_HD float canonical_exp(float x) {
   return hd_mul(p, hd_pow2(ki));
 }
 
-// acos for the parameter builders (the sky view's beta, sky.slang:76), bit-identical to oracle/oxc_oracle_atmosphere.c
-// orc_acos_canonical.  Binary64 throughout, one rounding to binary32: for |x| <= 1/2, pi/2 - asin(x); above, 2 asin(sqrt((1 - |x|) / 2))
-// (x > 0) or pi - that (x < 0); asin(s) = s + s z P(z), z = s^2 <= 1/4, by its series to s^57 (coefficients by their recurrence in
-// binary64).  Before the rounding the error is a few units of 2^-53 relative, so the result is within 1 ulp of the exact acos.
-// |x| > 1 and NaN give NaN.  Host code only: the builders run it once per call.
-__host__ inline float canonical_acos(float xf) {
+// acos, bit-identical to oracle/oxc_oracle_atmosphere.c orc_acos_canonical: the parameter builders' beta (sky.slang:76, once per
+// call on the host) and the sky IBL's per-sample view-zenith angle (sky.slang:49, on the device).  Binary64 throughout, one rounding
+// to binary32: for |x| <= 1/2, pi/2 - asin(x); above, 2 asin(sqrt((1 - |x|) / 2)) (x > 0) or pi - that (x < 0); asin(s) = s + s z P(z),
+// z = s^2 <= 1/4, by its series to s^57.  The coefficients c[n] = central(n) / (2n + 1), central(n) = central(n - 1) * (2n - 1) / (2n),
+// are the binary64 values of that recurrence as the oracle evaluates it (tests/test_oracle_sky_ibl.py recomputes them), written out so
+// that the device does not rerun it per call.  Before the rounding the error is a few units of 2^-53 relative, so the result is within
+// 1 ulp of the exact acos.  |x| > 1 and NaN give NaN (0x7FC00000).
+OXC_HD float canonical_acos(float xf) {
   const double x = (double)xf;
-  if (!(x >= -1.0 && x <= 1.0)) return __builtin_nanf("");
-  const double a = x < 0.0 ? -x : x;
-  const double s = a <= 0.5 ? x : sqrt((1.0 - a) * 0.5);
-  double c[29];
-  double central = 1.0; // (2n)! / (4^n (n!)^2)
-  for (int n = 0; n < 29; n++) {
-    if (n > 0) central = central * (double)(2 * n - 1) / (double)(2 * n);
-    c[n] = central / (double)(2 * n + 1);
+  if (!(x >= -1.0 && x <= 1.0)) {
+#ifdef __CUDA_ARCH__
+    return __uint_as_float(0x7FC00000u);
+#else
+    return __builtin_nanf("");
+#endif
   }
-  const double z = s * s;
-  double p = c[28];
-  for (int n = 27; n >= 1; n--) p = c[n] + z * p;
-  const double as = s + (s * z) * p;
+  const double a = x < 0.0 ? -x : x;
+#ifdef __CUDA_ARCH__
+  const double s = a <= 0.5 ? x : __dsqrt_rn(dmul64(dadd64(1.0, -a), 0.5));
+#else
+  const double s = a <= 0.5 ? x : sqrt((1.0 - a) * 0.5);
+#endif
+  const double z = dmul64(s, s);
+  double p = 0x1.e82be60d9127ep-10;
+  p = dadd64(0x1.018f963c229bfp-9, dmul64(z, p));
+  p = dadd64(0x1.1052bc5fa960ap-9, dmul64(z, p));
+  p = dadd64(0x1.208d3570ae5a6p-9, dmul64(z, p));
+  p = dadd64(0x1.3275586c5f2f0p-9, dmul64(z, p));
+  p = dadd64(0x1.464c0950f7d47p-9, dmul64(z, p));
+  p = dadd64(0x1.5c5f56efaaaabp-9, dmul64(z, p));
+  p = dadd64(0x1.750de64d7d05fp-9, dmul64(z, p));
+  p = dadd64(0x1.90cb77f60c7cep-9, dmul64(z, p));
+  p = dadd64(0x1.b026f57b13b14p-9, dmul64(z, p));
+  p = dadd64(0x1.d3d2a8e0dd67dp-9, dmul64(z, p));
+  p = dadd64(0x1.fcaf8fb6db6dbp-9, dmul64(z, p));
+  p = dadd64(0x1.15ee9d45d1746p-8, dmul64(z, p));
+  p = dadd64(0x1.31683bdef7bdfp-8, dmul64(z, p));
+  p = dadd64(0x1.51ba308d3dcb1p-8, dmul64(z, p));
+  p = dadd64(0x1.782dda12f684cp-8, dmul64(z, p));
+  p = dadd64(0x1.a6863d70a3d71p-8, dmul64(z, p));
+  p = dadd64(0x1.df3bd37a6f4dfp-8, dmul64(z, p));
+  p = dadd64(0x1.12ef3cf3cf3cfp-7, dmul64(z, p));
+  p = dadd64(0x1.3fde50d79435ep-7, dmul64(z, p));
+  p = dadd64(0x1.7a87878787878p-7, dmul64(z, p));
+  p = dadd64(0x1.c99999999999ap-7, dmul64(z, p));
+  p = dadd64(0x1.1c4ec4ec4ec4fp-6, dmul64(z, p));
+  p = dadd64(0x1.6e8ba2e8ba2e9p-6, dmul64(z, p));
+  p = dadd64(0x1.f1c71c71c71c7p-6, dmul64(z, p));
+  p = dadd64(0x1.6db6db6db6db7p-5, dmul64(z, p));
+  p = dadd64(0x1.3333333333333p-4, dmul64(z, p));
+  p = dadd64(0x1.5555555555555p-3, dmul64(z, p));
+  const double as = dadd64(s, dmul64(dmul64(s, z), p));
   const double PI_D = 3.141592653589793116;
-  if (a <= 0.5) return (float)(PI_D * 0.5 - as);
-  return (float)(x > 0.0 ? 2.0 * as : PI_D - 2.0 * as);
+  if (a <= 0.5) return d2f_rn(dadd64(dmul64(PI_D, 0.5), -as));
+  return d2f_rn(x > 0.0 ? dmul64(2.0, as) : dadd64(PI_D, -dmul64(2.0, as)));
+}
+
+// atan2 for the sky IBL's per-sample longitude (sky.slang:64), bit-identical to oracle/oxc_oracle_sky_ibl.c orc_atan2_canonical.
+// Binary64 throughout, one rounding to binary32.  Special cases as C99 Annex F: a NaN operand gives NaN (0x7FC00000); y = +-0 gives
+// +-0 for x > 0 or x = +0 and +-pi for x < 0 or x = -0; x = +-0 (y != 0) gives +-pi/2; y = +-inf gives +-pi/4 (x = +inf), +-3 pi/4
+// (x = -inf), else +-pi/2; x = +inf (y finite) gives +-0 and x = -inf +-pi; the sign is y's.  Otherwise t = min(|y|, |x|) / max(|y|, |x|)
+// in [0, 1]; above tan(pi/8), atan(t) = pi/4 + atan((t - 1) / (t + 1)), so the series argument u has |u| <= tan(pi/8) and
+// atan(u) = u + u z P(z), z = u^2 <= 0.1716, by its series to u^45 (truncation below 2^-60 relative); then pi/2 - a when |y| > |x|,
+// pi - a when x < 0.  Before the rounding the error is a few units of 2^-53 relative, so the result is within 1 ulp of the exact
+// atan2 (tests/test_oracle_sky_ibl.py checks 10^7 inputs against binary64).
+OXC_HD float canonical_atan2(float yf, float xf) {
+  const double y = (double)yf, x = (double)xf;
+  const double PI_D = 3.141592653589793116, PIO2 = dmul64(PI_D, 0.5), PIO4 = dmul64(PI_D, 0.25);
+  if (y != y || x != x) {
+#ifdef __CUDA_ARCH__
+    return __uint_as_float(0x7FC00000u);
+#else
+    return __builtin_nanf("");
+#endif
+  }
+  const double ay = y < 0.0 ? -y : y, ax = x < 0.0 ? -x : x;
+  const double INF = dmul64(1e300, 1e300);
+  const bool x_neg = signbit(x);
+  double r;
+  if (ay == 0.0) r = x_neg ? PI_D : 0.0;
+  else if (ay == INF && ax == INF) r = x_neg ? dadd64(PI_D, -PIO4) : PIO4;
+  else if (ay == INF || ax == 0.0) r = PIO2;
+  else if (ax == INF) r = x_neg ? PI_D : 0.0;
+  else {
+    const bool swap = ay > ax;
+    const double t = swap ? ddiv64(ax, ay) : ddiv64(ay, ax);
+    const bool reduce = t > 0.41421356237309503;
+    const double u = reduce ? ddiv64(dadd64(t, -1.0), dadd64(t, 1.0)) : t;
+    const double z = dmul64(u, u);
+    double p = -1.0 / 45.0;
+    p = dadd64(1.0 / 43.0, dmul64(z, p));
+    p = dadd64(-1.0 / 41.0, dmul64(z, p));
+    p = dadd64(1.0 / 39.0, dmul64(z, p));
+    p = dadd64(-1.0 / 37.0, dmul64(z, p));
+    p = dadd64(1.0 / 35.0, dmul64(z, p));
+    p = dadd64(-1.0 / 33.0, dmul64(z, p));
+    p = dadd64(1.0 / 31.0, dmul64(z, p));
+    p = dadd64(-1.0 / 29.0, dmul64(z, p));
+    p = dadd64(1.0 / 27.0, dmul64(z, p));
+    p = dadd64(-1.0 / 25.0, dmul64(z, p));
+    p = dadd64(1.0 / 23.0, dmul64(z, p));
+    p = dadd64(-1.0 / 21.0, dmul64(z, p));
+    p = dadd64(1.0 / 19.0, dmul64(z, p));
+    p = dadd64(-1.0 / 17.0, dmul64(z, p));
+    p = dadd64(1.0 / 15.0, dmul64(z, p));
+    p = dadd64(-1.0 / 13.0, dmul64(z, p));
+    p = dadd64(1.0 / 11.0, dmul64(z, p));
+    p = dadd64(-1.0 / 9.0, dmul64(z, p));
+    p = dadd64(1.0 / 7.0, dmul64(z, p));
+    p = dadd64(-1.0 / 5.0, dmul64(z, p));
+    p = dadd64(1.0 / 3.0, dmul64(z, p)); // P(z) = 1/3 - z/5 + ...; atan(u) = u - u z P(z)
+    double a = dadd64(u, -dmul64(dmul64(u, z), p));
+    if (reduce) a = dadd64(PIO4, a);
+    r = swap ? dadd64(PIO2, -a) : a;
+    if (x_neg) r = dadd64(PI_D, -r);
+  }
+  return d2f_rn(signbit(y) ? -r : r);
 }
 
 // cull.slang:169-171: determinant(f32x3x3(c0.xyw, c1.xyw, c2.xyw)) >= 0.0001

@@ -29,6 +29,7 @@
 #include "kernels_pbr.cuh"
 #include "kernels_contact_shadows.cuh"
 #include "kernels_atmosphere.cuh"
+#include "kernels_sky_ibl.cuh"
 
 using namespace oxc;
 
@@ -1544,15 +1545,17 @@ int oxc_contact_shadows(OxcContext* c, const OxcContactShadowCamera* cam, const 
   return OXC_OK;
 }
 
-// the sizes a call reads: 1..4096 (the transmittance LUT's x / y for both calls)
-static int atmosphere_check_sizes(const OxcAtmosphere& a, bool per_frame) {
+// the sizes a call reads: 1..4096 (the transmittance LUT's x / y for every call), the sky view's 2..4096 (sky_view: the per-frame
+// LUTs and the sky IBL), the aerial perspective's (aerial: the per-frame LUTs)
+static int atmosphere_check_sizes(const OxcAtmosphere& a, bool sky_view, bool aerial) {
   const uint32_t* t = a.transmittance_lut_size;
   if (t[0] == 0 || t[1] == 0 || t[0] > OXC_ATMOSPHERE_MAX_LUT_SIZE || t[1] > OXC_ATMOSPHERE_MAX_LUT_SIZE)
     return fail(OXC_E_INVALID, "transmittance_lut_size %u x %u outside 1..%u", t[0], t[1], OXC_ATMOSPHERE_MAX_LUT_SIZE);
-  if (!per_frame) return OXC_OK;
+  if (!sky_view) return OXC_OK;
   const uint32_t* v = a.sky_view_lut_size;
   if (v[0] < 2 || v[1] < 2 || v[0] > OXC_ATMOSPHERE_MAX_LUT_SIZE || v[1] > OXC_ATMOSPHERE_MAX_LUT_SIZE)
     return fail(OXC_E_INVALID, "sky_view_lut_size %u x %u outside 2..%u", v[0], v[1], OXC_ATMOSPHERE_MAX_LUT_SIZE);
+  if (!aerial) return OXC_OK;
   const uint32_t* ap = a.aerial_perspective_lut_size;
   if (ap[0] == 0 || ap[1] == 0 || ap[2] == 0 || ap[0] > OXC_ATMOSPHERE_MAX_LUT_SIZE || ap[1] > OXC_ATMOSPHERE_MAX_LUT_SIZE ||
       ap[2] > OXC_ATMOSPHERE_MAX_AERIAL_DEPTH)
@@ -1565,7 +1568,7 @@ int oxc_atmosphere_transmittance(OxcContext* c, const OxcAtmosphere* atmosphere,
   if (!c || !atmosphere || !lut_dev) return fail(OXC_E_INVALID, "null argument");
   if (reinterpret_cast<uintptr_t>(lut_dev) & 7u) return fail(OXC_E_INVALID, "lut_dev must be 8-byte aligned");
   int rc;
-  if ((rc = atmosphere_check_sizes(*atmosphere, false)) != OXC_OK) return rc;
+  if ((rc = atmosphere_check_sizes(*atmosphere, false, false)) != OXC_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
   const AtmosphereParams p = atmosphere_make_params(*atmosphere, nullptr, nullptr, 0.0f, nullptr, lut_dev, nullptr, nullptr, 0);
@@ -1584,7 +1587,7 @@ int oxc_atmosphere_sky_luts(OxcContext* c, const OxcAtmosphere* atmosphere, cons
        reinterpret_cast<uintptr_t>(aerial_perspective_dev)) & 7u)
     return fail(OXC_E_INVALID, "transmittance_dev, sky_view_dev and aerial_perspective_dev must be 8-byte aligned");
   int rc;
-  if ((rc = atmosphere_check_sizes(*atmosphere, true)) != OXC_OK) return rc;
+  if ((rc = atmosphere_check_sizes(*atmosphere, true, true)) != OXC_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
   const OxcAtmosphere& a = *atmosphere;
@@ -1595,6 +1598,31 @@ int oxc_atmosphere_sky_luts(OxcContext* c, const OxcAtmosphere* atmosphere, cons
   const AtmosphereParams p = atmosphere_make_params(a, camera, sun_direction, sun_intensity, transmittance_dev, nullptr, sky_view_dev,
                                                     aerial_perspective_dev, sky_blocks);
   k_atmosphere_sky_luts<<<sky_blocks + aerial_blocks, ATMOSPHERE_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_atmosphere_sky_ibl(OxcContext* c, const OxcAtmosphere* atmosphere, const OxcPbrCamera* camera, const float sun_direction[3],
+                           float sun_intensity, float sun_ambient_strength, uint32_t frame_index, const uint16_t* transmittance_dev,
+                           const uint16_t* sky_view_dev, uint16_t* cube_dev, void* stream) {
+  if (!c || !atmosphere || !camera || !sun_direction || !transmittance_dev || !sky_view_dev || !cube_dev)
+    return fail(OXC_E_INVALID, "null argument");
+  if ((reinterpret_cast<uintptr_t>(transmittance_dev) | reinterpret_cast<uintptr_t>(sky_view_dev) | reinterpret_cast<uintptr_t>(cube_dev)) & 7u)
+    return fail(OXC_E_INVALID, "transmittance_dev, sky_view_dev and cube_dev must be 8-byte aligned");
+  int rc;
+  if ((rc = atmosphere_check_sizes(*atmosphere, true, false)) != OXC_OK) return rc;
+  const OxcAtmosphere& a = *atmosphere;
+  // the cube is written while both LUTs are read: it may not share a byte with either
+  const uintptr_t cube = reinterpret_cast<uintptr_t>(cube_dev), cube_end = cube + (uintptr_t)OXC_SKY_IBL_CUBE_BYTES;
+  const uintptr_t t = reinterpret_cast<uintptr_t>(transmittance_dev), t_end = t + (uintptr_t)a.transmittance_lut_size[0] * a.transmittance_lut_size[1] * 8;
+  const uintptr_t sv = reinterpret_cast<uintptr_t>(sky_view_dev), sv_end = sv + (uintptr_t)a.sky_view_lut_size[0] * a.sky_view_lut_size[1] * 8;
+  if ((cube < t_end && t < cube_end) || (cube < sv_end && sv < cube_end))
+    return fail(OXC_E_INVALID, "cube_dev overlaps transmittance_dev or sky_view_dev");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  const SkyIblParams p = sky_ibl_make_params(a, *camera, sun_direction, sun_intensity, sun_ambient_strength, frame_index, transmittance_dev,
+                                             sky_view_dev, cube_dev);
+  k_atmosphere_sky_ibl<<<SKY_IBL_BLOCKS, SKY_IBL_THREADS, 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }
