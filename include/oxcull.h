@@ -1133,6 +1133,62 @@ int oxc_atmosphere_sky_ibl(OxcContext* ctx, const OxcAtmosphere* atmosphere, con
                            float sun_intensity, float sun_ambient_strength, uint32_t frame_index, const uint16_t* transmittance_dev,
                            const uint16_t* sky_view_dev, uint16_t* cube_dev, void* stream);
 
+/* Lighting under the atmosphere: the pbr_apply variant of RendererInstance::apply_pbr (Passes/PBR.cpp:312-432, passes/pbr_apply.slang
+ * :26-184 with the sky.slang functions it calls), which the reference runs instead of oxc_apply_pbr's when the scene has an
+ * AtmosphereComponent (HasAtmosphere, RendererInstance.cpp:1442-1460).  One float4 (RGBA) per pixel into out_dev, from the planes and
+ * lights oxc_apply_pbr takes (same layouts and alignment) and the sky's four binary16 RGBA planes (OxcPbrSky): the transmittance LUT as
+ * oxc_atmosphere_transmittance wrote it, the sky-view and aerial-perspective LUTs as oxc_atmosphere_sky_luts wrote them, the cube as
+ * oxc_atmosphere_sky_ibl wrote it.  No scratch, so the call is graph-capturable from its first call.  Settings read: scene_flags,
+ * sun_direction (L, as given), sun_intensity (Li), light_count; base_ambient_color and the sky_* fields are not read (the shader overwrites
+ * both sky terms) and HasSky changes nothing.  Atmosphere fields read: planet_radius, atmos_radius, aerial_perspective_start_km,
+ * aerial_perspective_exposure and the transmittance, sky-view and aerial-perspective sizes.
+ * Refused with OXC_E_INVALID, before anything is launched: everything oxc_apply_pbr refuses except OXC_SCENE_HAS_ATMOSPHERE; settings
+ * WITHOUT OXC_SCENE_HAS_ATMOSPHERE (that bit selects this shader); a NULL record, sky or sky plane; a sky plane not 8-byte aligned; the LUT
+ * sizes oxc_atmosphere_sky_luts refuses.  NaN, Inf and denormal values in the LUTs, cube, record, camera, settings and planes are accepted.
+ * SPECIFICATION (oracle/oxc_oracle_pbr_atmosphere.c orc_apply_pbr_atmosphere, bit for bit): oxc_apply_pbr's rules and its items 1-3, 5
+ * and 7 (pixel centre, binary16 normal plane and AO, binary32 G-buffer reads, light kinds, output with every NaN 0x7FFFFFFF), the
+ * atmosphere's rules (oxc_atmosphere_transmittance: get_eye_pos, canonical_exp / canonical_acos / canonical_atan2, the tap of item 5
+ * reading binary16 exactly), cross(a, b) = (a.y*b.z - a.z*b.y, a.z*b.x - a.x*b.z, a.x*b.y - a.y*b.x), normalize of a 2-vector = v /
+ * sqrt(v.x*v.x + v.y*v.y).  Commitments where the shader leaves the outcome open:
+ *   1. order: TransparentBackground and depth == 0 gives (0, 0, 0, 0); then the prologue, with the pixel's sun transmittance; then
+ *      depth == 0 takes the sky path (item 4) and every other pixel the full path.
+ *   2. per call, on the host: sun_cos_theta = dot(L, (0, 1, 0)); horizon_darkening = smoothstep(-0.1, 0.3, sun_cos_theta); draw_sun's
+ *      min_cos = canonical_cos(fl(fl(1 * PI) / 180)) with the argument 0x3C8EFA35; the camera's eye = get_eye_pos(camera.position) with
+ *      altitude h = eye.y as written (not length(eye) as the IBL), horizon = safe_sqrt(h*h - R*R), beta = canonical_acos(horizon / h),
+ *      PI - beta.
+ *   3. sun transmittance: the transmittance tap at transmittance_params_to_lut_uv(atmos_radius, planet_radius, (get_eye_pos(world).y,
+ *      sun_cos_theta)), rgb; direct = (T * Li) * horizon_darkening per channel, not gated by HasDirectionalLight (the shadow read is).
+ *   4. sky pixels: right = normalize(cross(up, -V)) with no fallback (NaN for a vertical view, which follows the rules), forward =
+ *      normalize(cross(right, up)), light_on_plane = plain normalize((dot(L, forward), dot(L, right))), the planet hit from the camera's
+ *      eye, sky_view_params_to_lut_uv as for the IBL, the sky-view tap on all four channels; without a planet hit rgb += (draw_sun(-V, L)
+ *      * Li) * T per channel, draw_sun = cos >= min_cos ? 1 : canonical_exp(-offset * 50000) * 0.5 + (1 / (0.02 + offset * 300)) * 0.01
+ *      with offset = min_cos - cos, cos = dot(-V, L).  Output (rgb * a, 1); there is no HasSky early return in this shader.
+ *   5. aerial perspective (sky.slang:258-293): per_slice_depth = f32(size.x) / f32(size.z), a binary32 division (the LUT pass's item 8
+ *      divides integers; the two differ at 32 x 32 x 24); rcp(x) = fl(1 / x); half_slice_depth 0x3F3504F3; near_depth_fade_out = 1.0 /
+ *      0.001 folded in binary32 like the other folds, fl(1 / fl(0.001)) = 0x4479FFFF (a binary64 fold would give 0x447A0000).  The 3D tap
+ *      is item 5's bilinear rule in slices z0 = floor(w * D - 0.5) and z0 + 1 (same NaN-safe clamped indices), then s0 + wz * (s1 - s0).
+ *      Then rgb *= weight, a = 1 - weight * (1 - a), rgb *= exposure; the contribution is rgb * a.
+ *   6. cube tap (TextureCube.SampleLevel, linear, level 0): the face by the major axis as in the Vulkan specification's cube map face
+ *      selection table, ties to X over Y over Z (X when |x| >= |y| and |x| >= |z|, else Y when |y| >= |z|), the positive face when the
+ *      major component is >= 0 (so -0 too); s = 0.5 * (sc / |ma|) + 0.5, t likewise; x = s * 32 - 0.5, the 2 x 2 footprint of item 5
+ *      with indices in -1..32.  Seamless, as the specification's cube map edge handling: a texel one step off an edge is the adjacent
+ *      face's texel that shares the edge; a corner texel (off both edges, which the specification leaves to the implementation) is
+ *      ((inside + across x) + across y) / 3 of the three texels that meet there.  A NaN or zero direction (normalize(lerp(N, R, 1 -
+ *      roughness)) is 0 / 0 for R = -N at roughness 0.5) selects by the same comparisons (all NaN: face 5; zero: face 0), reads texels 0 and
+ *      1 (NaN-safe indices) and returns NaN.  specular_sky = (rgb * a) * horizon_darkening at that direction, diffuse_sky likewise at N.
+ *   7. sum: ((((surface + lights) + indirect) + emission) + aerial), indirect as oxc_apply_pbr's with the two sky terms, surface with the
+ *      per-channel direct. */
+typedef struct OxcPbrSky {               /* the atmosphere variant's extra inputs, binary16 RGBA, 8-byte aligned */
+  const uint16_t* transmittance;         /* transmittance_lut_size.xy, as oxc_atmosphere_transmittance wrote it */
+  const uint16_t* sky_view;              /* sky_view_lut_size.xy, as oxc_atmosphere_sky_luts wrote it */
+  const uint16_t* aerial_perspective;    /* aerial_perspective_lut_size.xyz */
+  const uint16_t* sky_cube;              /* 6 x 32 x 32, oxc_atmosphere_sky_ibl's layout */
+} OxcPbrSky;
+OXC_STATIC_ASSERT(sizeof(OxcPbrSky) == 32, "PbrSky");
+int oxc_apply_pbr_atmosphere(OxcContext* ctx, const OxcPbrCamera* camera, const OxcPbrSettings* settings, const OxcAtmosphere* atmosphere,
+                             const OxcLight* lights_dev, const OxcPbrInputs* inputs, const OxcPbrSky* sky, uint32_t width, uint32_t height,
+                             float* out_dev, void* stream);
+
 int oxc_get_outputs(OxcContext* ctx, OxcOutputs* out);
 /* Instrumentation hook: 128 u64 counters that builds with -DOXC_RASTER_STATS fill (tools/raster_stats.py); zero otherwise. */
 void* oxc_debug_stats_ptr(OxcContext* ctx);
@@ -1287,6 +1343,18 @@ int oxr_apply_pbr_with_contact_shadows(OxrRenderer* r, const OxcCullCamera* came
                                        const OxcLight* lights_host, int cast_shadows, const OxcGtaoCamera* gtao_camera,
                                        const OxcGtaoSettings* gtao_settings, const OxcContactShadowCamera* contact_camera,
                                        const OxcContactShadowSettings* contact_settings, float* rgba_host);
+/* RendererInstance::apply_pbr with an atmosphere (PBR.cpp:312-432) and the passes before it, on the renderer's stream, synchronous:
+ *   1. the per-frame LUTs and the sky IBL cube update exactly as oxr_atmosphere_sky_ibl makes them (the same planes, the bake at the
+ *      first use, the same cube and call counter, which this call advances) with pbr_camera, settings->sun_direction and ->sun_intensity;
+ *   2. the G-buffer decode, shadow resolve, contact shadows and GTAO as oxr_apply_pbr_with_contact_shadows runs them;
+ *   3. oxc_apply_pbr_atmosphere over those planes and tables, the record's sizes replaced by the renderer's extents.
+ * settings must carry OXC_SCENE_HAS_ATMOSPHERE and OXC_SCENE_HAS_DIRECTIONAL_LIGHT (OXC_E_INVALID otherwise, before anything is
+ * enqueued): the reference updates its sky tables only under HasDirectionalLight (RendererInstance.cpp:1022), so HasAtmosphere
+ * without it samples tables no pass wrote in that frame.  width x height float4 to rgba_host.  OXC_E_CAPACITY as oxr_apply_pbr. */
+int oxr_apply_pbr_atmosphere(OxrRenderer* r, const OxcCullCamera* camera, const OxcPbrCamera* pbr_camera, const OxcPbrSettings* settings,
+                             const OxcAtmosphere* atmosphere, const OxcLight* lights_host, int cast_shadows, const OxcGtaoCamera* gtao_camera,
+                             const OxcGtaoSettings* gtao_settings, const OxcContactShadowCamera* contact_camera,
+                             const OxcContactShadowSettings* contact_settings, float* rgba_host);
 /* The atmosphere's lookup tables as the reference makes them, on the renderer's stream, synchronous.  At its first call the renderer
  * allocates its three planes at the reference's extents (transmittance 256 x 64, sky view 312 x 192, aerial perspective 32 x 32 x 32; about
  * 0.7 MiB) and bakes the transmittance LUT once with the DEFAULT record (GPU::Atmosphere{} with those sizes), as the reference's init does:

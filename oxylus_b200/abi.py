@@ -493,6 +493,15 @@ ATMOSPHERE_DEFAULTS = dict(rayleigh_scatter=(0.005802, 0.013558, 0.033100), rayl
                            sky_view_lut_size=(312, 192, 1), multiscattering_lut_size=(32, 32, 1), aerial_perspective_lut_size=(32, 32, 32))
 
 
+class PbrSky(C.Structure):
+    """OxcPbrSky: the atmospheric PBR apply's sky planes (device pointers, binary16 RGBA, 8-byte aligned)"""
+    _fields_ = [("transmittance", C.c_void_p), ("sky_view", C.c_void_p), ("aerial_perspective", C.c_void_p), ("sky_cube", C.c_void_p)]
+
+
+PBR_SKY_PLANES = ("transmittance", "sky_view", "aerial_perspective", "sky_cube")
+assert C.sizeof(PbrSky) == 32
+
+
 # the sky IBL cube (oxc_atmosphere_sky_ibl): 6 faces x 32 x 32 binary16 RGBA texels, 64 sky-view samples per texel per call
 SKY_IBL_CUBE_RES = 32
 SKY_IBL_SAMPLES = 64

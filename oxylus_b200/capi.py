@@ -22,7 +22,7 @@ SYMBOLS = [
     "oxc_decode_visbuffer", "oxc_decode_gbuffer", "oxc_build_hpb", "oxc_mark_visible_pages",
     "oxc_vsm_begin_frame", "oxc_vsm_invalidate_pages", "oxc_vsm_allocate_pages", "oxc_vsm_clear_dirty_pages", "oxc_cull_meshlets_hpb_dirty_dev",
     "oxc_vsm_draw_pages", "oxc_vsm_draw_stats", "oxc_vsm_resolve_shadows", "oxc_generate_ambient_occlusion", "oxc_apply_pbr",
-    "oxc_contact_shadows", "oxc_atmosphere_transmittance", "oxc_atmosphere_sky_luts", "oxc_atmosphere_sky_ibl",
+    "oxc_contact_shadows", "oxc_atmosphere_transmittance", "oxc_atmosphere_sky_luts", "oxc_atmosphere_sky_ibl", "oxc_apply_pbr_atmosphere", "oxr_apply_pbr_atmosphere",
     "oxc_get_outputs", "oxc_check_status", "oxc_mark_hiz_dirty", "oxc_bind_camera_buffer", "oxc_load_camera", "oxc_debug_stats_ptr",
     "oxc_mgpu_get_unique_id", "oxc_mgpu_init", "oxc_mgpu_init_with_comm", "oxc_mgpu_shutdown", "oxc_mgpu_info", "oxc_mgpu_exchange_hiz",
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
@@ -162,6 +162,10 @@ def load(build_if_missing=True):
     lib.oxc_atmosphere_sky_ibl.argtypes = [vp, C.POINTER(abi.Atmosphere), C.POINTER(abi.PbrCamera), vp, C.c_float, C.c_float, u32, vp, vp, vp,
                                            vp]
     lib.oxr_atmosphere_sky_ibl.argtypes = [vp, C.POINTER(abi.Atmosphere), C.POINTER(abi.PbrCamera), vp, C.c_float, vp]
+    lib.oxr_apply_pbr_atmosphere.argtypes = [vp, vp, C.POINTER(abi.PbrCamera), C.POINTER(abi.PbrSettings), C.POINTER(abi.Atmosphere), vp,
+                                             C.c_int, vp, vp, vp, vp, vp]
+    lib.oxc_apply_pbr_atmosphere.argtypes = [vp, C.POINTER(abi.PbrCamera), C.POINTER(abi.PbrSettings), C.POINTER(abi.Atmosphere), vp,
+                                             C.POINTER(abi.PbrInputs), C.POINTER(abi.PbrSky), u32, u32, vp, vp]
     _LIB = lib
     return lib
 
@@ -516,6 +520,15 @@ class Context:
         _check(self.lib.oxc_apply_pbr(self.h, C.byref(pbr_camera), C.byref(settings), _ptr(lights_dev), C.byref(t), w, h, _ptr(out_dev),
                                       self.stream), "oxc_apply_pbr")
 
+    def apply_pbr_atmosphere(self, pbr_camera, settings, atmosphere, lights_dev, inputs, sky, w, h, out_dev):
+        """oxc_apply_pbr_atmosphere: the lit RGBA (float4 per pixel) of a w x h frame under the atmosphere into out_dev.  As apply_pbr, plus
+        atmosphere (abi.Atmosphere) and sky: dict transmittance, sky_view, aerial_perspective, sky_cube -> device pointers (or
+        abi.PbrSky); settings must carry SCENE_HAS_ATMOSPHERE"""
+        t = inputs if isinstance(inputs, abi.PbrInputs) else abi.PbrInputs(*[inputs.get(k) for k in abi.PBR_INPUTS])
+        k = sky if isinstance(sky, abi.PbrSky) else abi.PbrSky(*[sky.get(n) for n in abi.PBR_SKY_PLANES])
+        _check(self.lib.oxc_apply_pbr_atmosphere(self.h, C.byref(pbr_camera), C.byref(settings), C.byref(atmosphere), _ptr(lights_dev),
+                                                 C.byref(t), C.byref(k), w, h, _ptr(out_dev), self.stream), "oxc_apply_pbr_atmosphere")
+
     def atmosphere_transmittance(self, atmosphere, lut_dev):
         """oxc_atmosphere_transmittance: the transmittance LUT (binary16 RGBA, atmosphere.transmittance_lut_size) into lut_dev"""
         _check(self.lib.oxc_atmosphere_transmittance(self.h, C.byref(atmosphere), _ptr(lut_dev), self.stream), "oxc_atmosphere_transmittance")
@@ -828,6 +841,25 @@ class Renderer:
         _check(self.lib.oxr_atmosphere_sky_ibl(self.h, C.byref(atmosphere), C.byref(camera), sun, float(np.float32(sun_intensity)), _ptr(cube)),
                "oxr_atmosphere_sky_ibl")
         return cube
+
+    def apply_pbr_atmosphere(self, cam, settings, atmosphere, lights=None, cast_shadows=False, gtao_camera=None, gtao_settings=None,
+                             pbr_camera=None, contact_camera=None, contact_settings=None):
+        """oxr_apply_pbr_atmosphere: the per-frame LUTs and the cube update (as atmosphere_sky_ibl, advancing its counter), the chain of
+        apply_pbr, then the atmospheric PBR apply with the record (abi.Atmosphere); settings must carry SCENE_HAS_ATMOSPHERE and
+        SCENE_HAS_DIRECTIONAL_LIGHT.  Returns float32 [height, width, 4]"""
+        from oxylus_b200 import synth
+
+        n = 0 if lights is None else len(lights)
+        settings = abi.PbrSettings.from_buffer_copy(settings)
+        settings.light_count = n
+        pc = pbr_camera if pbr_camera is not None else synth.pbr_camera(cam)
+        out = np.zeros((self.scene.height, self.scene.width, 4), dtype=np.float32)
+        opt = lambda v: C.byref(v) if v is not None else None
+        _check(self.lib.oxr_apply_pbr_atmosphere(self.h, _ptr(cam), C.byref(pc), C.byref(settings), C.byref(atmosphere),
+                                                 C.cast(lights, C.c_void_p) if n else None, int(bool(cast_shadows)), opt(gtao_camera),
+                                                 opt(gtao_settings), opt(contact_camera), opt(contact_settings), _ptr(out)),
+               "oxr_apply_pbr_atmosphere")
+        return out
 
     def apply_pbr(self, cam, settings, lights=None, cast_shadows=False, gtao_camera=None, gtao_settings=None, pbr_camera=None,
                   contact_camera=None, contact_settings=None):

@@ -443,15 +443,21 @@ int RendererInstance::generate_ambient_occlusion_device(const OxcGtaoCamera& gta
 // the lighting into the renderer's output plane
 auto RendererInstance::apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera& pbr_camera, const OxcPbrSettings& settings, const OxcLight* lights_host,
                                  bool cast_shadows, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* gtao_settings, float* rgba_host,
-                                 const OxcContactShadowCamera* contact_camera, const OxcContactShadowSettings* contact_settings) -> int {
+                                 const OxcContactShadowCamera* contact_camera, const OxcContactShadowSettings* contact_settings,
+                                 const OxcAtmosphere* atmosphere) -> int {
   if (!ctx_ || !error_.empty()) return OXC_E_STATE;
   const bool gtao = (settings.scene_flags & OXC_SCENE_HAS_GTAO) != 0;
   const bool contact = (settings.scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS) != 0;
   if (!rgba_host || (gtao && (!gtao_camera || !gtao_settings)) || (settings.light_count > 0 && !lights_host)) return OXC_E_INVALID;
   if (contact && (!contact_camera || !contact_settings || contact_settings->steps < 1u || contact_settings->steps > OXC_CONTACT_SHADOW_MAX_STEPS))
     return OXC_E_INVALID; // refused before anything is enqueued
-  if (settings.light_count > OXC_MAX_LIGHTS || (settings.scene_flags & OXC_SCENE_HAS_ATMOSPHERE))
-    return OXC_E_INVALID; // no atmosphere variant: refused before anything is enqueued
+  if (settings.light_count > OXC_MAX_LIGHTS || (!atmosphere && (settings.scene_flags & OXC_SCENE_HAS_ATMOSPHERE)))
+    return OXC_E_INVALID; // the atmosphere variant takes a record: refused before anything is enqueued
+  // the atmosphere variant: HasAtmosphere selects it, and the reference makes its sky tables only under HasDirectionalLight
+  // (RendererInstance.cpp:1022), so without a sun it would read tables no pass wrote that frame
+  if (atmosphere && (settings.scene_flags & (OXC_SCENE_HAS_ATMOSPHERE | OXC_SCENE_HAS_DIRECTIONAL_LIGHT)) !=
+                        (OXC_SCENE_HAS_ATMOSPHERE | OXC_SCENE_HAS_DIRECTIONAL_LIGHT))
+    return OXC_E_INVALID;
   if (cast_shadows && !vsm_.updated) return OXC_E_STATE;
   cudaStream_t s = static_cast<cudaStream_t>(stream_);
   const size_t px = (size_t)width_ * height_;
@@ -465,9 +471,18 @@ auto RendererInstance::apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera
     cudaFree(d_pbr_); d_pbr_ = nullptr;
     return OXC_E_CAPACITY;
   }
+  int rc;
+  OxcAtmosphere sized{};
+  if (atmosphere) { // RendererInstance.cpp:1022: the per-frame LUTs and the cube update before the geometry's lighting chain
+    if ((rc = sky_ibl_device(*atmosphere, pbr_camera, settings.sun_direction, settings.sun_intensity)) != OXC_OK) return rc;
+    sized = *atmosphere;
+    for (int i = 0; i < 3; i++) {
+      sized.transmittance_lut_size[i] = i < 2 ? kTransmittanceLut[i] : 1; sized.sky_view_lut_size[i] = i < 2 ? kSkyViewLut[i] : 1;
+      sized.multiscattering_lut_size[i] = i < 2 ? kMultiscatteringLut[i] : 1; sized.aerial_perspective_lut_size[i] = kAerialLut[i];
+    }
+  }
   OxcGBufferTargets gb{};
   gb.albedo = d_gbuffer_; gb.normal = d_gbuffer_ + px * 4; gb.emissive = d_gbuffer_ + px * 8; gb.metallic_roughness_occlusion = d_gbuffer_ + px * 12;
-  int rc;
   if ((rc = decode_gbuffer_device(camera, gb)) != OXC_OK) return rc;
   OxcPbrInputs in{};
   in.albedo = gb.albedo; in.normal = gb.normal; in.emissive = gb.emissive; in.metallic_roughness_occlusion = gb.metallic_roughness_occlusion;
@@ -489,7 +504,13 @@ auto RendererInstance::apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera
   if (settings.light_count &&
       cudaMemcpyAsync(d_lights_, lights_host, settings.light_count * sizeof(OxcLight), cudaMemcpyHostToDevice, s) != cudaSuccess)
     return fail(OXC_E_CUDA);
-  rc = oxc_apply_pbr(ctx_, &pbr_camera, &settings, d_lights_, &in, width_, height_, d_pbr_, stream_);
+  if (atmosphere) {
+    const size_t t_texels = (size_t)kTransmittanceLut[0] * kTransmittanceLut[1], sv_texels = (size_t)kSkyViewLut[0] * kSkyViewLut[1];
+    const OxcPbrSky sky{d_atmosphere_, d_atmosphere_ + t_texels * 4, d_atmosphere_ + (t_texels + sv_texels) * 4, d_sky_ibl_cube_};
+    rc = oxc_apply_pbr_atmosphere(ctx_, &pbr_camera, &settings, &sized, d_lights_, &in, &sky, width_, height_, d_pbr_, stream_);
+  } else {
+    rc = oxc_apply_pbr(ctx_, &pbr_camera, &settings, d_lights_, &in, width_, height_, d_pbr_, stream_);
+  }
   if (rc != OXC_OK) return fail(rc);
   if (cudaMemcpyAsync(rgba_host, d_pbr_, px * 16, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
     return fail(OXC_E_CUDA);
@@ -572,9 +593,9 @@ auto RendererInstance::atmosphere_luts(const OxcAtmosphere& atmosphere, const Ox
 }
 
 // the per-frame LUTs as atmosphere_luts makes them, then the sky IBL cube (PBR.cpp:52-94) into the renderer's cube with
-// sun_ambient_strength 0.15 and frame_index = the count of earlier calls, synchronous
-auto RendererInstance::atmosphere_sky_ibl(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3],
-                                          float sun_intensity, uint16_t* cube_host) -> int {
+// sun_ambient_strength 0.15 and frame_index = the count of earlier calls, on stream_ without a copy
+int RendererInstance::sky_ibl_device(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3],
+                                     float sun_intensity) {
   OxcAtmosphere sized;
   int rc;
   if ((rc = atmosphere_luts_device(atmosphere, camera, sun_direction, sun_intensity, &sized)) != OXC_OK) return rc;
@@ -595,6 +616,15 @@ auto RendererInstance::atmosphere_sky_ibl(const OxcAtmosphere& atmosphere, const
                                    stream_)) != OXC_OK)
     return fail(rc);
   sky_ibl_calls_++;
+  return OXC_OK;
+}
+
+// sky_ibl_device, then the cube to the host, synchronous
+auto RendererInstance::atmosphere_sky_ibl(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3],
+                                          float sun_intensity, uint16_t* cube_host) -> int {
+  int rc;
+  if ((rc = sky_ibl_device(atmosphere, camera, sun_direction, sun_intensity)) != OXC_OK) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
   if ((cube_host && cudaMemcpyAsync(cube_host, d_sky_ibl_cube_, OXC_SKY_IBL_CUBE_BYTES, cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
       cudaStreamSynchronize(s) != cudaSuccess)
     return fail(OXC_E_CUDA);
@@ -1123,6 +1153,15 @@ int oxr_apply_pbr(OxrRenderer* r, const OxcCullCamera* camera, const OxcPbrCamer
   // HasContactShadows needs the contact-shadow pass's camera and settings: oxr_apply_pbr_with_contact_shadows takes them
   if (settings->scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS) return OXC_E_INVALID;
   return r->impl.apply_pbr(*camera, *pbr_camera, *settings, lights_host, cast_shadows != 0, gtao_camera, gtao_settings, rgba_host);
+}
+
+int oxr_apply_pbr_atmosphere(OxrRenderer* r, const OxcCullCamera* camera, const OxcPbrCamera* pbr_camera, const OxcPbrSettings* settings,
+                             const OxcAtmosphere* atmosphere, const OxcLight* lights_host, int cast_shadows, const OxcGtaoCamera* gtao_camera,
+                             const OxcGtaoSettings* gtao_settings, const OxcContactShadowCamera* contact_camera,
+                             const OxcContactShadowSettings* contact_settings, float* rgba_host) {
+  if (!r || !camera || !pbr_camera || !settings || !atmosphere) return OXC_E_INVALID;
+  return r->impl.apply_pbr(*camera, *pbr_camera, *settings, lights_host, cast_shadows != 0, gtao_camera, gtao_settings, rgba_host, contact_camera,
+                           contact_settings, atmosphere);
 }
 
 int oxr_atmosphere_luts(OxrRenderer* r, const OxcAtmosphere* atmosphere, const OxcPbrCamera* camera, const float sun_direction[3],

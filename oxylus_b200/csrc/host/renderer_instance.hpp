@@ -90,7 +90,10 @@ public:
   // arguments required then) between the resolve and the GTAO, as the reference orders them; width x height float4 to the host
   auto apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera& pbr_camera, const OxcPbrSettings& settings, const OxcLight* lights_host,
                  bool cast_shadows, const OxcGtaoCamera* gtao_camera, const OxcGtaoSettings* gtao_settings, float* rgba_host,
-                 const OxcContactShadowCamera* contact_camera = nullptr, const OxcContactShadowSettings* contact_settings = nullptr) -> int;
+                 const OxcContactShadowCamera* contact_camera = nullptr, const OxcContactShadowSettings* contact_settings = nullptr,
+                 const OxcAtmosphere* atmosphere = nullptr) -> int;
+  // with a record (apply_pbr_atmosphere, PBR.cpp:312-432): the settings must carry HasAtmosphere and HasDirectionalLight; the per-frame
+  // LUTs and the cube update run first (RendererInstance.cpp:1022, as atmosphere_sky_ibl), then the chain above, then the atmospheric pass
   // the contact_shadows pass (RendererInstance.cpp:990-1020) on the last rendered frame's depth; width x height floats to the host
   auto contact_shadows(const OxcContactShadowCamera& contact_camera, const OxcContactShadowSettings& settings, float* contact_host) -> int;
   // the atmosphere's LUTs (RendererInstance.cpp:203-226 bake with the default record, once; PBR.cpp:11-50 and :96-140 per call with
@@ -198,6 +201,7 @@ private:
                              OxcAtmosphere* sized_out);
   uint16_t* d_sky_ibl_cube_ = nullptr; // the sky IBL cube, allocated and zeroed by the first atmosphere_sky_ibl
   uint32_t sky_ibl_calls_ = 0;         // atmosphere_sky_ibl calls so far: the frame_index of the next one
+  int sky_ibl_device(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3], float sun_intensity);
   OxcLight* d_lights_ = nullptr;    // apply_pbr's lights buffer (OXC_MAX_LIGHTS records), allocated with d_pbr_
   bool has_external_depth_ = false;
   // transforms as the host last uploaded them, and on the device the values before the upload that last changed each of them

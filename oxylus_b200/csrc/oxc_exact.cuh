@@ -276,8 +276,8 @@ OXC_HD float d2f_rn(double a) {
 // r = (x - k * PIO2_HI) - k * PIO2_LO (PIO2_HI has 33 significant bits, so k * PIO2_HI is exact for |k| < 2^20), Taylor
 // polynomials of sin (to r^15) and cos (to r^16) on |r| <= pi/4, the quadrant k mod 4, one rounding to binary32.
 // Error against the exact sin / cos: <= 1 ulp of the binary32 result on [0, 2 pi]; <= 2^-24 absolute for |x| <= 2^21 (the hash's
-// arguments reach 1.43e6 at 3840 x 2160).  Non-finite x gives NaN.
-OXC_DI void canonical_sincos(float xf, float& s_out, float& c_out) {
+// arguments reach 1.43e6 at 3840 x 2160).  Non-finite x gives NaN.  The host runs it for per-call constants (draw_sun's cosine).
+OXC_HD void canonical_sincos(float xf, float& s_out, float& c_out) {
   const double x = (double)xf;
   if (!(x - x == 0.0)) { s_out = c_out = xf - xf; return; } // inf / NaN -> NaN
   const double k = rint(dmul64(x, 0.63661977236758134308));
@@ -307,7 +307,7 @@ OXC_DI void canonical_sincos(float xf, float& s_out, float& c_out) {
   c_out = d2f_rn(cv);
 }
 OXC_DI float canonical_sin(float x) { float s, c; canonical_sincos(x, s, c); return s; }
-OXC_DI float canonical_cos(float x) { float s, c; canonical_sincos(x, s, c); return c; }
+OXC_HD float canonical_cos(float x) { float s, c; canonical_sincos(x, s, c); return c; }
 
 OXC_HD double ddiv64(double a, double b) {
 #ifdef __CUDA_ARCH__

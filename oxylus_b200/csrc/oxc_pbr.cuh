@@ -186,51 +186,65 @@ OXC_DI void pbr_add_light(const PbrSurface& s, PbrV3 world, const PbrLight& l, P
 // the stored value: every NaN is written as 0x7FFFFFFF
 OXC_DI float pbr_store(float v) { return v != v ? __uint_as_float(0x7FFFFFFFu) : v; }
 
-// fs_main (pbr_apply_no_atmos.slang:23-127) of pixel (x, y) with the staged lights
-OXC_DI float4 pbr_pixel(const PbrParams& p, const PbrLight* lights, int x, int y) {
-  const size_t pix = (size_t)y * p.width + x;
-  const float depth = p.depth[pix];
-  if ((p.flags & PBR_FLAG_TRANSPARENT) && depth == 0.0f) return make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-  const float u = fd(fa((float)x, 0.5f), (float)p.width), v = fd(fa((float)y, 0.5f), (float)p.height);
-  const float4 alb = __ldg(p.albedo + pix);
+// what both fs_main variants compute from the G-buffer before their sky tests (pbr_apply_no_atmos.slang:40-67, pbr_apply.slang:57-83):
+// the surface terms that depend on no light and no sky (PbrSurface's N, V and NoV; the rest is set by pbr_shade), the world position,
+// R, the smooth normal and NoL
+struct PbrPixel {
+  PbrSurface s;
+  PbrV3 world, R, smooth, Ls;
+  float4 alb, em;
+  float u, v, metallic, roughness, occlusion, NoL;
+};
+
+OXC_DI PbrPixel pbr_prologue(const PbrParams& p, size_t pix, float depth, int x, int y) {
+  PbrPixel q;
+  q.u = fd(fa((float)x, 0.5f), (float)p.width); q.v = fd(fa((float)y, 0.5f), (float)p.height);
+  q.alb = __ldg(p.albedo + pix);
   const float4 nrm = __ldg(p.normal + pix);
   const PbrV3 mapped = pbr_oct_to_vec3(round_to_half(nrm.x), round_to_half(nrm.y));
-  const PbrV3 smooth = pbr_oct_to_vec3(round_to_half(nrm.z), round_to_half(nrm.w));
-  const float4 em = __ldg(p.emissive + pix);
+  q.smooth = pbr_oct_to_vec3(round_to_half(nrm.z), round_to_half(nrm.w));
+  q.em = __ldg(p.emissive + pix);
   const float4 mro = __ldg(p.mro + pix);
-  const float metallic = vmin(vmax(mro.x, 0.0f), 1.0f);
-  const float roughness = vmin(vmax(mro.y, 0.045f), 1.0f);
+  q.metallic = vmin(vmax(mro.x, 0.0f), 1.0f);
+  q.roughness = vmin(vmax(mro.y, 0.045f), 1.0f);
   const float ssao = p.ao ? round_to_half(__ldg(p.ao + pix)) : 1.0f;
-  const float occlusion = fm(mro.z, ssao);
+  q.occlusion = fm(mro.z, ssao);
   // world position :56-58
-  const float nx = fs(fm(u, 2.0f), 1.0f), ny = fs(fm(v, 2.0f), 1.0f);
+  const float nx = fs(fm(q.u, 2.0f), 1.0f), ny = fs(fm(q.v, 2.0f), 1.0f);
   float h[4];
 #pragma unroll
   for (int i = 0; i < 4; i++) {
     const float4 r = p.inv_pv_row[i];
     h[i] = fa(fa(fa(fm(r.x, nx), fm(r.y, ny)), fm(r.z, depth)), fm(r.w, 1.0f));
   }
-  const PbrV3 world = v3(fd(h[0], h[3]), fd(h[1], h[3]), fd(h[2], h[3]));
+  q.world = v3(fd(h[0], h[3]), fd(h[1], h[3]), fd(h[2], h[3]));
   // :63-67
-  PbrSurface s;
-  s.V = pbr_normalize(v3(fs(p.cam_pos[0], world.x), fs(p.cam_pos[1], world.y), fs(p.cam_pos[2], world.z)));
-  s.N = pbr_normalize(mapped);
-  const PbrV3 I = v3(-s.V.x, -s.V.y, -s.V.z);
-  const float dIN = pbr_dot(I, s.N);
-  const PbrV3 R = v3(fs(I.x, fm(fm(2.0f, s.N.x), dIN)), fs(I.y, fm(fm(2.0f, s.N.y), dIN)), fs(I.z, fm(fm(2.0f, s.N.z), dIN)));
-  s.NoV = fa(fabsf(pbr_dot(s.N, s.V)), 1e-5f);
-  const PbrV3 Ls = v3(p.sun[0], p.sun[1], p.sun[2]);
-  const float NoL = vmax(pbr_dot(s.N, Ls), 0.0f);
-  if ((p.flags & PBR_FLAG_SKY) && depth == 0.0f)
-    return p.sky_has_texture ? make_float4(1.0f, 1.0f, 1.0f, 1.0f)
-                             : make_float4(pbr_store(p.sky_solid.x), pbr_store(p.sky_solid.y), pbr_store(p.sky_solid.z), pbr_store(p.sky_solid.w));
-  const bool has_dir = (p.flags & PBR_FLAG_DIRECTIONAL) != 0;
+  q.s.V = pbr_normalize(v3(fs(p.cam_pos[0], q.world.x), fs(p.cam_pos[1], q.world.y), fs(p.cam_pos[2], q.world.z)));
+  q.s.N = pbr_normalize(mapped);
+  const PbrV3 I = v3(-q.s.V.x, -q.s.V.y, -q.s.V.z);
+  const float dIN = pbr_dot(I, q.s.N);
+  q.R = v3(fs(I.x, fm(fm(2.0f, q.s.N.x), dIN)), fs(I.y, fm(fm(2.0f, q.s.N.y), dIN)), fs(I.z, fm(fm(2.0f, q.s.N.z), dIN)));
+  q.s.NoV = fa(fabsf(pbr_dot(q.s.N, q.s.V)), 1e-5f);
+  q.Ls = v3(p.sun[0], p.sun[1], p.sun[2]);
+  q.NoL = vmax(pbr_dot(q.s.N, q.Ls), 0.0f);
+  return q;
+}
+
+// directional_shadow * contact_shadow (pbr_apply_no_atmos.slang:73-75, pbr_apply.slang:85-87)
+OXC_DI float pbr_visibility(const PbrParams& p, size_t pix, bool has_dir) {
   const float dshadow = has_dir && p.shadow ? __ldg(p.shadow + pix) : 1.0f;
   const float cshadow = (p.flags & PBR_FLAG_CONTACT) ? __ldg(p.contact + pix) : 1.0f;
-  const float visibility = fm(dshadow, cshadow);
-  const float direct = has_dir ? p.sun_intensity : 0.0f;
-  const bool has_sky = (p.flags & PBR_FLAG_SKY) != 0;
-  const PbrV3 env = has_sky ? v3(p.sky_ambient[0], p.sky_ambient[1], p.sky_ambient[2]) : v3(p.base_ambient[0], p.base_ambient[1], p.base_ambient[2]);
+  return fm(dshadow, cshadow);
+}
+
+// what both variants compute after their sky terms (pbr_apply_no_atmos.slang:86-126, pbr_apply.slang:143-183), with the variant's
+// diffuse and specular sky and per-channel direct illuminance: the stored (((surface + lights) + indirect) + emission) [+ aerial], the
+// aerial perspective term added only where `aerial` is given
+OXC_DI float4 pbr_shade(const PbrParams& p, const PbrLight* lights, PbrPixel& q, const PbrV3& diffuse_sky, const PbrV3& specular_sky,
+                        const PbrV3& direct, float visibility, const PbrV3* aerial) {
+  PbrSurface& s = q.s;
+  const float4 alb = q.alb;
+  const float metallic = q.metallic, roughness = q.roughness, occlusion = q.occlusion;
   // :86-100
   s.albedo = v3(alb.x, alb.y, alb.z);
   s.metallic = metallic;
@@ -244,29 +258,51 @@ OXC_DI float4 pbr_pixel(const PbrParams& p, const PbrLight* lights, int x, int y
   const PbrV3 kD = v3(fm(one_m, fs(1.0f, kS.x)), fm(one_m, fs(1.0f, kS.y)), fm(one_m, fs(1.0f, kS.z)));
   // specular_occlusion_horizon :52-54
   const float spec_occ = pbr_sat(fa(fs(canonical_pow(fa(s.NoV, occlusion), canonical_pow(2.0f, fs(fm(-16.0f, roughness), 1.0f))), 1.0f), occlusion));
-  const PbrV3 indirect = v3(fa(fm(fm(fm(fm(kD.x, env.x), alb.x), PBR_INV_PI), occlusion), fm(fm(kS.x, env.x), spec_occ)),
-                            fa(fm(fm(fm(fm(kD.y, env.y), alb.y), PBR_INV_PI), occlusion), fm(fm(kS.y, env.y), spec_occ)),
-                            fa(fm(fm(fm(fm(kD.z, env.z), alb.z), PBR_INV_PI), occlusion), fm(fm(kS.z, env.z), spec_occ)));
+  const PbrV3 indirect = v3(fa(fm(fm(fm(fm(kD.x, diffuse_sky.x), alb.x), PBR_INV_PI), occlusion), fm(fm(kS.x, specular_sky.x), spec_occ)),
+                            fa(fm(fm(fm(fm(kD.y, diffuse_sky.y), alb.y), PBR_INV_PI), occlusion), fm(fm(kS.y, specular_sky.y), spec_occ)),
+                            fa(fm(fm(fm(fm(kD.z, diffuse_sky.z), alb.z), PBR_INV_PI), occlusion), fm(fm(kS.z, specular_sky.z), spec_occ)));
   // GGX_energy_compensation :46-50, which depends on no light
   const float Ess = pbr_sat(fa(ABx, ABy));
   const float one_ess = fs(1.0f, Ess), ess_den = vmax(Ess, 1e-4f);
   s.energy = v3(fa(1.0f, fd(fm(s.F0.x, one_ess), ess_den)), fa(1.0f, fd(fm(s.F0.y, one_ess), ess_den)), fa(1.0f, fd(fm(s.F0.z, one_ess), ess_den)));
   // :102-113
   PbrV3 total = v3(0.0f, 0.0f, 0.0f);
-  for (uint32_t i = 0; i < p.light_count; i++) pbr_add_light(s, world, lights[i], total);
+  for (uint32_t i = 0; i < p.light_count; i++) pbr_add_light(s, q.world, lights[i], total);
   // :115-123
-  float horizon = pbr_sat(fa(1.0f, fm(1.3f, pbr_dot(R, smooth))));
+  float horizon = pbr_sat(fa(1.0f, fm(1.3f, pbr_dot(q.R, q.smooth))));
   horizon = fm(horizon, horizon);
   PbrV3 surf = v3(0.0f, 0.0f, 0.0f);
-  if (NoL > 0.0f) {
+  if (q.NoL > 0.0f) {
     PbrV3 d, sp;
-    pbr_brdf(s, Ls, d, sp);
-    surf = v3(fm(fm(fm(fa(d.x, fm(sp.x, horizon)), direct), NoL), visibility), fm(fm(fm(fa(d.y, fm(sp.y, horizon)), direct), NoL), visibility),
-              fm(fm(fm(fa(d.z, fm(sp.z, horizon)), direct), NoL), visibility));
+    pbr_brdf(s, q.Ls, d, sp);
+    surf = v3(fm(fm(fm(fa(d.x, fm(sp.x, horizon)), direct.x), q.NoL), visibility), fm(fm(fm(fa(d.y, fm(sp.y, horizon)), direct.y), q.NoL), visibility),
+              fm(fm(fm(fa(d.z, fm(sp.z, horizon)), direct.z), q.NoL), visibility));
   }
   // :125-126
+  const float4 em = q.em;
+  if (aerial)
+    return make_float4(pbr_store(fa(fa(fa(fa(surf.x, total.x), indirect.x), em.x), aerial->x)),
+                       pbr_store(fa(fa(fa(fa(surf.y, total.y), indirect.y), em.y), aerial->y)),
+                       pbr_store(fa(fa(fa(fa(surf.z, total.z), indirect.z), em.z), aerial->z)), 1.0f);
   return make_float4(pbr_store(fa(fa(fa(surf.x, total.x), indirect.x), em.x)), pbr_store(fa(fa(fa(surf.y, total.y), indirect.y), em.y)),
                      pbr_store(fa(fa(fa(surf.z, total.z), indirect.z), em.z)), 1.0f);
+}
+
+// fs_main (pbr_apply_no_atmos.slang:23-127) of pixel (x, y) with the staged lights
+OXC_DI float4 pbr_pixel(const PbrParams& p, const PbrLight* lights, int x, int y) {
+  const size_t pix = (size_t)y * p.width + x;
+  const float depth = p.depth[pix];
+  if ((p.flags & PBR_FLAG_TRANSPARENT) && depth == 0.0f) return make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  PbrPixel q = pbr_prologue(p, pix, depth, x, y);
+  if ((p.flags & PBR_FLAG_SKY) && depth == 0.0f)
+    return p.sky_has_texture ? make_float4(1.0f, 1.0f, 1.0f, 1.0f)
+                             : make_float4(pbr_store(p.sky_solid.x), pbr_store(p.sky_solid.y), pbr_store(p.sky_solid.z), pbr_store(p.sky_solid.w));
+  const bool has_dir = (p.flags & PBR_FLAG_DIRECTIONAL) != 0;
+  const float visibility = pbr_visibility(p, pix, has_dir);
+  const float direct = has_dir ? p.sun_intensity : 0.0f;
+  const bool has_sky = (p.flags & PBR_FLAG_SKY) != 0;
+  const PbrV3 env = has_sky ? v3(p.sky_ambient[0], p.sky_ambient[1], p.sky_ambient[2]) : v3(p.base_ambient[0], p.base_ambient[1], p.base_ambient[2]);
+  return pbr_shade(p, lights, q, env, env, v3(direct, direct, direct), visibility, nullptr);
 }
 
 } // namespace oxc

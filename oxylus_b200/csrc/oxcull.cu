@@ -30,6 +30,7 @@
 #include "kernels_contact_shadows.cuh"
 #include "kernels_atmosphere.cuh"
 #include "kernels_sky_ibl.cuh"
+#include "kernels_pbr_atmosphere.cuh"
 
 using namespace oxc;
 
@@ -1500,24 +1501,32 @@ int oxc_generate_ambient_occlusion(OxcContext* c, const OxcGtaoCamera* cam, cons
   return OXC_OK;
 }
 
-int oxc_apply_pbr(OxcContext* c, const OxcPbrCamera* cam, const OxcPbrSettings* st, const OxcLight* lights_dev, const OxcPbrInputs* in,
-                  uint32_t w, uint32_t h, float* out_dev, void* stream) {
-  if (!c || !cam || !st || !in || !out_dev) return fail(OXC_E_INVALID, "null argument");
-  if (!in->depth || !in->albedo || !in->normal || !in->emissive || !in->metallic_roughness_occlusion) return fail(OXC_E_INVALID, "null input plane");
-  if (st->light_count > OXC_MAX_LIGHTS) return fail(OXC_E_INVALID, "light_count %u above %u", st->light_count, OXC_MAX_LIGHTS);
-  if (st->light_count > 0 && !lights_dev) return fail(OXC_E_INVALID, "null lights with light_count %u", st->light_count);
-  if (st->scene_flags & OXC_SCENE_HAS_ATMOSPHERE) return fail(OXC_E_INVALID, "HasAtmosphere: the atmosphere variant is not available");
-  if ((st->scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS) && !in->contact_shadow)
+// what oxc_apply_pbr and oxc_apply_pbr_atmosphere both refuse: the planes, lights, extent and alignment: the planes, lights, extent and alignment
+static int pbr_check_inputs(const OxcPbrSettings& st, const OxcLight* lights_dev, const OxcPbrInputs& in, uint32_t w, uint32_t h,
+                            const float* out_dev) {
+  if (!in.depth || !in.albedo || !in.normal || !in.emissive || !in.metallic_roughness_occlusion) return fail(OXC_E_INVALID, "null input plane");
+  if (st.light_count > OXC_MAX_LIGHTS) return fail(OXC_E_INVALID, "light_count %u above %u", st.light_count, OXC_MAX_LIGHTS);
+  if (st.light_count > 0 && !lights_dev) return fail(OXC_E_INVALID, "null lights with light_count %u", st.light_count);
+  if ((st.scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS) && !in.contact_shadow)
     return fail(OXC_E_INVALID, "null contact_shadow plane under HasContactShadows");
   if (w == 0 || h == 0) return fail(OXC_E_INVALID, "empty extent %u x %u", w, h);
   if (w > 32768u || h > 32768u) return fail(OXC_E_INVALID, "extent %u x %u above 32768", w, h);
-  if ((reinterpret_cast<uintptr_t>(in->albedo) | reinterpret_cast<uintptr_t>(in->normal) | reinterpret_cast<uintptr_t>(in->emissive) |
-       reinterpret_cast<uintptr_t>(in->metallic_roughness_occlusion) | reinterpret_cast<uintptr_t>(out_dev) |
+  if ((reinterpret_cast<uintptr_t>(in.albedo) | reinterpret_cast<uintptr_t>(in.normal) | reinterpret_cast<uintptr_t>(in.emissive) |
+       reinterpret_cast<uintptr_t>(in.metallic_roughness_occlusion) | reinterpret_cast<uintptr_t>(out_dev) |
        reinterpret_cast<uintptr_t>(lights_dev)) & 15u)
     return fail(OXC_E_INVALID, "float4 planes, out_dev and lights_dev must be 16-byte aligned");
-  if ((reinterpret_cast<uintptr_t>(in->depth) | reinterpret_cast<uintptr_t>(in->ambient_occlusion) | reinterpret_cast<uintptr_t>(in->shadow) |
-       reinterpret_cast<uintptr_t>(in->contact_shadow)) & 3u)
+  if ((reinterpret_cast<uintptr_t>(in.depth) | reinterpret_cast<uintptr_t>(in.ambient_occlusion) | reinterpret_cast<uintptr_t>(in.shadow) |
+       reinterpret_cast<uintptr_t>(in.contact_shadow)) & 3u)
     return fail(OXC_E_INVALID, "depth, ambient_occlusion, shadow and contact_shadow must be 4-byte aligned");
+  return OXC_OK;
+}
+
+int oxc_apply_pbr(OxcContext* c, const OxcPbrCamera* cam, const OxcPbrSettings* st, const OxcLight* lights_dev, const OxcPbrInputs* in,
+                  uint32_t w, uint32_t h, float* out_dev, void* stream) {
+  if (!c || !cam || !st || !in || !out_dev) return fail(OXC_E_INVALID, "null argument");
+  if (st->scene_flags & OXC_SCENE_HAS_ATMOSPHERE) return fail(OXC_E_INVALID, "HasAtmosphere: the atmosphere variant is oxc_apply_pbr_atmosphere");
+  int rc;
+  if ((rc = pbr_check_inputs(*st, lights_dev, *in, w, h, out_dev)) != OXC_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
   const PbrParams p = pbr_make_params(*cam, *st, lights_dev, *in, w, h, out_dev);
@@ -1623,6 +1632,27 @@ int oxc_atmosphere_sky_ibl(OxcContext* c, const OxcAtmosphere* atmosphere, const
   const SkyIblParams p = sky_ibl_make_params(a, *camera, sun_direction, sun_intensity, sun_ambient_strength, frame_index, transmittance_dev,
                                              sky_view_dev, cube_dev);
   k_atmosphere_sky_ibl<<<SKY_IBL_BLOCKS, SKY_IBL_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_apply_pbr_atmosphere(OxcContext* c, const OxcPbrCamera* cam, const OxcPbrSettings* st, const OxcAtmosphere* atmosphere,
+                             const OxcLight* lights_dev, const OxcPbrInputs* in, const OxcPbrSky* sky, uint32_t w, uint32_t h, float* out_dev,
+                             void* stream) {
+  if (!c || !cam || !st || !atmosphere || !in || !sky || !out_dev) return fail(OXC_E_INVALID, "null argument");
+  if (!(st->scene_flags & OXC_SCENE_HAS_ATMOSPHERE)) return fail(OXC_E_INVALID, "settings without HasAtmosphere: oxc_apply_pbr draws them");
+  int rc;
+  if ((rc = pbr_check_inputs(*st, lights_dev, *in, w, h, out_dev)) != OXC_OK) return rc;
+  if (!sky->transmittance || !sky->sky_view || !sky->aerial_perspective || !sky->sky_cube) return fail(OXC_E_INVALID, "null sky plane");
+  if ((reinterpret_cast<uintptr_t>(sky->transmittance) | reinterpret_cast<uintptr_t>(sky->sky_view) |
+       reinterpret_cast<uintptr_t>(sky->aerial_perspective) | reinterpret_cast<uintptr_t>(sky->sky_cube)) & 7u)
+    return fail(OXC_E_INVALID, "sky planes must be 8-byte aligned");
+  if ((rc = atmosphere_check_sizes(*atmosphere, true, true)) != OXC_OK) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  const PbrAtmParams p = pbr_atmosphere_make_params(*cam, *st, *atmosphere, lights_dev, *in, *sky, w, h, out_dev);
+  const dim3 grid((w + PBR_TILE_X - 1) / PBR_TILE_X, (h + PBR_TILE_Y - 1) / PBR_TILE_Y);
+  k_apply_pbr_atmosphere<<<grid, PBR_THREADS, 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }
