@@ -988,7 +988,7 @@ int oxc_apply_pbr(OxcContext* ctx, const OxcPbrCamera* camera, const OxcPbrSetti
  *      penetration = 1 / p.z - min(lin, unf).  The first step with distance < 0 is the candidate; the pixel is in contact when
  *      penetration < depth_thickness and distance < depth_thickness, and then shadow = smoothstep(1, 0.3, penetration /
  *      depth_thickness); otherwise shadow = 0.
- *   5. nearest tap at uv: texel (floor(u * W), floor(v * H)) with NaN-safe saturating indices (oxc_alpha.cuh alpha_f2i), clamped to
+ *   5. nearest tap at uv: texel (floor(u * W), floor(v * H)) with NaN-safe saturating indices (oxc_shader_math.cuh sat_i32), clamped to
  *      the edge.  Bilinear tap at uv: x = u * W - 0.5, x0 = floor(x), wx = x - x0 (y likewise), texels x0, x0 + 1 / y0, y0 + 1 with the
  *      same index rule, top = a00 + wx * (a10 - a00), bottom = a01 + wx * (a11 - a01), top + wy * (bottom - top): the GTAO's level tap
  *      (oxc_generate_ambient_occlusion item 6).  Deviation: no 8-bit quantisation of the weights, as the alpha test's.

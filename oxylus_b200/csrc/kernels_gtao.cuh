@@ -22,15 +22,15 @@ __global__ void __launch_bounds__(GTAO_PREFILTER_SIDE * GTAO_PREFILTER_SIDE) k_g
   const float d01 = gtao_level0(p, x0, y0 + 1), d11 = gtao_level0(p, x0 + 1, y0 + 1);
   const int W = p.width, H = p.height;
   if (y0 < H) {
-    if (x0 < W) p.mips[(size_t)y0 * W + x0] = gtao_mip_store(d00);
-    if (x0 + 1 < W) p.mips[(size_t)y0 * W + x0 + 1] = gtao_mip_store(d10);
+    if (x0 < W) p.mips[(size_t)y0 * W + x0] = nan_canonical(d00);
+    if (x0 + 1 < W) p.mips[(size_t)y0 * W + x0 + 1] = nan_canonical(d10);
   }
   if (y0 + 1 < H) {
-    if (x0 < W) p.mips[(size_t)(y0 + 1) * W + x0] = gtao_mip_store(d01);
-    if (x0 + 1 < W) p.mips[(size_t)(y0 + 1) * W + x0 + 1] = gtao_mip_store(d11);
+    if (x0 < W) p.mips[(size_t)(y0 + 1) * W + x0] = nan_canonical(d01);
+    if (x0 + 1 < W) p.mips[(size_t)(y0 + 1) * W + x0 + 1] = nan_canonical(d11);
   }
   float d = gtao_weighted_average(d00, d10, d01, d11);
-  if (bx < p.mip_w[1] && by < p.mip_h[1]) p.mips[p.mip_off[1] + (size_t)by * p.mip_w[1] + bx] = gtao_mip_store(d);
+  if (bx < p.mip_w[1] && by < p.mip_h[1]) p.mips[p.mip_off[1] + (size_t)by * p.mip_w[1] + bx] = nan_canonical(d);
   prev[lx][ly] = d;
 #pragma unroll
   for (int k = 2; k < GTAO_LEVELS; k++) {
@@ -41,7 +41,7 @@ __global__ void __launch_bounds__(GTAO_PREFILTER_SIDE * GTAO_PREFILTER_SIDE) k_g
     if ((lx & (2 * step - 1)) == 0 && (ly & (2 * step - 1)) == 0) {
       d = gtao_weighted_average(d, prev[lx + step][ly], prev[lx][ly + step], prev[lx + step][ly + step]);
       const int tx = bx >> (k - 1), ty = by >> (k - 1);
-      if (tx < p.mip_w[k] && ty < p.mip_h[k]) p.mips[p.mip_off[k] + (size_t)ty * p.mip_w[k] + tx] = gtao_mip_store(d);
+      if (tx < p.mip_w[k] && ty < p.mip_h[k]) p.mips[p.mip_off[k] + (size_t)ty * p.mip_w[k] + tx] = nan_canonical(d);
       prev[lx][ly] = d;
     }
   }
@@ -60,7 +60,7 @@ __global__ void __launch_bounds__(GTAO_THREADS) k_gtao_main(const __grid_constan
   float centre;
   const size_t pix = (size_t)y * p.width + x;
   p.edges[pix] = gtao_edges(p, x, y, &centre);
-  p.noisy[pix] = gtao_half_bits(gtao_occlusion(p, x, y, centre));
+  p.noisy[pix] = half_bits(gtao_occlusion(p, x, y, centre));
 }
 
 __global__ void __launch_bounds__(GTAO_THREADS) k_gtao_denoise(const __grid_constant__ GtaoParams p) {

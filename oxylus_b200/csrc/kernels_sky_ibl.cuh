@@ -20,15 +20,15 @@ __global__ void __launch_bounds__(SKY_IBL_THREADS) k_atmosphere_sky_ibl(const __
   const int texel = (int)blockIdx.x * SKY_IBL_TEXELS_PER_CTA + (int)threadIdx.x / SKY_IBL_SAMPLES;
   const int face = texel / (SKY_IBL_RES * SKY_IBL_RES), y = texel / SKY_IBL_RES % SKY_IBL_RES, x = texel % SKY_IBL_RES;
   const SkyIblTexel t = sky_ibl_texel(p, face, x, y); // reads the history before the first thread of the texel overwrites it
-  const AtmV3 s = sky_ibl_sample(p, t, i);
+  const Vec3 s = sky_ibl_sample(p, t, i);
   s_sample[0][threadIdx.x] = s.x;
   s_sample[1][threadIdx.x] = s.y;
   s_sample[2][threadIdx.x] = s.z;
   __syncthreads();
   if (i != 0) return;
-  AtmV3 sum = atm_v3(0.0f, 0.0f, 0.0f);
+  Vec3 sum = vec3(0.0f, 0.0f, 0.0f);
   for (int k = 0; k < SKY_IBL_SAMPLES; k++)
-    sum = atm_add(sum, atm_v3(s_sample[0][threadIdx.x + k], s_sample[1][threadIdx.x + k], s_sample[2][threadIdx.x + k]));
+    sum = vadd(sum, vec3(s_sample[0][threadIdx.x + k], s_sample[1][threadIdx.x + k], s_sample[2][threadIdx.x + k]));
   sky_ibl_finish(p, t, face, x, y, sum);
 }
 

@@ -5,9 +5,7 @@
 // Specification: include/oxcull.h (comment above OxcMaterial) == oracle/oxc_oracle.c (comment above raster_triangle),
 // operation for operation.
 #pragma once
-#include <climits>
-
-#include "oxc_exact.cuh"
+#include "oxc_shader_math.cuh"
 
 namespace oxc {
 
@@ -37,11 +35,6 @@ OXC_DI void alpha_tri_setup(const float4 c0, const float4 c1, const float4 c2, f
   t.rw[0] = fd(1.0f, c0.w); t.rw[1] = fd(1.0f, c2.w); t.rw[2] = fd(1.0f, c1.w); // the rw of to_screen (raster spec step 3)
   t.u[0] = u0; t.u[1] = u2; t.u[2] = u1;
   t.v[0] = v0; t.v[1] = v2; t.v[2] = v1;
-}
-
-// float -> int, NaN -> 0, saturating (the host build and the device agree for every input)
-OXC_DI int alpha_f2i(float f) {
-  return !(f == f) ? 0 : (f >= 2147483648.0f ? INT_MAX : (f <= -2147483648.0f ? INT_MIN : (int)f));
 }
 
 OXC_DI uint32_t alpha_wrap(long long i, uint32_t n, uint32_t mode) {
@@ -74,13 +67,13 @@ OXC_DI float alpha_sample_level(const AlphaMaterial& m, uint32_t level, uint32_t
   }
   const float fw = (float)w, fh = (float)h;
   if (filter == OXC_FILTER_NEAREST) {
-    const int ix = alpha_f2i(floorf(fm(u, fw))), iy = alpha_f2i(floorf(fm(v, fh)));
+    const int ix = sat_i32(floorf(fm(u, fw))), iy = sat_i32(floorf(fm(v, fh)));
     return alpha_texel(m, base, w, alpha_wrap(ix, w, m.address_u), alpha_wrap(iy, h, m.address_v));
   }
   const float x = fs(fm(u, fw), 0.5f), y = fs(fm(v, fh), 0.5f);
   const float x0 = floorf(x), y0 = floorf(y);
   const float wx = fs(x, x0), wy = fs(y, y0);
-  const int ix = alpha_f2i(x0), iy = alpha_f2i(y0);
+  const int ix = sat_i32(x0), iy = sat_i32(y0);
   const uint32_t xa = alpha_wrap(ix, w, m.address_u), xb = alpha_wrap((long long)ix + 1, w, m.address_u);
   const uint32_t ya = alpha_wrap(iy, h, m.address_v), yb = alpha_wrap((long long)iy + 1, h, m.address_v);
   const float a00 = alpha_texel(m, base, w, xa, ya), a10 = alpha_texel(m, base, w, xb, ya), a01 = alpha_texel(m, base, w, xa, yb),
@@ -97,11 +90,6 @@ OXC_DI void alpha_interpolate(const AlphaTri& t, long long e0, long long e1, lon
   const float l0 = fm(p0, inv), l1 = fm(p1, inv), l2 = fm(p2, inv);
   u = fa(fa(fm(l0, t.u[0]), fm(l1, t.u[1])), fm(l2, t.u[2]));
   v = fa(fa(fm(l0, t.v[0]), fm(l1, t.v[1])), fm(l2, t.v[2]));
-}
-
-OXC_DI float lerp_levels(float f, float lo, float hi) { return fa(fm(fs(1.0f, f), lo), fm(f, hi)); }
-OXC_DI float4 lerp_levels(float f, float4 lo, float4 hi) {
-  return make_float4(lerp_levels(f, lo.x, hi.x), lerp_levels(f, lo.y, hi.y), lerp_levels(f, lo.z, hi.z), lerp_levels(f, lo.w, hi.w));
 }
 
 // SampleGrad's level rule (oracle spec 4) from the texel-space derivatives mx = ddx(u) * width0, my = ddx(v) * height0, nx / ny

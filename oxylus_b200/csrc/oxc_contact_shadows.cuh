@@ -5,7 +5,7 @@
 // No warp intrinsics, no shared memory: tests compile this source for the host.
 // Specification: include/oxcull.h (comment above oxc_contact_shadows) == oracle/oxc_oracle_contact_shadows.c, operation for operation.
 #pragma once
-#include "oxc_gtao.cuh" // alpha_f2i, gtao_clamp
+#include "oxc_shader_math.cuh"
 
 namespace oxc {
 
@@ -53,8 +53,6 @@ OXC_DI ContactShadowConstants cs_constants(const ContactShadowParams& p) {
   return c;
 }
 
-OXC_DI float cs_sign(float x) { return x > 0.0f ? 1.0f : (x < 0.0f ? -1.0f : 0.0f); }
-OXC_DI uint32_t cs_u32(float f) { return !(f > 0.0f) ? 0u : (f >= 4294967296.0f ? 0xFFFFFFFFu : (uint32_t)f); }
 OXC_DI float cs_to_uv(float c) { return fa(fm(c, 0.5f), 0.5f); } // raymarch.slang:15-17
 
 // SampleLevel(linear_clamp, uv, 0) of the depth plane, in two parts so that the nearest tap can pick among the four texels: the
@@ -69,8 +67,8 @@ OXC_DI BilinearTap cs_bilinear_tap(int w, int h, float u, float v) {
   const float x0 = floorf(x), y0 = floorf(y);
   BilinearTap t;
   t.wx = fs(x, x0); t.wy = fs(y, y0);
-  const long long ix = alpha_f2i(x0), iy = alpha_f2i(y0);
-  t.xa = gtao_clamp(ix, w); t.xb = gtao_clamp(ix + 1, w); t.ya = gtao_clamp(iy, h); t.yb = gtao_clamp(iy + 1, h);
+  const long long ix = sat_i32(x0), iy = sat_i32(y0);
+  t.xa = clamp_index(ix, w); t.xb = clamp_index(ix + 1, w); t.ya = clamp_index(iy, h); t.yb = clamp_index(iy + 1, h);
   return t;
 }
 OXC_DI float cs_bilinear_blend(const BilinearTap& t, float a00, float a10, float a01, float a11) {
@@ -79,7 +77,7 @@ OXC_DI float cs_bilinear_blend(const BilinearTap& t, float a00, float a10, float
 }
 
 // SampleLevel(nearest_clamp, uv, 0): texel column floor(u * W) (row likewise), NaN-safe saturating, clamped to the edge
-OXC_DI int cs_nearest_index(float u, int n) { return gtao_clamp(alpha_f2i(floorf(fm(u, (float)n))), n); }
+OXC_DI int cs_nearest_index(float u, int n) { return clamp_index(sat_i32(floorf(fm(u, (float)n))), n); }
 
 // DepthRaymarchDistanceFn::call (raymarch.slang:254-322): the bilinear and the nearest tap at the point's uv.  The nearest texel is
 // always one of the bilinear tap's four: with a = fl(u * W), x = fl(a - 0.5) is a - 0.5 exactly below 2^23 and a or a - 1 above, so
@@ -118,7 +116,7 @@ OXC_DI float cs_pixel(const ContactShadowParams& p, const ContactShadowConstants
   for (int i = 0; i < 4; i++) pp[i] = row_dot4(p.proj_row[i], pv[0], pv[1], pv[2], pv[3]);
   const float end_cs[3] = {fd(pp[0], pp[3]), fd(pp[1], pp[3]), fd(pp[2], pp[3])};
   // :542-546 to_cs, :502-537 to_cs_dir_impl(dir, false)
-  const float s = cs_sign(end_cs[2]);
+  const float s = sign(end_cs[2]);
   float e[4] = {fa(cs[0], fm(fs(end_cs[0], cs[0]), s)), fa(cs[1], fm(fs(end_cs[1], cs[1]), s)), fa(cs[2], fm(fs(end_cs[2], cs[2]), s)),
                 fa(1.0f, fm(0.0f, s))};
   const float den = fm(e[3] >= 0.0f ? 1.0f : -1.0f, vmax(1e-10f, fabsf(e[3])));
@@ -143,7 +141,7 @@ OXC_DI float cs_pixel(const ContactShadowParams& p, const ContactShadowConstants
   // :588-595 the step count
   const float su = cs_to_uv(cs[0]), sv = cs_to_uv(cs[1]);
   const float lx = fm(fs(cs_to_uv(fa(cs[0], fm(delta[0], m))), su), fw), ly = fm(fs(cs_to_uv(fa(cs[1], fm(delta[1], m))), sv), fh);
-  const uint32_t len = cs_u32(floorf(fd(fsq(fa(fm(lx, lx), fm(ly, ly))), 1.0f)));
+  const uint32_t len = sat_u32(floorf(fd(fsq(fa(fm(lx, lx), fm(ly, ly))), 1.0f)));
   const uint32_t m_steps = p.steps < len ? p.steps : len;
   const uint32_t n = m_steps > 2u ? m_steps : 2u;
   // :104-175 the linear search, t = lerp(0, 1, pow((step + 1) / n, 1)) = (step + 1) / n
@@ -158,7 +156,7 @@ OXC_DI float cs_pixel(const ContactShadowParams& p, const ContactShadowConstants
   float shadow = 0.0f;
   if (hit && penetration < c.depth_thickness && distance < c.depth_thickness) {
     // smoothstep(1.0, 0.3, penetration / depth_thickness)
-    const float ts = vmin(vmax(fd(fs(fd(penetration, c.depth_thickness), 1.0f), fs(0.3f, 1.0f)), 0.0f), 1.0f);
+    const float ts = saturate(fd(fs(fd(penetration, c.depth_thickness), 1.0f), fs(0.3f, 1.0f)));
     shadow = fm(fm(ts, ts), fs(3.0f, fm(2.0f, ts)));
   }
   return fs(1.0f, shadow);

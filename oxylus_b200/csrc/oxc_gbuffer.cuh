@@ -9,7 +9,7 @@
 #include <string>
 #include <vector>
 
-#include "oxc_alpha.cuh" // alpha_wrap, alpha_f2i, sample_grad_levels
+#include "oxc_alpha.cuh"
 
 namespace oxc {
 
@@ -116,13 +116,13 @@ OXC_DI float4 gb_sample_level(const GBufImage& im, uint32_t address_u, uint32_t 
   }
   const float fw = (float)w, fh = (float)h;
   if (filter == OXC_FILTER_NEAREST) {
-    const int ix = alpha_f2i(floorf(fm(u, fw))), iy = alpha_f2i(floorf(fm(v, fh)));
+    const int ix = sat_i32(floorf(fm(u, fw))), iy = sat_i32(floorf(fm(v, fh)));
     return gb_texel(im.format, base, w, alpha_wrap(ix, w, address_u), alpha_wrap(iy, h, address_v));
   }
   const float x = fs(fm(u, fw), 0.5f), y = fs(fm(v, fh), 0.5f);
   const float x0 = floorf(x), y0 = floorf(y);
   const float wx = fs(x, x0), wy = fs(y, y0);
-  const int ix = alpha_f2i(x0), iy = alpha_f2i(y0);
+  const int ix = sat_i32(x0), iy = sat_i32(y0);
   const uint32_t xa = alpha_wrap(ix, w, address_u), xb = alpha_wrap((long long)ix + 1, w, address_u);
   const uint32_t ya = alpha_wrap(iy, h, address_v), yb = alpha_wrap((long long)iy + 1, h, address_v);
   const float4 a00 = gb_texel(im.format, base, w, xa, ya), a10 = gb_texel(im.format, base, w, xb, ya), a01 = gb_texel(im.format, base, w, xa, yb),
@@ -151,9 +151,6 @@ OXC_DI void vec3_to_oct(float vx, float vy, float vz, float& ex, float& ey) {
     ex = ox; ey = oy;
   }
 }
-
-// sign() of HLSL as a float, NaN -> 0
-OXC_DI float gb_sign(float x) { return x > 0.0f ? 1.0f : (x < 0.0f ? -1.0f : 0.0f); }
 
 // What the decode's geometry half hands the material evaluation for one decoded pixel.
 struct GBufferPixel {
@@ -192,7 +189,7 @@ OXC_DI void gbuffer_shade(const GBufMaterial& m, const GBufImage* images /* this
     const float dx_n = dot3(pdx[0], pdx[1], pdx[2], nx, ny, nz), dy_n = dot3(pdy[0], pdy[1], pdy[2], nx, ny, nz);
     const float sx[3] = {fs(pdx[0], fm(dx_n, nx)), fs(pdx[1], fm(dx_n, ny)), fs(pdx[2], fm(dx_n, nz))};
     const float sy[3] = {fs(pdy[0], fm(dy_n, nx)), fs(pdy[1], fm(dy_n, ny)), fs(pdy[2], fm(dy_n, nz))};
-    const float js = gb_sign(fs(fm(dxu, dyv), fm(dxv, dyu)));
+    const float js = sign(fs(fm(dxu, dyv), fm(dxv, dyu)));
     float tx = fm(js, fs(fm(dyv, sx[0]), fm(dxv, sy[0]))), ty = fm(js, fs(fm(dyv, sx[1]), fm(dxv, sy[1]))),
           tz = fm(js, fs(fm(dyv, sx[2]), fm(dxv, sy[2])));
     if (js != 0.0f) {
@@ -201,7 +198,7 @@ OXC_DI void gbuffer_shade(const GBufMaterial& m, const GBufImage* images /* this
     }
     // cross(n, pos_ddx), then w = js * sign(dot(pos_ddy, .))
     const float cx = fs(fm(ny, pdx[2]), fm(nz, pdx[1])), cy = fs(fm(nz, pdx[0]), fm(nx, pdx[2])), cz = fs(fm(nx, pdx[1]), fm(ny, pdx[0]));
-    const float nw = -fm(js, gb_sign(dot3(pdy[0], pdy[1], pdy[2], cx, cy, cz)));
+    const float nw = -fm(js, sign(dot3(pdy[0], pdy[1], pdy[2], cx, cy, cz)));
     const float bx = fm(nw, fs(fm(ny, tz), fm(nz, ty))), by = fm(nw, fs(fm(nz, tx), fm(nx, tz))), bz = fm(nw, fs(fm(nx, ty), fm(ny, tx)));
     float ox = nx, oy = ny, oz = nz;
     if (m.flags & OXC_MATERIAL_HAS_NORMAL_IMAGE) {

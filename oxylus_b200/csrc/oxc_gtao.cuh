@@ -4,15 +4,13 @@
 // No warp intrinsics, no shared memory: tests compile this source for the host.
 // Specification: include/oxcull.h (comment above oxc_generate_ambient_occlusion) == oracle/oxc_oracle_gtao.c, operation for operation.
 #pragma once
-#include "oxc_alpha.cuh"
-#include "oxc_vsm_resolve.cuh"
+#include "oxc_shader_math.cuh"
 
 namespace oxc {
 
 constexpr int GTAO_LEVELS = 5;                 // vbgtao_main.slang:14
 constexpr uint32_t GTAO_SECTORS = 32u;         // :12
 constexpr float GTAO_HALF_PI = 1.57079632679f; // common/math.slang:3-4
-constexpr float GTAO_PI = 3.1415926535897932384626433832795f;
 
 struct GtaoParams {
   const float* depth;
@@ -59,10 +57,6 @@ __host__ inline GtaoParams gtao_make_params(const OxcGtaoCamera& cam, const OxcG
   return p;
 }
 
-OXC_DI float gtao_sat(float x) { return vmin(vmax(x, 0.0f), 1.0f); }
-OXC_DI float gtao_sign(float x) { return x > 0.0f ? 1.0f : (x < 0.0f ? -1.0f : 0.0f); }
-OXC_DI uint32_t gtao_u32(float f) { return !(f > 0.0f) ? 0u : (f >= 4294967296.0f ? 0xFFFFFFFFu : (uint32_t)f); }
-OXC_DI int gtao_clamp(long long i, int n) { return (int)(i < 0 ? 0 : (i > n - 1 ? n - 1 : i)); }
 OXC_DI uint32_t gtao_popc(uint32_t v) {
 #ifdef __CUDA_ARCH__
   return (uint32_t)__popc(v);
@@ -70,21 +64,6 @@ OXC_DI uint32_t gtao_popc(uint32_t v) {
   return (uint32_t)__builtin_popcount(v);
 #endif
 }
-
-// binary32 -> binary16 bits, round to nearest even (the R16F noisy-occlusion store; the values stored are in [0, 1])
-OXC_DI uint16_t gtao_half_bits(float f) {
-#ifdef __CUDA_ARCH__
-  return __half_as_ushort(__float2half_rn(f));
-#else
-  const float r = round_to_half(f);
-  const uint32_t u = __float_as_uint(r), s = (u >> 16) & 0x8000u, a = u & 0x7FFFFFFFu;
-  if (a > 0x7F800000u) return (uint16_t)(s | 0x7FFFu);
-  if (a == 0x7F800000u) return (uint16_t)(s | 0x7C00u);
-  if (a >= 0x38800000u) return (uint16_t)(s | (((a >> 23) - 112u) << 10) | ((a >> 13) & 0x3FFu));
-  return (uint16_t)(s | (uint32_t)fm(__uint_as_float(a), 16777216.0f));
-#endif
-}
-OXC_DI float gtao_half_float(uint16_t h) { return __half2float(__ushort_as_half(h)); }
 
 // RendererInstance.cpp:151-170, the Hilbert index of (x, y) in the 64 x 64 noise table
 OXC_DI uint32_t gtao_hilbert_index(uint32_t px, uint32_t py) {
@@ -100,9 +79,6 @@ OXC_DI uint32_t gtao_hilbert_index(uint32_t px, uint32_t py) {
   return index;
 }
 
-// the value a mip texel is stored as: a NaN is written as 0x7FFFFFFF, the NaN the GPU's arithmetic produces (the host's differs)
-OXC_DI float gtao_mip_store(float v) { return v != v ? __uint_as_float(0x7FFFFFFFu) : v; }
-
 // vbgtao_prefilter.slang:19-21
 OXC_DI float gtao_linearize(const GtaoParams& p, float d) { return fd(p.m23, fa(d, p.m22)); }
 
@@ -114,8 +90,8 @@ OXC_DI float gtao_weighted_average(float d0, float d1, float d2, float d3) {
   const float falloff_mul = fd(-1.0f, falloff_range);
   const float falloff_add = fa(fd(falloff_from, falloff_range), 1.0f);
   const float mn = vmin(vmin(d0, d1), vmin(d2, d3));
-  const float w0 = gtao_sat(fa(fm(fs(d0, mn), falloff_mul), falloff_add)), w1 = gtao_sat(fa(fm(fs(d1, mn), falloff_mul), falloff_add));
-  const float w2 = gtao_sat(fa(fm(fs(d2, mn), falloff_mul), falloff_add)), w3 = gtao_sat(fa(fm(fs(d3, mn), falloff_mul), falloff_add));
+  const float w0 = saturate(fa(fm(fs(d0, mn), falloff_mul), falloff_add)), w1 = saturate(fa(fm(fs(d1, mn), falloff_mul), falloff_add));
+  const float w2 = saturate(fa(fm(fs(d2, mn), falloff_mul), falloff_add)), w3 = saturate(fa(fm(fs(d3, mn), falloff_mul), falloff_add));
   const float total = fa(fa(fa(w0, w1), w2), w3);
   return fd(fa(fa(fa(fm(w0, d0), fm(w1, d1)), fm(w2, d2)), fm(w3, d3)), total);
 }
@@ -144,8 +120,8 @@ OXC_DI float gtao_bilinear(const GtaoParams& p, int k, float u, float v) {
   const float x = fs(fm(u, (float)w), 0.5f), y = fs(fm(v, (float)h), 0.5f);
   const float x0 = floorf(x), y0 = floorf(y);
   const float wx = fs(x, x0), wy = fs(y, y0);
-  const long long ix = alpha_f2i(x0), iy = alpha_f2i(y0);
-  const int xa = gtao_clamp(ix, w), xb = gtao_clamp(ix + 1, w), ya = gtao_clamp(iy, h), yb = gtao_clamp(iy + 1, h);
+  const long long ix = sat_i32(x0), iy = sat_i32(y0);
+  const int xa = clamp_index(ix, w), xb = clamp_index(ix + 1, w), ya = clamp_index(iy, h), yb = clamp_index(iy + 1, h);
   const float a00 = __ldg(&lvl[(size_t)ya * w + xa]), a10 = __ldg(&lvl[(size_t)ya * w + xb]);
   const float a01 = __ldg(&lvl[(size_t)yb * w + xa]), a11 = __ldg(&lvl[(size_t)yb * w + xb]);
   const float top = fa(a00, fm(wx, fs(a10, a00))), bot = fa(a01, fm(wx, fs(a11, a01)));
@@ -164,15 +140,15 @@ OXC_DI float gtao_sample_level(const GtaoParams& p, float u, float v, float lamb
 OXC_DI float gtao_fast_acos(float in_x) {
   const float x = fabsf(in_x);
   float res = fa(fm(-0.156583f, x), GTAO_HALF_PI);
-  res = fm(res, fsq(gtao_sat(fs(1.0f, x))));
-  return in_x >= 0.0f ? res : fs(GTAO_PI, res);
+  res = fm(res, fsq(saturate(fs(1.0f, x))));
+  return in_x >= 0.0f ? res : fs(PI, res);
 }
 
 // :102-119
 OXC_DI uint32_t gtao_update_sectors(float min_h, float max_h, uint32_t bitmask) {
-  const uint32_t angle = gtao_u32(ceilf(fm(gtao_sat(fs(max_h, min_h)), (float)GTAO_SECTORS)));
+  const uint32_t angle = sat_u32(ceilf(fm(saturate(fs(max_h, min_h)), (float)GTAO_SECTORS)));
   if (angle == 0u) return bitmask;
-  uint32_t start = gtao_u32(fm(gtao_sat(min_h), (float)GTAO_SECTORS));
+  uint32_t start = sat_u32(fm(saturate(min_h), (float)GTAO_SECTORS));
   start = start < GTAO_SECTORS - 1u ? start : GTAO_SECTORS - 1u;
   return bitmask | ((0xFFFFFFFFu >> (GTAO_SECTORS - angle)) << start);
 }
@@ -189,8 +165,8 @@ OXC_DI uint32_t gtao_sector_mask(float thickness, float dx, float dy, float dz, 
   gtao_normalize(dx, dy, dz, ax, ay, az);
   gtao_normalize(bx, by, bz, cx, cy, cz);
   float h0 = gtao_fast_acos(dot3(ax, ay, az, vx, vy, vz)), h1 = gtao_fast_acos(dot3(cx, cy, cz, vx, vy, vz));
-  h0 = gtao_sat(fd(fa(fa(fm(sd, -h0), n), GTAO_HALF_PI), GTAO_PI));
-  h1 = gtao_sat(fd(fa(fa(fm(sd, -h1), n), GTAO_HALF_PI), GTAO_PI));
+  h0 = saturate(fd(fa(fa(fm(sd, -h0), n), GTAO_HALF_PI), PI));
+  h1 = saturate(fd(fa(fa(fm(sd, -h1), n), GTAO_HALF_PI), PI));
   return sd >= 0.0f ? gtao_update_sectors(h1, h0, 0u) : gtao_update_sectors(h0, h1, 0u);
 }
 
@@ -198,8 +174,8 @@ OXC_DI uint32_t gtao_sector_mask(float thickness, float dx, float dy, float dz, 
 OXC_DI void gtao_noise(uint32_t x, uint32_t y, uint32_t noise_index, float& n0, float& n1) {
   const uint32_t index = gtao_hilbert_index(x & 63u, y & 63u) + 288u * (noise_index & 63u);
   const float fi = (float)index;
-  n0 = vfract(fa(0.5f, fm(fi, 0.75487766624669276005f)));
-  n1 = vfract(fa(0.5f, fm(fi, 0.5698402909980532659114f)));
+  n0 = frac(fa(0.5f, fm(fi, 0.75487766624669276005f)));
+  n1 = frac(fa(0.5f, fm(fi, 0.5698402909980532659114f)));
 }
 
 // :69-100 calculate_edges: the packed edges of pixel (x, y); *centre receives its linear depth
@@ -207,8 +183,8 @@ OXC_DI uint32_t gtao_edges(const GtaoParams& p, int x, int y, float* centre) {
   const float* m0 = p.mips;
   const int W = p.width, H = p.height;
   const float c = __ldg(&m0[(size_t)y * W + x]);
-  const float l = __ldg(&m0[(size_t)y * W + gtao_clamp((long long)x - 1, W)]), r = __ldg(&m0[(size_t)y * W + gtao_clamp((long long)x + 1, W)]);
-  const float t = __ldg(&m0[(size_t)gtao_clamp((long long)y - 1, H) * W + x]), b = __ldg(&m0[(size_t)gtao_clamp((long long)y + 1, H) * W + x]);
+  const float l = __ldg(&m0[(size_t)y * W + clamp_index((long long)x - 1, W)]), r = __ldg(&m0[(size_t)y * W + clamp_index((long long)x + 1, W)]);
+  const float t = __ldg(&m0[(size_t)clamp_index((long long)y - 1, H) * W + x]), b = __ldg(&m0[(size_t)clamp_index((long long)y + 1, H) * W + x]);
   float e[4] = {fs(l, c), fs(r, c), fs(t, c), fs(b, c)};
   const float slr = fm(fs(e[1], e[0]), 0.5f), stb = fm(fs(e[3], e[2]), 0.5f);
   const float adj[4] = {fa(e[0], slr), fa(e[1], -slr), fa(e[2], stb), fa(e[3], -stb)};
@@ -216,8 +192,8 @@ OXC_DI uint32_t gtao_edges(const GtaoParams& p, int x, int y, float* centre) {
   uint32_t packed = 0;
 #pragma unroll
   for (int i = 0; i < 4; i++) {
-    const float v = gtao_sat(fs(1.25f, fd(vmin(fabsf(e[i]), fabsf(adj[i])), scale)));
-    packed |= (uint32_t)rintf(fm(gtao_sat(v), 255.0f)) << (8 * i);
+    const float v = saturate(fs(1.25f, fd(vmin(fabsf(e[i]), fabsf(adj[i])), scale)));
+    packed |= (uint32_t)rintf(fm(saturate(v), 255.0f)) << (8 * i);
   }
   *centre = c;
   return packed;
@@ -264,7 +240,7 @@ OXC_DI float gtao_occlusion(const GtaoParams& p, int x, int y, float ld) {
   const float min_s = fd(1.3f, vmax(fm(sr_u, rx), 1.3f));
   float visibility = 0.0f;
   for (float slice_t = 0.0f; slice_t < slice_count; slice_t = fa(slice_t, 1.0f)) {
-    const float phi = fm(fd(fa(slice_t, n0), slice_count), GTAO_PI);
+    const float phi = fm(fd(fa(slice_t, n0), slice_count), PI);
     float sn, cs;
     canonical_sincos(phi, sn, cs);
     const float dd = dot3(cs, sn, 0.0f, vx, vy, vz);
@@ -274,14 +250,14 @@ OXC_DI float gtao_occlusion(const GtaoParams& p, int x, int y, float ld) {
     const float na = dot3(nx, ny, nz, axx, axy, axz);
     const float pnx = fs(nx, fm(axx, na)), pny = fs(ny, fm(axy, na)), pnz = fs(nz, fm(axz, na));
     const float pnl = vmax(length3(pnx, pny, pnz), 1e-6f);
-    const float sign_norm = gtao_sign(dot3(odx, ody, odz, pnx, pny, pnz));
-    const float cos_norm = gtao_sat(fd(dot3(pnx, pny, pnz, vx, vy, vz), pnl));
+    const float sign_norm = sign(dot3(odx, ody, odz, pnx, pny, pnz));
+    const float cos_norm = saturate(fd(dot3(pnx, pny, pnz, vx, vy, vz), pnl));
     const float n = fm(sign_norm, gtao_fast_acos(cos_norm));
     const float mul_u = fm(cs, sr_u), mul_v = fm(-sn, sr_v);
     uint32_t bitmask = 0;
     float occlusion = 0.0f;
     for (float sample_t = 0.0f; sample_t < sps; sample_t = fa(sample_t, 1.0f)) {
-      const float sample_noise = vfract(fa(n1, fm(fa(slice_t, fm(sample_t, sps)), 0.6180339887498948482f)));
+      const float sample_noise = frac(fa(n1, fm(fa(slice_t, fm(sample_t, sps)), 0.6180339887498948482f)));
       float s = fd(fa(sample_t, sample_noise), sps);
       s = fm(s, s);
       s = fa(s, min_s);
@@ -297,16 +273,16 @@ OXC_DI float gtao_occlusion(const GtaoParams& p, int x, int y, float ld) {
       const float e2x = fs(s2x, ox), e2y = fs(s2y, oy), e2z = fs(s2z, oz);
       const uint32_t m1 = gtao_sector_mask(p.thickness, e1x, e1y, e1z, vx, vy, vz, 1.0f, n);
       const uint32_t m2 = gtao_sector_mask(p.thickness, e2x, e2y, e2z, vx, vy, vz, -1.0f, n);
-      const float f1 = gtao_sat(fa(fm(length3(e1x, e1y, e1z), falloff_mul), falloff_add));
-      const float f2 = gtao_sat(fa(fm(length3(e2x, e2y, e2z), falloff_mul), falloff_add));
+      const float f1 = saturate(fa(fm(length3(e1x, e1y, e1z), falloff_mul), falloff_add));
+      const float f2 = saturate(fa(fm(length3(e2x, e2y, e2z), falloff_mul), falloff_add));
       occlusion = fa(occlusion, fd(fm(f1, (float)gtao_popc(m1 & ~bitmask)), (float)GTAO_SECTORS));
       bitmask |= m1;
       occlusion = fa(occlusion, fd(fm(f2, (float)gtao_popc(m2 & ~bitmask)), (float)GTAO_SECTORS));
       bitmask |= m2;
     }
-    visibility = fa(visibility, gtao_sat(fs(1.0f, occlusion)));
+    visibility = fa(visibility, saturate(fs(1.0f, occlusion)));
   }
-  return gtao_sat(fd(visibility, slice_count));
+  return saturate(fd(visibility, slice_count));
 }
 
 OXC_DI float gtao_unorm8(uint32_t v, int i) { return fd((float)((v >> (8 * i)) & 0xFFu), 255.0f); }
@@ -314,8 +290,8 @@ OXC_DI float gtao_unorm8(uint32_t v, int i) { return fd((float)((v >> (8 * i)) &
 // vbgtao_denoise.slang:14-82 for pixel (x, y)
 OXC_DI float gtao_denoise(const GtaoParams& p, int x, int y) {
   const int W = p.width, H = p.height;
-  const int xl = gtao_clamp((long long)x - 1, W), xr = gtao_clamp((long long)x + 1, W);
-  const size_t rt = (size_t)gtao_clamp((long long)y - 1, H) * W, rc = (size_t)y * W, rb = (size_t)gtao_clamp((long long)y + 1, H) * W;
+  const int xl = clamp_index((long long)x - 1, W), xr = clamp_index((long long)x + 1, W);
+  const size_t rt = (size_t)clamp_index((long long)y - 1, H) * W, rc = (size_t)y * W, rb = (size_t)clamp_index((long long)y + 1, H) * W;
   const uint32_t ec = __ldg(&p.edges[rc + x]), el = __ldg(&p.edges[rc + xl]), er = __ldg(&p.edges[rc + xr]);
   const uint32_t et = __ldg(&p.edges[rt + x]), eb = __ldg(&p.edges[rb + x]);
   const float center_w = 1.2f;
@@ -328,15 +304,15 @@ OXC_DI float gtao_denoise(const GtaoParams& p, int x, int y) {
   const float bl_w = fm(0.425f, fa(fm(bottom_w, gtao_unorm8(eb, 0)), fm(left_w, gtao_unorm8(el, 3))));
   const float br_w = fm(0.425f, fa(fm(bottom_w, gtao_unorm8(eb, 1)), fm(right_w, gtao_unorm8(er, 3))));
   const uint16_t* q = p.noisy;
-  float sum = fm(gtao_half_float(__ldg(&q[rc + x])), center_w);
-  sum = fa(sum, fm(gtao_half_float(__ldg(&q[rc + xl])), left_w));
-  sum = fa(sum, fm(gtao_half_float(__ldg(&q[rc + xr])), right_w));
-  sum = fa(sum, fm(gtao_half_float(__ldg(&q[rt + x])), top_w));
-  sum = fa(sum, fm(gtao_half_float(__ldg(&q[rb + x])), bottom_w));
-  sum = fa(sum, fm(gtao_half_float(__ldg(&q[rt + xl])), tl_w));
-  sum = fa(sum, fm(gtao_half_float(__ldg(&q[rt + xr])), tr_w));
-  sum = fa(sum, fm(gtao_half_float(__ldg(&q[rb + xl])), bl_w));
-  sum = fa(sum, fm(gtao_half_float(__ldg(&q[rb + xr])), br_w));
+  float sum = fm(half_float(__ldg(&q[rc + x])), center_w);
+  sum = fa(sum, fm(half_float(__ldg(&q[rc + xl])), left_w));
+  sum = fa(sum, fm(half_float(__ldg(&q[rc + xr])), right_w));
+  sum = fa(sum, fm(half_float(__ldg(&q[rt + x])), top_w));
+  sum = fa(sum, fm(half_float(__ldg(&q[rb + x])), bottom_w));
+  sum = fa(sum, fm(half_float(__ldg(&q[rt + xl])), tl_w));
+  sum = fa(sum, fm(half_float(__ldg(&q[rt + xr])), tr_w));
+  sum = fa(sum, fm(half_float(__ldg(&q[rb + xl])), bl_w));
+  sum = fa(sum, fm(half_float(__ldg(&q[rb + xr])), br_w));
   float sw = center_w;
   sw = fa(sw, left_w);
   sw = fa(sw, right_w);

@@ -30,8 +30,6 @@ struct PbrAtmParams {
   float ap_start, ap_exposure;
 };
 
-__host__ inline float pbra_host_sat(float x) { return atm_host_max(x, 0.0f) < 1.0f ? atm_host_max(x, 0.0f) : 1.0f; }
-
 // the kernel's parameters from the C ABI's arguments (oxc_apply_pbr_atmosphere, and the host build of the tests)
 __host__ inline PbrAtmParams pbr_atmosphere_make_params(const OxcPbrCamera& cam, const OxcPbrSettings& st, const OxcAtmosphere& a,
                                                         const OxcLight* lights, const OxcPbrInputs& in, const OxcPbrSky& sky, uint32_t w,
@@ -41,14 +39,14 @@ __host__ inline PbrAtmParams pbr_atmosphere_make_params(const OxcPbrCamera& cam,
   p.atm = atmosphere_make_params(a, &cam, st.sun_direction, st.sun_intensity, sky.transmittance, nullptr, nullptr, nullptr, 0);
   // sky_view_params_to_lut_uv with altitude = eye_pos.y as pbr_apply.slang:110 passes it (not length(eye_pos))
   const float alt = p.atm.eye_y;
-  const float horizon = sqrtf(atm_host_max(0.0f, alt * alt - a.planet_radius * a.planet_radius));
+  const float horizon = sqrtf(vmax(0.0f, alt * alt - a.planet_radius * a.planet_radius));
   p.atm.beta = canonical_acos(horizon / alt);
-  p.atm.zenith_horizon = ATM_PI - p.atm.beta;
+  p.atm.zenith_horizon = PI - p.atm.beta;
   p.sky_view = sky.sky_view; p.aerial = sky.aerial_perspective; p.cube = sky.sky_cube;
   p.min_altitude = a.planet_radius + ATM_PLANET_RADIUS_OFFSET;
   const float* L = st.sun_direction;
   p.sun_cos_theta = (L[0] * 0.0f + L[1] * 1.0f) + L[2] * 0.0f;
-  const float t = pbra_host_sat((p.sun_cos_theta - PBRA_HD_LO) / (PBRA_HD_HI - PBRA_HD_LO));
+  const float t = saturate((p.sun_cos_theta - PBRA_HD_LO) / (PBRA_HD_HI - PBRA_HD_LO));
   p.horizon_darkening = (t * t) * (3.0f - 2.0f * t);
   p.min_cos = canonical_cos(PBRA_SUN_RADIANS);
   p.ap_per_slice_depth = (float)a.aerial_perspective_lut_size[0] / (float)a.aerial_perspective_lut_size[2];
@@ -69,8 +67,8 @@ OXC_DI float pbra_draw_sun(float min_cos, float cos_theta) {
 // one binary16 RGBA texel of a plane, read exactly
 OXC_DI void pbra_texel(const uint16_t* plane, size_t texel, float o[4]) {
   const uint2 q = __ldg(reinterpret_cast<const uint2*>(plane) + texel);
-  o[0] = gtao_half_float((uint16_t)q.x); o[1] = gtao_half_float((uint16_t)(q.x >> 16));
-  o[2] = gtao_half_float((uint16_t)q.y); o[3] = gtao_half_float((uint16_t)(q.y >> 16));
+  o[0] = half_float((uint16_t)q.x); o[1] = half_float((uint16_t)(q.x >> 16));
+  o[2] = half_float((uint16_t)q.y); o[3] = half_float((uint16_t)(q.y >> 16));
 }
 
 // SampleLevel(linear_clamp, (u, v, w), 0) of the aerial-perspective LUT: the atmosphere's bilinear rule (item 5) in slices z0 and z0 + 1
@@ -80,8 +78,8 @@ OXC_DI void pbra_tap3(const PbrAtmParams& p, float u, float v, float w, float ou
   const float z = fs(fm(w, (float)D), 0.5f);
   const float z0 = floorf(z);
   const float wz = fs(z, z0);
-  const long long iz = alpha_f2i(z0);
-  const int za = gtao_clamp(iz, D), zb = gtao_clamp(iz + 1, D);
+  const long long iz = sat_i32(z0);
+  const int za = clamp_index(iz, D), zb = clamp_index(iz + 1, D);
   float s0[4], s1[4];
   sib_tap4(p.aerial + (size_t)za * H * W * 4, W, H, u, v, s0);
   sib_tap4(p.aerial + (size_t)zb * H * W * 4, W, H, u, v, s1);
@@ -89,16 +87,16 @@ OXC_DI void pbra_tap3(const PbrAtmParams& p, float u, float v, float w, float ou
 }
 
 // sample_aerial_perspective (sky.slang:258-293) at tex_coord (u, v) and camera_relative_pos d
-OXC_DI void pbra_aerial(const PbrAtmParams& p, float u, float v, PbrV3 d, float out[4]) {
+OXC_DI void pbra_aerial(const PbrAtmParams& p, float u, float v, Vec3 d, float out[4]) {
   const float dz = (float)p.atm.ap_d;
-  const float relative_depth = vmax(0.0f, fs(fsq(pbr_dot(d, d)), p.ap_start));
+  const float relative_depth = vmax(0.0f, fs(fsq(vdot(d, d)), p.ap_start));
   const float linear_slice = fm(relative_depth, fd(1.0f, p.ap_per_slice_depth));
   const float linear_w = fm(linear_slice, fd(1.0f, dz));
   const float non_linear_w = fsq(linear_w);
   const float non_linear_slice = fm(non_linear_w, dz);
   float weight = 1.0f;
-  if (non_linear_slice < PBRA_HALF_SLICE) weight = pbr_sat(fm(fm(non_linear_slice, non_linear_slice), 2.0f));
-  weight = fm(weight, pbr_sat(fm(relative_depth, PBRA_NEAR_FADE)));
+  if (non_linear_slice < PBRA_HALF_SLICE) weight = saturate(fm(fm(non_linear_slice, non_linear_slice), 2.0f));
+  weight = fm(weight, saturate(fm(relative_depth, PBRA_NEAR_FADE)));
   pbra_tap3(p, u, v, non_linear_w, out);
   for (int c = 0; c < 3; c++) out[c] = fm(out[c], weight);
   out[3] = fs(1.0f, fm(weight, fs(1.0f, out[3])));
@@ -164,16 +162,16 @@ OXC_DI void pbra_cube_fetch(const uint16_t* cube, int f, int i, int j, float o[4
 // TextureCube.SampleLevel(linear_clamp, r, 0) of the 32 x 32 cube: face and (sc, tc, ma) by pbra_cube_face, s = 0.5 * (sc / |ma|) + 0.5
 // (t likewise), x = s * 32 - 0.5, x0 = floor(x), wx = x - x0 (y likewise), NaN-safe indices clamped to -1..32, the 2 x 2 footprint
 // through pbra_cube_fetch, the atmosphere's bilinear order (top = a00 + wx * (a10 - a00), bottom likewise, top + wy * (bottom - top))
-OXC_DI void pbra_cube_tap(const uint16_t* cube, PbrV3 r, float out[4]) {
+OXC_DI void pbra_cube_tap(const uint16_t* cube, Vec3 r, float out[4]) {
   float sc, tc, ma;
   const int f = pbra_cube_face(r.x, r.y, r.z, sc, tc, ma);
   const float s = fa(fm(0.5f, fd(sc, fabsf(ma))), 0.5f), t = fa(fm(0.5f, fd(tc, fabsf(ma))), 0.5f);
   const float x = fs(fm(s, (float)SKY_IBL_RES), 0.5f), y = fs(fm(t, (float)SKY_IBL_RES), 0.5f);
   const float x0 = floorf(x), y0 = floorf(y);
   const float wx = fs(x, x0), wy = fs(y, y0);
-  const long long ix = alpha_f2i(x0), iy = alpha_f2i(y0);
-  const int i0 = gtao_clamp(ix + 1, SKY_IBL_RES + 2) - 1, j0 = gtao_clamp(iy + 1, SKY_IBL_RES + 2) - 1;
-  const int i1 = gtao_clamp(ix + 2, SKY_IBL_RES + 2) - 1, j1 = gtao_clamp(iy + 2, SKY_IBL_RES + 2) - 1;
+  const long long ix = sat_i32(x0), iy = sat_i32(y0);
+  const int i0 = clamp_index(ix + 1, SKY_IBL_RES + 2) - 1, j0 = clamp_index(iy + 1, SKY_IBL_RES + 2) - 1;
+  const int i1 = clamp_index(ix + 2, SKY_IBL_RES + 2) - 1, j1 = clamp_index(iy + 2, SKY_IBL_RES + 2) - 1;
   float a00[4], a10[4], a01[4], a11[4];
   pbra_cube_fetch(cube, f, i0, j0, a00);
   pbra_cube_fetch(cube, f, i1, j0, a10);
@@ -198,46 +196,44 @@ OXC_DI float4 pbr_atmosphere_pixel(const PbrAtmParams& p, const PbrLight* lights
   float mu, rr, T[4];
   atm_transmittance_uv(p.atm.atmos_radius, p.atm.planet_radius, world_eye_y, p.sun_cos_theta, mu, rr);
   sib_tap4(p.atm.transmittance, p.atm.t_w, p.atm.t_h, mu, rr, T);
-  const PbrV3 direct = v3(fm(fm(T[0], b.sun_intensity), p.horizon_darkening), fm(fm(T[1], b.sun_intensity), p.horizon_darkening),
-                          fm(fm(T[2], b.sun_intensity), p.horizon_darkening));
-  const PbrV3 Vn = v3(-q.s.V.x, -q.s.V.y, -q.s.V.z);
+  const Vec3 direct = vec3(fm(fm(T[0], b.sun_intensity), p.horizon_darkening), fm(fm(T[1], b.sun_intensity), p.horizon_darkening),
+                           fm(fm(T[2], b.sun_intensity), p.horizon_darkening));
   if (depth == 0.0f) {
     // :108-124
-    const AtmV3 up = atm_v3(0.0f, 1.0f, 0.0f), mv = atm_v3(Vn.x, Vn.y, Vn.z);
-    const AtmV3 right = atm_normalize(sib_cross(up, mv));
-    const AtmV3 forward = atm_normalize(sib_cross(right, up));
-    const AtmV3 L = atm_v3(q.Ls.x, q.Ls.y, q.Ls.z);
-    float lx = atm_dot(L, forward), ly = atm_dot(L, right);
+    const Vec3 up = vec3(0.0f, 1.0f, 0.0f), mv = vec3(-q.s.V.x, -q.s.V.y, -q.s.V.z), L = q.Ls;
+    const Vec3 right = vnormalize(vcross(up, mv));
+    const Vec3 forward = vnormalize(vcross(right, up));
+    float lx = vdot(L, forward), ly = vdot(L, right);
     const float ll = fsq(fa(fm(lx, lx), fm(ly, ly)));
     lx = fd(lx, ll); ly = fd(ly, ll);
-    const float view_zenith_cos = atm_dot(mv, up);
+    const float view_zenith_cos = vdot(mv, up);
     float t;
-    const bool hit = atm_ray_sphere_nearest(atm_v3(0.0f, p.atm.eye_y, 0.0f), mv, p.atm.planet_radius, t);
+    const bool hit = atm_ray_sphere_nearest(vec3(0.0f, p.atm.eye_y, 0.0f), mv, p.atm.planet_radius, t);
     float u, v, s[4];
     sky_ibl_sky_view_uv(p.atm, hit, view_zenith_cos, lx, ly, u, v);
     sib_tap4(p.sky_view, p.atm.sv_w, p.atm.sv_h, u, v, s);
     if (!hit) {
-      const float sun = fm(pbra_draw_sun(p.min_cos, atm_dot(mv, L)), b.sun_intensity);
+      const float sun = fm(pbra_draw_sun(p.min_cos, vdot(mv, L)), b.sun_intensity);
       for (int c = 0; c < 3; c++) s[c] = fa(s[c], fm(sun, T[c]));
     }
-    return make_float4(pbr_store(fm(s[0], s[3])), pbr_store(fm(s[1], s[3])), pbr_store(fm(s[2], s[3])), 1.0f);
+    return make_float4(nan_canonical(fm(s[0], s[3])), nan_canonical(fm(s[1], s[3])), nan_canonical(fm(s[2], s[3])), 1.0f);
   }
   // :126-141
   float ap[4];
   pbra_aerial(p, q.u, q.v,
-              v3(fm(fs(q.world.x, b.cam_pos[0]), ATM_CAMERA_SCALE_UNIT), fm(fs(q.world.y, b.cam_pos[1]), ATM_CAMERA_SCALE_UNIT),
-                 fm(fs(q.world.z, b.cam_pos[2]), ATM_CAMERA_SCALE_UNIT)),
+              vec3(fm(fs(q.world.x, b.cam_pos[0]), ATM_CAMERA_SCALE_UNIT), fm(fs(q.world.y, b.cam_pos[1]), ATM_CAMERA_SCALE_UNIT),
+                   fm(fs(q.world.z, b.cam_pos[2]), ATM_CAMERA_SCALE_UNIT)),
               ap);
-  const PbrV3 aerial = v3(fm(ap[0], ap[3]), fm(ap[1], ap[3]), fm(ap[2], ap[3]));
+  const Vec3 aerial = vec3(fm(ap[0], ap[3]), fm(ap[1], ap[3]), fm(ap[2], ap[3]));
   const float k = fs(1.0f, q.roughness);
-  const PbrV3 N = q.s.N;
-  const PbrV3 rd = pbr_normalize(v3(fa(N.x, fm(fs(q.R.x, N.x), k)), fa(N.y, fm(fs(q.R.y, N.y), k)), fa(N.z, fm(fs(q.R.z, N.z), k))));
+  const Vec3 N = q.s.N;
+  const Vec3 rd = vnormalize(vec3(fa(N.x, fm(fs(q.R.x, N.x), k)), fa(N.y, fm(fs(q.R.y, N.y), k)), fa(N.z, fm(fs(q.R.z, N.z), k))));
   float ss[4], ds[4];
   pbra_cube_tap(p.cube, rd, ss);
   pbra_cube_tap(p.cube, N, ds);
   const float hd = p.horizon_darkening;
-  const PbrV3 specular_sky = v3(fm(fm(ss[0], ss[3]), hd), fm(fm(ss[1], ss[3]), hd), fm(fm(ss[2], ss[3]), hd));
-  const PbrV3 diffuse_sky = v3(fm(fm(ds[0], ds[3]), hd), fm(fm(ds[1], ds[3]), hd), fm(fm(ds[2], ds[3]), hd));
+  const Vec3 specular_sky = vec3(fm(fm(ss[0], ss[3]), hd), fm(fm(ss[1], ss[3]), hd), fm(fm(ss[2], ss[3]), hd));
+  const Vec3 diffuse_sky = vec3(fm(fm(ds[0], ds[3]), hd), fm(fm(ds[1], ds[3]), hd), fm(fm(ds[2], ds[3]), hd));
   return pbr_shade(b, lights, q, diffuse_sky, specular_sky, direct, visibility, &aerial);
 }
 

@@ -1,0 +1,84 @@
+// oxc_shader_math.cuh — the HLSL-semantics primitives the screen-space passes' per-pixel headers share: max / min / saturate / sign /
+// frac with the shaders' NaN rules, the saturating float -> integer conversions and the index clamp of the software taps, the binary16
+// conversions of the planes the passes store, pi, and one 3-vector with the canonical operation order.  Each states its NaN and
+// rounding rule once, so every pass that calls it gives the same bits.
+// No warp intrinsics, no shared memory: tests compile this source for the host.
+#pragma once
+#include <climits>
+
+#include "oxc_exact.cuh"
+
+namespace oxc {
+
+constexpr float PI = 0x1.921fb6p+1f; // 0x40490FDB, common/math.slang:4
+
+// HLSL max / min with IEEE maxNum / minNum NaN handling (a NaN operand yields the other one); equal operands yield b
+OXC_HD float vmax(float a, float b) { return (b != b || a > b) ? a : b; }
+OXC_HD float vmin(float a, float b) { return (b != b || a < b) ? a : b; }
+OXC_HD float saturate(float x) { return vmin(vmax(x, 0.0f), 1.0f); } // NaN -> 0
+OXC_DI float sign(float x) { return x > 0.0f ? 1.0f : (x < 0.0f ? -1.0f : 0.0f); } // NaN -> 0
+OXC_DI float frac(float x) { return fs(x, floorf(x)); } // x - floor(x)
+
+// float -> i32, truncating, saturating, NaN -> 0 (cvt.rzi.s32.f32; the host build and the device agree for every input)
+OXC_DI int sat_i32(float f) { return !(f == f) ? 0 : (f >= 2147483648.0f ? INT_MAX : (f <= -2147483648.0f ? INT_MIN : (int)f)); }
+// float -> u32, truncating, saturating, NaN -> 0
+OXC_DI uint32_t sat_u32(float f) { return !(f > 0.0f) ? 0u : (f >= 4294967296.0f ? 0xFFFFFFFFu : (uint32_t)f); }
+// a texel index clamped to the edge of an extent n >= 1
+OXC_DI int clamp_index(long long i, int n) { return (int)(i < 0 ? 0 : (i > n - 1 ? n - 1 : i)); }
+
+// the blend of two mip levels' values: (1 - f) * lo + f * hi
+OXC_DI float lerp_levels(float f, float lo, float hi) { return fa(fm(fs(1.0f, f), lo), fm(f, hi)); }
+OXC_DI float4 lerp_levels(float f, float4 lo, float4 hi) {
+  return make_float4(lerp_levels(f, lo.x, hi.x), lerp_levels(f, lo.y, hi.y), lerp_levels(f, lo.z, hi.z), lerp_levels(f, lo.w, hi.w));
+}
+
+// binary32 -> binary16 with round-to-nearest-even -> binary32 (the R16G16B16A16Sfloat normal attachment); NaN stays NaN
+OXC_DI float round_to_half(float f) {
+#ifdef __CUDA_ARCH__
+  return __half2float(__float2half_rn(f));
+#else
+  const uint32_t u = __float_as_uint(f), sign = u & 0x80000000u, a = u & 0x7FFFFFFFu;
+  if (a >= 0x7F800000u) return f;                                        // inf, NaN
+  if (a >= 0x38800000u) {                                                // half normal range: keep 10 fraction bits
+    const uint32_t r = (a + 0xFFFu + ((a >> 13) & 1u)) & ~0x1FFFu;
+    return __uint_as_float(sign | (r > 0x477FE000u ? 0x7F800000u : r)); // above 65504: inf
+  }
+  const float m = rintf(__uint_as_float(a) * 16777216.0f);             // half subnormals: multiples of 2^-24
+  return __uint_as_float(sign | __float_as_uint(m * 5.9604644775390625e-08f));
+#endif
+}
+
+// binary32 -> binary16 bits, round to nearest even
+OXC_DI uint16_t half_bits(float f) {
+#ifdef __CUDA_ARCH__
+  return __half_as_ushort(__float2half_rn(f));
+#else
+  const float r = round_to_half(f);
+  const uint32_t u = __float_as_uint(r), s = (u >> 16) & 0x8000u, a = u & 0x7FFFFFFFu;
+  if (a > 0x7F800000u) return (uint16_t)(s | 0x7FFFu);
+  if (a == 0x7F800000u) return (uint16_t)(s | 0x7C00u);
+  if (a >= 0x38800000u) return (uint16_t)(s | (((a >> 23) - 112u) << 10) | ((a >> 13) & 0x3FFu));
+  return (uint16_t)(s | (uint32_t)fm(__uint_as_float(a), 16777216.0f));
+#endif
+}
+OXC_DI float half_float(uint16_t h) { return __half2float(__ushort_as_half(h)); }
+
+// the value a binary32 plane is stored as: a NaN is written as 0x7FFFFFFF, the NaN the GPU's arithmetic produces (the host's differs)
+OXC_DI float nan_canonical(float v) { return v != v ? __uint_as_float(0x7FFFFFFFu) : v; }
+
+// a 3-vector; every operation rounds each component once, dot is (a.x * b.x + a.y * b.y) + a.z * b.z
+struct Vec3 {
+  float x, y, z;
+};
+OXC_DI Vec3 vec3(float x, float y, float z) { return Vec3{x, y, z}; }
+OXC_DI float vdot(Vec3 a, Vec3 b) { return dot3(a.x, a.y, a.z, b.x, b.y, b.z); }
+OXC_DI float vlength(Vec3 a) { return fsq(vdot(a, a)); }
+OXC_DI Vec3 vadd(Vec3 a, Vec3 b) { return vec3(fa(a.x, b.x), fa(a.y, b.y), fa(a.z, b.z)); }
+OXC_DI Vec3 vsub(Vec3 a, Vec3 b) { return vec3(fs(a.x, b.x), fs(a.y, b.y), fs(a.z, b.z)); }
+OXC_DI Vec3 vmul(Vec3 a, Vec3 b) { return vec3(fm(a.x, b.x), fm(a.y, b.y), fm(a.z, b.z)); }
+OXC_DI Vec3 vscale(Vec3 a, float s) { return vec3(fm(a.x, s), fm(a.y, s), fm(a.z, s)); } // a * s
+OXC_DI Vec3 vdiv(Vec3 a, float s) { return vec3(fd(a.x, s), fd(a.y, s), fd(a.z, s)); }
+OXC_DI Vec3 vnormalize(Vec3 a) { return vdiv(a, vlength(a)); }
+OXC_DI Vec3 vcross(Vec3 a, Vec3 b) { return vec3(fs(fm(a.y, b.z), fm(a.z, b.y)), fs(fm(a.z, b.x), fm(a.x, b.z)), fs(fm(a.x, b.y), fm(a.y, b.x))); }
+
+} // namespace oxc

@@ -3,7 +3,7 @@
 // no warp intrinsics, no shared memory, so tests compile this source for the host; kernels_sky_ibl.cuh lays the samples out.
 // Specification: include/oxcull.h (comment above oxc_atmosphere_sky_ibl) == oracle/oxc_oracle_sky_ibl.c, operation for operation.
 #pragma once
-#include "oxc_atmosphere.cuh" // AtmosphereParams, AtmV3 and its operations, atm_ray_sphere_nearest, atm_transmittance_uv, atm_store
+#include "oxc_atmosphere.cuh"
 
 namespace oxc {
 
@@ -53,12 +53,7 @@ __host__ inline SkyIblParams sky_ibl_make_params(const OxcAtmosphere& a, const O
   return p;
 }
 
-OXC_DI AtmV3 sib_cross(AtmV3 a, AtmV3 b) {
-  return atm_v3(fs(fm(a.y, b.z), fm(a.z, b.y)), fs(fm(a.z, b.x), fm(a.x, b.z)), fs(fm(a.x, b.y), fm(a.y, b.x)));
-}
-OXC_DI float sib_frac(float x) { return fs(x, floorf(x)); }
 OXC_DI float sib_sanitize(float x) { return fabsf(x) < __uint_as_float(0x7F800000u) ? x : 0.0f; } // isfinite ? x : 0
-OXC_DI float sib_saturate(float x) { return vmin(vmax(x, 0.0f), 1.0f); }
 
 // SampleLevel(linear_clamp, (u, v), 0) of a w x h binary16 RGBA plane, all four channels: the atmosphere's tap rule (include/oxcull.h,
 // atmosphere item 5) for any plane
@@ -66,22 +61,22 @@ OXC_DI void sib_tap4(const uint16_t* plane, int w, int h, float u, float v, floa
   const float x = fs(fm(u, (float)w), 0.5f), y = fs(fm(v, (float)h), 0.5f);
   const float x0 = floorf(x), y0 = floorf(y);
   const float wx = fs(x, x0), wy = fs(y, y0);
-  const long long ix = alpha_f2i(x0), iy = alpha_f2i(y0);
-  const int xa = gtao_clamp(ix, w), xb = gtao_clamp(ix + 1, w), ya = gtao_clamp(iy, h), yb = gtao_clamp(iy + 1, h);
+  const long long ix = sat_i32(x0), iy = sat_i32(y0);
+  const int xa = clamp_index(ix, w), xb = clamp_index(ix + 1, w), ya = clamp_index(iy, h), yb = clamp_index(iy + 1, h);
   const uint2* t = reinterpret_cast<const uint2*>(plane);
   const uint2 q[4] = {__ldg(t + (size_t)ya * w + xa), __ldg(t + (size_t)ya * w + xb), __ldg(t + (size_t)yb * w + xa),
                       __ldg(t + (size_t)yb * w + xb)};
   for (int c = 0; c < 4; c++) {
     const int sh = (c & 1) * 16;
     float a[4];
-    for (int k = 0; k < 4; k++) a[k] = gtao_half_float((uint16_t)(((c < 2) ? q[k].x : q[k].y) >> sh));
+    for (int k = 0; k < 4; k++) a[k] = half_float((uint16_t)(((c < 2) ? q[k].x : q[k].y) >> sh));
     const float top = fa(a[0], fm(wx, fs(a[1], a[0]))), bot = fa(a[2], fm(wx, fs(a[3], a[2])));
     out[c] = fa(top, fm(wy, fs(bot, top)));
   }
 }
 
 // sky_ibl.slang:21-30 and :67-68: the direction of texel (x, y) of `face`; the face matrices by rows, mul(M, v) row by row
-OXC_DI AtmV3 sky_ibl_dir(int face, int x, int y) {
+OXC_DI Vec3 sky_ibl_dir(int face, int x, int y) {
   const float u = fd(fa((float)x, 0.5f), (float)SKY_IBL_RES), v = fd(fa((float)y, 0.5f), (float)SKY_IBL_RES);
   const float qx = fs(fm(u, 2.0f), 1.0f), qy = fs(fm(v, 2.0f), 1.0f), qz = -1.0f;
   float m[9];
@@ -93,34 +88,34 @@ OXC_DI AtmV3 sky_ibl_dir(int face, int x, int y) {
     case 4: { const float r[9] = {1, 0, 0, 0, -1, 0, 0, 0, -1}; for (int k = 0; k < 9; k++) m[k] = r[k]; break; }
     default: { const float r[9] = {-1, 0, 0, 0, -1, 0, 0, 0, 1}; for (int k = 0; k < 9; k++) m[k] = r[k]; break; }
   }
-  return atm_normalize(atm_v3(dot3(m[0], m[1], m[2], qx, qy, qz), dot3(m[3], m[4], m[5], qx, qy, qz), dot3(m[6], m[7], m[8], qx, qy, qz)));
+  return vnormalize(vec3(dot3(m[0], m[1], m[2], qx, qy, qz), dot3(m[3], m[4], m[5], qx, qy, qz), dot3(m[6], m[7], m[8], qx, qy, qz)));
 }
 
 // what every sample of a texel shares: its direction and tangent frame (:72-74), its history (:76-77) and the rotation (:79-82)
 struct SkyIblTexel {
-  AtmV3 dir, tangent, bitangent;
+  Vec3 dir, tangent, bitangent;
   float history[4];
   bool has_history;
   float rotation;
 };
 
 // sky_ibl.slang:41-44 interleaved_gradient_noise
-OXC_DI float sky_ibl_ign(float px, float py) { return sib_frac(fm(SKY_IBL_IGN_Z, sib_frac(fa(fm(px, SKY_IBL_IGN_X), fm(py, SKY_IBL_IGN_Y))))); }
+OXC_DI float sky_ibl_ign(float px, float py) { return frac(fm(SKY_IBL_IGN_Z, frac(fa(fm(px, SKY_IBL_IGN_X), fm(py, SKY_IBL_IGN_Y))))); }
 
 OXC_DI SkyIblTexel sky_ibl_texel(const SkyIblParams& p, int face, int x, int y) {
   SkyIblTexel t;
   t.dir = sky_ibl_dir(face, x, y);
-  const AtmV3 up = fabsf(t.dir.y) < SKY_IBL_UP_LIMIT ? atm_v3(0.0f, 1.0f, 0.0f) : atm_v3(1.0f, 0.0f, 0.0f);
-  t.tangent = atm_normalize(sib_cross(up, t.dir));
-  t.bitangent = sib_cross(t.dir, t.tangent);
+  const Vec3 up = fabsf(t.dir.y) < SKY_IBL_UP_LIMIT ? vec3(0.0f, 1.0f, 0.0f) : vec3(1.0f, 0.0f, 0.0f);
+  t.tangent = vnormalize(vcross(up, t.dir));
+  t.bitangent = vcross(t.dir, t.tangent);
   const uint2 h = *reinterpret_cast<const uint2*>(p.cube + ((size_t)(face * SKY_IBL_RES + y) * SKY_IBL_RES + x) * 4);
-  t.history[0] = gtao_half_float((uint16_t)h.x); t.history[1] = gtao_half_float((uint16_t)(h.x >> 16));
-  t.history[2] = gtao_half_float((uint16_t)h.y); t.history[3] = gtao_half_float((uint16_t)(h.y >> 16));
+  t.history[0] = half_float((uint16_t)h.x); t.history[1] = half_float((uint16_t)(h.x >> 16));
+  t.history[2] = half_float((uint16_t)h.y); t.history[3] = half_float((uint16_t)(h.y >> 16));
   const float inf = __uint_as_float(0x7F800000u);
   t.has_history = t.history[3] > 0.0f && fabsf(t.history[0]) < inf && fabsf(t.history[1]) < inf && fabsf(t.history[2]) < inf;
   const float f = (float)face;
   const float base = sky_ibl_ign(fa((float)x, fm(f, 37.0f)), fa((float)y, fm(f, 17.0f)));
-  t.rotation = t.has_history ? sib_frac(fa(base, fm(p.frame, SKY_IBL_GOLDEN))) : base;
+  t.rotation = t.has_history ? frac(fa(base, fm(p.frame, SKY_IBL_GOLDEN))) : base;
   return t;
 }
 
@@ -150,7 +145,7 @@ OXC_DI void sky_ibl_sky_view_uv(const AtmosphereParams& a, bool intersect_planet
     v = fa(fm(coord, 0.5f), 0.5f);
   }
   const float theta = canonical_atan2(-ly, -lx);
-  u = fd(fa(theta, ATM_PI), ATM_TAU); // 2.0 * PI folds to TAU exactly
+  u = fd(fa(theta, PI), ATM_TAU); // 2.0 * PI folds to TAU exactly
   // from_unit_to_sub_uvs (:11-13): (uv + 0.5 / res) * (res / (res + 1))
   const float rw = (float)a.sv_w, rh = (float)a.sv_h;
   u = fm(fa(u, fd(0.5f, rw)), fd(rw, fa(rw, 1.0f)));
@@ -158,14 +153,14 @@ OXC_DI void sky_ibl_sky_view_uv(const AtmosphereParams& a, bool intersect_planet
 }
 
 // sky.slang:296-322 get_atmosphere_illuminance_along_ray(sun, (0, eye_y, 0), eye_dir), its up vector and normalized sun per call
-OXC_DI AtmV3 sky_ibl_illuminance(const SkyIblParams& p, AtmV3 eye_dir) {
-  const AtmV3 up = atm_v3(p.up[0], p.up[1], p.up[2]);
-  const float view_zenith_cos = atm_dot(eye_dir, up);
-  const AtmV3 side_raw = sib_cross(up, eye_dir);
-  const AtmV3 side = atm_length(side_raw) > SKY_IBL_SIDE_MIN ? atm_normalize(side_raw) : atm_v3(1.0f, 0.0f, 0.0f);
-  const AtmV3 forward = atm_normalize(sib_cross(side, up));
-  const AtmV3 sun = atm_v3(p.sun[0], p.sun[1], p.sun[2]);
-  float lx = atm_dot(sun, forward), ly = atm_dot(sun, side);
+OXC_DI Vec3 sky_ibl_illuminance(const SkyIblParams& p, Vec3 eye_dir) {
+  const Vec3 up = vec3(p.up[0], p.up[1], p.up[2]);
+  const float view_zenith_cos = vdot(eye_dir, up);
+  const Vec3 side_raw = vcross(up, eye_dir);
+  const Vec3 side = vlength(side_raw) > SKY_IBL_SIDE_MIN ? vnormalize(side_raw) : vec3(1.0f, 0.0f, 0.0f);
+  const Vec3 forward = vnormalize(vcross(side, up));
+  const Vec3 sun = vec3(p.sun[0], p.sun[1], p.sun[2]);
+  float lx = vdot(sun, forward), ly = vdot(sun, side);
   // safe_normalize (common/math.slang:90-93): len_sq > 1e-20 ? v * rsqrt(len_sq) : (1, 0), rsqrt(x) = fl(1 / fl(sqrt(x)))
   const float len_sq = fa(fm(lx, lx), fm(ly, ly));
   if (len_sq > SKY_IBL_SAFE_NORMALIZE_MIN) {
@@ -175,41 +170,41 @@ OXC_DI AtmV3 sky_ibl_illuminance(const SkyIblParams& p, AtmV3 eye_dir) {
     lx = 1.0f; ly = 0.0f;
   }
   float t;
-  const bool intersect_planet = atm_ray_sphere_nearest(atm_v3(0.0f, p.atm.eye_y, 0.0f), eye_dir, p.atm.planet_radius, t);
+  const bool intersect_planet = atm_ray_sphere_nearest(vec3(0.0f, p.atm.eye_y, 0.0f), eye_dir, p.atm.planet_radius, t);
   float u, v;
   sky_ibl_sky_view_uv(p.atm, intersect_planet, view_zenith_cos, lx, ly, u, v);
   float s[4];
   sib_tap4(p.sky_view, p.atm.sv_w, p.atm.sv_h, u, v, s);
-  return atm_v3(sib_sanitize(fm(s[0], s[3])), sib_sanitize(fm(s[1], s[3])), sib_sanitize(fm(s[2], s[3])));
+  return vec3(sib_sanitize(fm(s[0], s[3])), sib_sanitize(fm(s[1], s[3])), sib_sanitize(fm(s[2], s[3])));
 }
 
 // sky_ibl.slang:46-52 and :86-97: sample i of a texel, sanitized
-OXC_DI AtmV3 sky_ibl_sample(const SkyIblParams& p, const SkyIblTexel& t, int i) {
+OXC_DI Vec3 sky_ibl_sample(const SkyIblParams& p, const SkyIblTexel& t, int i) {
   const float u1 = fd(fa((float)i, 0.5f), (float)SKY_IBL_SAMPLES);
-  const float u2 = sib_frac(fa(sky_ibl_radical_inverse((uint32_t)i), t.rotation));
+  const float u2 = frac(fa(sky_ibl_radical_inverse((uint32_t)i), t.rotation));
   const float r = fsq(u1);
   const float phi = fm(ATM_TAU, u2);
   float sn, cs;
   canonical_sincos(phi, sn, cs);
   const float lx = fm(r, cs), ly = fm(r, sn), lz = fsq(vmax(0.0f, fs(1.0f, u1)));
-  const AtmV3 input_dir = atm_normalize(atm_add(atm_add(atm_scale(t.tangent, lx), atm_scale(t.bitangent, ly)), atm_scale(t.dir, lz)));
-  const AtmV3 s = sky_ibl_illuminance(p, input_dir);
-  return atm_v3(sib_sanitize(s.x), sib_sanitize(s.y), sib_sanitize(s.z));
+  const Vec3 input_dir = vnormalize(vadd(vadd(vscale(t.tangent, lx), vscale(t.bitangent, ly)), vscale(t.dir, lz)));
+  const Vec3 s = sky_ibl_illuminance(p, input_dir);
+  return vec3(sib_sanitize(s.x), sib_sanitize(s.y), sib_sanitize(s.z));
 }
 
 // sky_ibl.slang:99-115 for a texel whose 64 samples sum (in index order, from 0) to `sum`: the sun term, the clamp, the history lerp and
 // the store of (rgb, 1)
-OXC_DI void sky_ibl_finish(const SkyIblParams& p, const SkyIblTexel& t, int face, int x, int y, AtmV3 sum) {
+OXC_DI void sky_ibl_finish(const SkyIblParams& p, const SkyIblTexel& t, int face, int x, int y, Vec3 sum) {
   const AtmosphereParams& a = p.atm;
   float mu, rr;
   atm_transmittance_uv(a.atmos_radius, a.planet_radius, a.eye_y, p.sun_cos_zenith, mu, rr);
   float sun_color[4];
   sib_tap4(a.transmittance, a.t_w, a.t_h, mu, rr, sun_color);
-  const float sun_facing = sib_saturate(dot3(t.dir.x, t.dir.y, t.dir.z, p.sun_raw[0], p.sun_raw[1], p.sun_raw[2]));
+  const float sun_facing = saturate(dot3(t.dir.x, t.dir.y, t.dir.z, p.sun_raw[0], p.sun_raw[1], p.sun_raw[2]));
   const float est[3] = {sum.x, sum.y, sum.z};
   float out[3];
   for (int c = 0; c < 3; c++) {
-    const float sun_term = fd(fm(fm(fm(p.sun_ambient_strength, sun_color[c]), p.sun_intensity), sun_facing), ATM_PI);
+    const float sun_term = fd(fm(fm(fm(p.sun_ambient_strength, sun_color[c]), p.sun_intensity), sun_facing), PI);
     const float frame_result = vmin(vmax(sib_sanitize(fa(fd(est[c], (float)SKY_IBL_SAMPLES), sun_term)), 0.0f), ATM_HALF_MAX);
     out[c] = t.has_history ? fa(t.history[c], fm(fs(frame_result, t.history[c]), SKY_IBL_ALPHA)) : frame_result;
   }
@@ -219,8 +214,8 @@ OXC_DI void sky_ibl_finish(const SkyIblParams& p, const SkyIblTexel& t, int face
 // the whole texel with its 64 samples in one serial loop, as the shader writes it
 OXC_DI void sky_ibl_texel_serial(const SkyIblParams& p, int face, int x, int y) {
   const SkyIblTexel t = sky_ibl_texel(p, face, x, y);
-  AtmV3 sum = atm_v3(0.0f, 0.0f, 0.0f);
-  for (int i = 0; i < SKY_IBL_SAMPLES; i++) sum = atm_add(sum, sky_ibl_sample(p, t, i));
+  Vec3 sum = vec3(0.0f, 0.0f, 0.0f);
+  for (int i = 0; i < SKY_IBL_SAMPLES; i++) sum = vadd(sum, sky_ibl_sample(p, t, i));
   sky_ibl_finish(p, t, face, x, y, sum);
 }
 

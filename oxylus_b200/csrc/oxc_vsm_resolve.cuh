@@ -4,34 +4,9 @@
 // No warp intrinsics, no shared memory: tests compile this source for the host.
 // Specification: include/oxcull.h (comment above oxc_vsm_resolve_shadows) == oracle/oxc_oracle_vsm_resolve.c, operation for operation.
 #pragma once
-#include <climits>
-
-#include "oxc_exact.cuh"
+#include "oxc_shader_math.cuh"
 
 namespace oxc {
-
-// HLSL max / min with IEEE maxNum / minNum NaN handling (a NaN operand yields the other one); equal operands yield b
-OXC_DI float vmax(float a, float b) { return (b != b || a > b) ? a : b; }
-OXC_DI float vmin(float a, float b) { return (b != b || a < b) ? a : b; }
-OXC_DI float vfract(float x) { return fs(x, floorf(x)); } // fract(x) = x - floor(x)
-// float -> i32, truncating, saturating, NaN -> 0 (cvt.rzi.s32.f32)
-OXC_DI int vsm_f2i(float f) { return !(f == f) ? 0 : (f >= 2147483648.0f ? INT_MAX : (f <= -2147483648.0f ? INT_MIN : (int)f)); }
-
-// binary32 -> binary16 with round-to-nearest-even -> binary32 (the R16G16B16A16Sfloat normal attachment); NaN stays NaN
-OXC_DI float round_to_half(float f) {
-#ifdef __CUDA_ARCH__
-  return __half2float(__float2half_rn(f));
-#else
-  const uint32_t u = __float_as_uint(f), sign = u & 0x80000000u, a = u & 0x7FFFFFFFu;
-  if (a >= 0x7F800000u) return f;                                        // inf, NaN
-  if (a >= 0x38800000u) {                                                // half normal range: keep 10 fraction bits
-    const uint32_t r = (a + 0xFFFu + ((a >> 13) & 1u)) & ~0x1FFFu;
-    return __uint_as_float(sign | (r > 0x477FE000u ? 0x7F800000u : r)); // above 65504: inf
-  }
-  const float m = rintf(__uint_as_float(a) * 16777216.0f);             // half subnormals: multiples of 2^-24
-  return __uint_as_float(sign | __float_as_uint(m * 5.9604644775390625e-08f));
-#endif
-}
 
 // com::hammersley2d (common/math.slang:189-191): (i / N, reversebits(i) * 2^-32); host precomputation of the kernel's constants
 __host__ __device__ inline void vsm_hammersley(uint32_t i, uint32_t n, float& a, float& b) {
@@ -151,7 +126,7 @@ OXC_DI uint32_t vsm_select_clipmap(const P& p, float u, float v, float d) {
 OXC_DI bool vsm_wrapped_page(float cu, float cv, int size, int off_x, int off_y, int& wx, int& wy) {
   if (cu < 0.0f || cv < 0.0f || cu > 1.0f || cv > 1.0f) return false;
   const float fsz = (float)size;
-  const int vx = vsm_f2i(floorf(fm(cu, fsz))), vy = vsm_f2i(floorf(fm(cv, fsz)));
+  const int vx = sat_i32(floorf(fm(cu, fsz))), vy = sat_i32(floorf(fm(cv, fsz)));
   if (vx < 0 || vy < 0 || vx > size - 1 || vy > size - 1) return false;
   const float fox = (float)(vx + off_x), foy = (float)(vy + off_y);
   wx = (int)fs(fox, fm(fsz, floorf(fd(fox, fsz))));
@@ -187,7 +162,7 @@ OXC_DI float vsm_sample_depth(const VsmResolveParams& p, int ci, float x, float 
   if (!(e & 4u)) return VSM_DEPTH_MISS; // Backed
   const uint32_t addr = e >> 16, n = (uint32_t)p.phys_per_row;
   const float fP = (float)p.atlas_size, fps = (float)p.page_size;
-  const float tx = (float)vsm_f2i(floorf(fm(cu, fP))), ty = (float)vsm_f2i(floorf(fm(cv, fP))); // :56
+  const float tx = (float)sat_i32(floorf(fm(cu, fP))), ty = (float)sat_i32(floorf(fm(cv, fP))); // :56
   const int ix = (int)fs(tx, fm(fps, floorf(fd(tx, fps)))), iy = (int)fs(ty, fm(fps, floorf(fd(ty, fps)))); // :57 com::mod
   const long long ax = (long long)(addr % n) * p.page_size + ix, ay = (long long)(addr / n) * p.page_size + iy; // :55, 58
   if (ax < 0 || ay < 0 || ax >= p.atlas_size || ay >= p.atlas_size) return 0.0f;
@@ -208,14 +183,14 @@ OXC_DI float vsm_sample_fallback(const VsmResolveParams& p, int ci, float x, flo
 // :27-30 hash2 of the pixel position (x + 0.5, y + 0.5)
 OXC_DI void vsm_hash2(float px, float py, float& n0, float& n1) {
   const float d0 = fa(fm(px, 127.1f), fm(py, 311.7f)), d1 = fa(fm(px, 269.5f), fm(py, 183.3f));
-  n0 = vfract(fm(canonical_sin(d0), 43758.5453f));
-  n1 = vfract(fm(canonical_sin(d1), 43758.5453f));
+  n0 = frac(fm(canonical_sin(d0), 43758.5453f));
+  n1 = frac(fm(canonical_sin(d1), 43758.5453f));
 }
 
 // one PCSS tap (:119-127 / :161-169): returns the fall-back depth at the offset point, bias_norm through `bias_norm`
 OXC_DI float vsm_tap(const VsmResolveParams& p, const VsmBasis& b, int ci, float ox, float oy, float oz, float hx, float hy, float nx,
                      float ny, float radius, float nol, float base_bias, float inv_z, float& bias_norm) {
-  const float xi_x = vfract(fa(hx, nx)), xi_y = vfract(fa(hy, ny));
+  const float xi_x = frac(fa(hx, nx)), xi_y = frac(fa(hy, ny));
   const float r = fm(fsq(xi_x), radius);
   const float theta = fm(xi_y, 6.28318548f); // TAU
   float s, c;

@@ -41,14 +41,14 @@ int main(int argc, char** argv) {
                                                                                  gtao_virtual_level<3>, gtao_virtual_level<4>};
   for (int k = 0; k < GTAO_LEVELS; k++)
     for (int ty = 0; ty < p.mip_h[k]; ty++)
-      for (int tx = 0; tx < p.mip_w[k]; tx++) mips[(size_t)p.mip_off[k] + (size_t)ty * p.mip_w[k] + tx] = gtao_mip_store(level[k](p, tx, ty));
+      for (int tx = 0; tx < p.mip_w[k]; tx++) mips[(size_t)p.mip_off[k] + (size_t)ty * p.mip_w[k] + tx] = nan_canonical(level[k](p, tx, ty));
   size_t sky = 0;
   for (int y = 0; y < (int)H; y++)
     for (int x = 0; x < (int)W; x++) {
       float centre;
       edges[(size_t)y * W + x] = gtao_edges(p, x, y, &centre);
       sky += centre >= fm(p.far_clip, 0.999f);
-      noisy[(size_t)y * W + x] = gtao_half_bits(gtao_occlusion(p, x, y, centre));
+      noisy[(size_t)y * W + x] = half_bits(gtao_occlusion(p, x, y, centre));
     }
   for (int y = 0; y < (int)H; y++)
     for (int x = 0; x < (int)W; x++) ao[(size_t)y * W + x] = gtao_denoise(p, x, y);

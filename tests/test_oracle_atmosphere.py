@@ -33,9 +33,9 @@ def bits(x):
 
 
 PI = f32(math.pi)
-# name in oxc_atmosphere.cuh -> (bits, how the shader's value is formed)
+# name in oxc_atmosphere.cuh (PI: oxc_shader_math.cuh) -> (bits, how the shader's value is formed)
 CONSTANTS = {
-    "ATM_PI": (0x40490FDB, PI),
+    "PI": (0x40490FDB, PI),
     "ATM_TAU": (0x40C90FDB, f32(2 * math.pi)),
     "ATM_INV_4PI": (0x3DA2F983, f32(1) / (f32(4) * PI)),          # 1.0 / (4.0 * PI), 4 * PI exact
     "ATM_RAYLEIGH_K": (0x3D747645, f32(3) / (f32(16) * PI)),      # 3.0 / (16.0 * PI), 16 * PI exact
@@ -50,7 +50,7 @@ CONSTANTS = {
 def test_constants_bits():
     """each constant of the kernel header and of the oracle is the binary32 value the shader forms, with the bits the specification
     states; the folded quotients give the same bits in binary32 and in binary64 rounded once"""
-    src = open(os.path.join(ROOT, "oxylus_b200", "csrc", "oxc_atmosphere.cuh")).read()
+    src = "".join(open(os.path.join(ROOT, "oxylus_b200", "csrc", h)).read() for h in ("oxc_atmosphere.cuh", "oxc_shader_math.cuh"))
     orc = open(os.path.join(ROOT, "oracle", "oxc_oracle_atmosphere.c")).read()
     hdr = open(os.path.join(ROOT, "include", "oxcull.h")).read()
     for name, (b, value) in CONSTANTS.items():
