@@ -1189,6 +1189,105 @@ int oxc_apply_pbr_atmosphere(OxcContext* ctx, const OxcPbrCamera* camera, const 
                              const OxcLight* lights_dev, const OxcPbrInputs* inputs, const OxcPbrSky* sky, uint32_t width, uint32_t height,
                              float* out_dev, void* stream);
 
+/* Post-processing inputs of the tonemap (RendererInstance.cpp:1270-1286, Passes/PostProcess.cpp): eye adaptation, then bloom.  Both read
+ * the lit frame as either PBR apply writes it: width x height float4 (RGBA) per pixel, row-major, 16-byte aligned; alpha is not read.
+ * Rules of both (bit for bit with oracle/oxc_oracle_post.c): binary32, no contraction, operations in written order; max / min with the
+ * NaN rules of oxc_apply_pbr (a NaN operand yields the other one); clamp(x, a, b) = min(max(x, a), b); lerp(a, b, t) = a + (b - a) * t;
+ * f32(u32) rounds to nearest even; every stored NaN is 0x7FFFFFFF.  Deviation from the reference: both read the binary32 lit plane, and
+ * bloom keeps every level in binary32, where the reference stores B10G11R11 (whose conversion is not bit-defined).
+ *
+ * Eye adaptation (PostProcess.cpp:7-77, passes/histogram_generate.slang, histogram_average.slang): the 256-bin luminance histogram of the
+ * frame, then the exposure record's update.  The reference runs it under HasEyeAdaptation, which it sets only for a scene with an
+ * AutoExposureComponent.  exposure_dev: the persistent record, read and written in place (the reference fills it with 1.0 once, at
+ * allocation).  histogram_dev: 256 u32, zeroed by the call on its stream (a memset node in a graph); after the call it holds this frame's
+ * bins.  No other scratch, so the call is graph-capturable from its first call.
+ * Refused with OXC_E_INVALID, before anything is enqueued: a NULL argument, a frame not 16-byte aligned, a record not 8-byte aligned or a
+ * histogram not 4-byte aligned, a zero extent or one above 32768, a histogram or record that shares a byte with the frame or each other.
+ * NaN, Inf and denormal settings, delta_time and pixels are accepted and follow the rules below.
+ * SPECIFICATION (oracle/oxc_oracle_post.c orc_eye_adaptation):
+ *   1. per call, on the host (eye_adaptation_make_params): pixel_count = f32(width * height) (a u32 product); exposure_range = max_exposure
+ *      - min_exposure; time_coeff = 1 - canonical_exp(-adaptation_speed * delta_time) (the reference's glm::exp on the host); bias_scale =
+ *      (100 * ev100_bias) / 12.5.
+ *   2. per pixel: lum = (r * 0.2127 + g * 0.7152) + b * 0.0722 (0x3E59CE07, 0x3F371759, 0x3D93DD98).  lum < 0.001 (0x3A83126F) gives bin
+ *      0; otherwise mapped = ((canonical_log2(lum) - min_exposure) / exposure_range) * 254 + 1 and the bin is clamp(sat_i32(mapped), 0,
+ *      255), sat_i32 truncating and saturating, NaN -> 0.  So a NaN pixel, a -inf or negative one and one below 0.001 land in bin 0 (NaN
+ *      fails the comparison, canonical_log2(NaN) = -3e38 maps below 0); +inf lands in bin 255 (canonical_log2(+inf) = 3e38) for finite
+ *      settings with min < max; a finite lum with canonical_log2(lum) < min_exposure has mapped < 1 and lands in bin 0 (bin 1 at equality),
+ *      one with canonical_log2(lum) >= max_exposure has mapped >= 255 and lands in bin 255.  NaN settings send every pixel to bin 0.
+ *   3. average: weighted = sum over i of bins[i] * i mod 2^32 (the shader's u32 InterlockedAdd; it wraps once more than 16,843,009 pixels
+ *      fall in bin 255); avg = f32(weighted) / max(pixel_count - f32(bins[0]), 1) - 1; desired = exp2((avg / 254) * exposure_range +
+ *      min_exposure); adapted = last + (desired - last) * time_coeff; ev100 = canonical_log2(adapted * bias_scale); exposure = 1 /
+ *      (exp2(ev100) * 1.2) (0x3F99999A).  exp2(x) = canonical_pow(2, x) (binary64 inside, within 1 ulp, the same bits on the host and
+ *      the device).  The record receives (adapted, exposure). */
+typedef struct OxcEyeAdaptationSettings { /* GPU::EyeAdaptationSettings; the AutoExposureComponent defaults are -11.5, 18, 1.1, 1 */
+  float min_exposure;
+  float max_exposure;
+  float adaptation_speed;
+  float ev100_bias;
+} OxcEyeAdaptationSettings;
+OXC_STATIC_ASSERT(sizeof(OxcEyeAdaptationSettings) == 16, "EyeAdaptationSettings");
+typedef struct OxcExposure {              /* HistogramLuminance (passes/histogram.slang) */
+  float adapted_luminance;
+  float exposure;
+} OxcExposure;
+OXC_STATIC_ASSERT(sizeof(OxcExposure) == 8, "Exposure");
+#define OXC_HISTOGRAM_BIN_COUNT 256u
+int oxc_eye_adaptation(OxcContext* ctx, const float* frame_dev, uint32_t width, uint32_t height, const OxcEyeAdaptationSettings* settings,
+                       float delta_time, OxcExposure* exposure_dev, uint32_t* histogram_dev, void* stream);
+
+/* Bloom (PostProcess.cpp:79-203, passes/bloom_prefilter.slang, bloom_downsample.slang, bloom_upsample.slang): the prefilter of the frame
+ * into level 0 of the downsampled chain, the downsample chain, then the upsample chain; the bloom image the tonemap reads is level 0 of
+ * the upsampled chain.  Both chains hold levels 0..n-1 of the half extent, float4 texels, packed in level order, each row-major: level k
+ * is max(1, (width / 2) >> k) x max(1, (height / 2) >> k), n = the bit length of max(width / 2, height / 2) (Texture::calculate_mip_count,
+ * u32(log2f(m)) + 1; 10 levels at 1920 x 1080, 11 at 3840 x 2160); oxc_bloom_chain_texels gives the texels of one chain.  Level n-1 of
+ * the upsampled chain is never written, as in the reference, except for n = 1 (item 6).  The exposure record (oxc_eye_adaptation's) is
+ * read only under OXC_SCENE_HAS_EYE_ADAPTATION, where it is required; without it the exposure is 1 and exposure_dev may be NULL.  No
+ * scratch, so the call is graph-capturable from its first call.  Settings: the cvars bloom_threshold 1.0, bloom_soft_threshold 0.125,
+ * bloom_clamp 4.0, bloom_radius 0.75 by default; bloom_intensity belongs to the tonemap.
+ * Refused with OXC_E_INVALID, before anything is launched: what oxc_eye_adaptation refuses for the frame and the record; width or height
+ * below 2 (a zero half extent, an image the reference cannot create); NULL or misaligned (16-byte) targets; targets that share a byte
+ * with the frame, the record or each other.
+ * SPECIFICATION (oracle/oxc_oracle_post.c orc_bloom), binary32 rgb, every stored texel (rgb, 1):
+ *   1. taps: the atmosphere's item-5 bilinear rule on binary32 texels: x = u * W - 0.5, x0 = floor(x), wx = x - x0 (y likewise), texels
+ *      x0, x0 + 1 / y0, y0 + 1 with NaN-safe saturating indices, top = a00 + wx * (a10 - a00), bottom likewise, top + wy * (bottom - top).
+ *      The prefilter and the downsample read ClampToBorder with transparent black (a texel outside the level reads 0, LinearSamplerBorder);
+ *      the upsample reads ClampToEdge (LinearSamplerClamped).
+ *   2. texel t of a pass: uv = (f32(t) + 0.5) / f32(size), texel_size = 1 / f32(size), size the DESTINATION level's extent in all three
+ *      passes; an offset tap at uv + texel_size * (dx, dy), per component, the product first.
+ *   3. prefilter (level 0 of downsampled from the frame): the 13 taps a..m; groups (((a + b) + d) + e) * 0.25 * exposure, (b c e f),
+ *      (d e g h), (e f h i), (j k l m) likewise; group = min(group, clamp_value); weight = 1 / (1 + luminance(group)) with luminance's
+ *      0.299 / 0.587 / 0.114 (not the histogram's weights); prefilter: brightness = max(r, max(g, b)), knee = threshold * soft_threshold,
+ *      soft = clamp((brightness - threshold) + knee, 0, 2 * knee), soft = ((soft * soft) * 0.25) / (knee + 1e-5), contribution =
+ *      max(soft, brightness - threshold) / max(brightness, 1e-5), (group * contribution) * weight; color_sum and weight_sum add the five
+ *      groups in index order from 0; the texel is color_sum / (weight_sum + 1e-5).
+ *   4. downsample, for i = 1..n-1, level i - 1 into level i: ((a + c) + g) + i) * 0.03125 + (((b + d) + f) + h) * 0.0625 + ((((e + j) + k) +
+ *      l) + m) * 0.125.
+ *   5. upsample, for i = n-1..1, into upsampled level i - 1: the 9-tap tent (e * 0.25 + (((b + d) + f) + h) * 0.125) + (((a + c) + g) + i)
+ *      * 0.0625 at offsets -1..1 of downsampled level n-1 when i = n-1 and of upsampled level i otherwise; then lerp(tap(downsampled level
+ *      i - 1, uv), tent, radius).
+ *   6. n = 1 (width and height in 2..3): no upsample runs and the reference's output is its per-frame clear, vuk::Black<float>; the call
+ *      writes (0, 0, 0, 1).  vuk's sources are not part of the reference tree, so this value is a commitment, not read from the code. */
+typedef struct OxcBloomSettings {
+  float threshold;
+  float soft_threshold;
+  float clamp_value;
+  float radius;
+  uint32_t scene_flags; /* OXC_SCENE_*: only OXC_SCENE_HAS_EYE_ADAPTATION is read */
+} OxcBloomSettings;
+OXC_STATIC_ASSERT(sizeof(OxcBloomSettings) == 20, "BloomSettings");
+typedef struct OxcBloomTargets { /* float4 texels, 16-byte aligned, oxc_bloom_chain_texels each */
+  float* downsampled;
+  float* upsampled;
+} OxcBloomTargets;
+OXC_STATIC_ASSERT(sizeof(OxcBloomTargets) == 16, "BloomTargets");
+#define OXC_BLOOM_MAX_LEVELS 15u /* half extents up to 16384 */
+/* n, the level count of a width x height frame's chains (0 below 2 x 2), and the float4 texels of one chain (the sum of its level
+ * extents): the size helpers of the caller's targets */
+uint32_t oxc_bloom_level_count(uint32_t width, uint32_t height);
+uint64_t oxc_bloom_chain_texels(uint32_t width, uint32_t height);
+int oxc_bloom(OxcContext* ctx, const float* frame_dev, uint32_t width, uint32_t height, const OxcBloomSettings* settings,
+              const OxcExposure* exposure_dev, const OxcBloomTargets* targets, void* stream);
+
 int oxc_get_outputs(OxcContext* ctx, OxcOutputs* out);
 /* Instrumentation hook: 128 u64 counters that builds with -DOXC_RASTER_STATS fill (tools/raster_stats.py); zero otherwise. */
 void* oxc_debug_stats_ptr(OxcContext* ctx);
@@ -1373,6 +1472,18 @@ int oxr_atmosphere_luts(OxrRenderer* r, const OxcAtmosphere* atmosphere, const O
  * planes cannot be allocated; a failed call does not advance the count. */
 int oxr_atmosphere_sky_ibl(OxrRenderer* r, const OxcAtmosphere* atmosphere, const OxcPbrCamera* camera, const float sun_direction[3],
                            float sun_intensity, uint16_t* cube_host);
+/* Eye adaptation (PostProcess.cpp:7-77) on the lit plane of the renderer's last oxr_apply_pbr* call, on the renderer's stream,
+ * synchronous: oxc_eye_adaptation into the renderer's exposure record and histogram.  The first call allocates both and fills the record
+ * with (1, 1), as the reference's vuk::fill does; the record persists across calls.  exposure_host (may be NULL) receives the record
+ * after the call.  OXC_E_INVALID before any oxr_apply_pbr* call; OXC_E_CAPACITY, with the camera path left usable, when the record cannot
+ * be allocated.  The frame's outputs and the lit plane are left as they were. */
+int oxr_eye_adaptation(OxrRenderer* r, const OxcEyeAdaptationSettings* settings, float delta_time, OxcExposure* exposure_host);
+/* Bloom (PostProcess.cpp:79-203) of the same lit plane, on the renderer's stream, synchronous: oxc_bloom into the renderer's two chains
+ * (allocated at the first call), reading the renderer's exposure record under OXC_SCENE_HAS_EYE_ADAPTATION (OXC_E_STATE before an
+ * oxr_eye_adaptation then).  bloom_host (may be NULL) receives upsampled level 0, (width / 2) x (height / 2) float4.  OXC_E_INVALID before
+ * any oxr_apply_pbr* call or for a frame below 2 x 2; OXC_E_CAPACITY, with the camera path left usable, when the chains cannot be
+ * allocated.  The frame's outputs and the lit plane are left as they were. */
+int oxr_bloom(OxrRenderer* r, const OxcBloomSettings* settings, float* bloom_host);
 
 /* ------------------------------------------------------------------------------------------------
  * oxb_* — mesh builder (SURVEY §8f.2): host-side producer of the blob layout above, mirroring build_gltf_mesh

@@ -511,6 +511,58 @@ SKY_IBL_CUBE_BYTES = 6 * SKY_IBL_CUBE_RES * SKY_IBL_CUBE_RES * 8
 SKY_IBL_SUN_AMBIENT_STRENGTH = 0.15
 
 
+class EyeAdaptationSettings(C.Structure):
+    """OxcEyeAdaptationSettings (GPU::EyeAdaptationSettings)"""
+    _fields_ = [("min_exposure", C.c_float), ("max_exposure", C.c_float), ("adaptation_speed", C.c_float), ("ev100_bias", C.c_float)]
+
+
+class Exposure(C.Structure):
+    """OxcExposure: the persistent exposure record (HistogramLuminance), 8 B"""
+    _fields_ = [("adapted_luminance", C.c_float), ("exposure", C.c_float)]
+
+
+class BloomSettings(C.Structure):
+    """OxcBloomSettings: the bloom cvars the passes read and the scene flags (only HasEyeAdaptation is read)"""
+    _fields_ = [("threshold", C.c_float), ("soft_threshold", C.c_float), ("clamp_value", C.c_float), ("radius", C.c_float),
+                ("scene_flags", C.c_uint32)]
+
+
+class BloomTargets(C.Structure):
+    """OxcBloomTargets: the two chains (device pointers, float4 texels, 16-byte aligned)"""
+    _fields_ = [("downsampled", C.c_void_p), ("upsampled", C.c_void_p)]
+
+
+assert C.sizeof(EyeAdaptationSettings) == 16 and C.sizeof(Exposure) == 8 and C.sizeof(BloomSettings) == 20 and C.sizeof(BloomTargets) == 16
+HISTOGRAM_BIN_COUNT = 256
+BLOOM_MAX_LEVELS = 15
+
+
+def eye_adaptation_settings(min_exposure=-11.5, max_exposure=18.0, adaptation_speed=1.1, ev100_bias=1.0):
+    """EyeAdaptationSettings with the AutoExposureComponent defaults"""
+    return EyeAdaptationSettings(*[float(np.float32(v)) for v in (min_exposure, max_exposure, adaptation_speed, ev100_bias)])
+
+
+def bloom_settings(threshold=1.0, soft_threshold=0.125, clamp_value=4.0, radius=0.75, scene_flags=0):
+    """BloomSettings with the reference's cvar defaults (bloom_threshold, bloom_soft_threshold, bloom_clamp, bloom_radius)"""
+    return BloomSettings(*[float(np.float32(v)) for v in (threshold, soft_threshold, clamp_value, radius)], int(scene_flags))
+
+
+def bloom_levels(width: int, height: int):
+    """[(w, h, first texel)] of the levels of a width x height frame's bloom chains (oxc_bloom's layout)"""
+    w, h = width // 2, height // 2
+    out, off = [], 0
+    for k in range(max(w, h).bit_length()):
+        lw, lh = max(1, w >> k), max(1, h >> k)
+        out.append((lw, lh, off))
+        off += lw * lh
+    return out
+
+
+def bloom_chain_texels(width: int, height: int) -> int:
+    """float4 texels of one bloom chain (oxc_bloom_chain_texels)"""
+    return sum(w * h for w, h, _ in bloom_levels(width, height))
+
+
 def atmosphere(**overrides):
     """Atmosphere with the GPU::Atmosphere{} defaults and the reference's LUT sizes; any field may be overridden by name"""
     a = Atmosphere()

@@ -23,6 +23,7 @@ SYMBOLS = [
     "oxc_vsm_begin_frame", "oxc_vsm_invalidate_pages", "oxc_vsm_allocate_pages", "oxc_vsm_clear_dirty_pages", "oxc_cull_meshlets_hpb_dirty_dev",
     "oxc_vsm_draw_pages", "oxc_vsm_draw_stats", "oxc_vsm_resolve_shadows", "oxc_generate_ambient_occlusion", "oxc_apply_pbr",
     "oxc_contact_shadows", "oxc_atmosphere_transmittance", "oxc_atmosphere_sky_luts", "oxc_atmosphere_sky_ibl", "oxc_apply_pbr_atmosphere", "oxr_apply_pbr_atmosphere",
+    "oxc_eye_adaptation", "oxc_bloom", "oxc_bloom_level_count", "oxc_bloom_chain_texels", "oxr_eye_adaptation", "oxr_bloom",
     "oxc_get_outputs", "oxc_check_status", "oxc_mark_hiz_dirty", "oxc_bind_camera_buffer", "oxc_load_camera", "oxc_debug_stats_ptr",
     "oxc_mgpu_get_unique_id", "oxc_mgpu_init", "oxc_mgpu_init_with_comm", "oxc_mgpu_shutdown", "oxc_mgpu_info", "oxc_mgpu_exchange_hiz",
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
@@ -166,6 +167,12 @@ def load(build_if_missing=True):
                                              C.c_int, vp, vp, vp, vp, vp]
     lib.oxc_apply_pbr_atmosphere.argtypes = [vp, C.POINTER(abi.PbrCamera), C.POINTER(abi.PbrSettings), C.POINTER(abi.Atmosphere), vp,
                                              C.POINTER(abi.PbrInputs), C.POINTER(abi.PbrSky), u32, u32, vp, vp]
+    lib.oxc_eye_adaptation.argtypes = [vp, vp, u32, u32, C.POINTER(abi.EyeAdaptationSettings), C.c_float, vp, vp, vp]
+    lib.oxc_bloom.argtypes = [vp, vp, u32, u32, C.POINTER(abi.BloomSettings), vp, C.POINTER(abi.BloomTargets), vp]
+    lib.oxr_eye_adaptation.argtypes = [vp, C.POINTER(abi.EyeAdaptationSettings), C.c_float, C.POINTER(abi.Exposure)]
+    lib.oxr_bloom.argtypes = [vp, C.POINTER(abi.BloomSettings), vp]
+    lib.oxc_bloom_level_count.restype, lib.oxc_bloom_level_count.argtypes = u32, [u32, u32]
+    lib.oxc_bloom_chain_texels.restype, lib.oxc_bloom_chain_texels.argtypes = C.c_uint64, [u32, u32]
     _LIB = lib
     return lib
 
@@ -529,6 +536,19 @@ class Context:
         _check(self.lib.oxc_apply_pbr_atmosphere(self.h, C.byref(pbr_camera), C.byref(settings), C.byref(atmosphere), _ptr(lights_dev),
                                                  C.byref(t), C.byref(k), w, h, _ptr(out_dev), self.stream), "oxc_apply_pbr_atmosphere")
 
+    def eye_adaptation(self, frame_dev, w, h, settings, delta_time, exposure_dev, histogram_dev):
+        """oxc_eye_adaptation: the 256-bin luminance histogram of a w x h float4 frame into histogram_dev (zeroed by the call) and the
+        exposure record (abi.Exposure, 8 B at exposure_dev) updated in place.  settings: abi.EyeAdaptationSettings"""
+        _check(self.lib.oxc_eye_adaptation(self.h, _ptr(frame_dev), w, h, C.byref(settings), float(np.float32(delta_time)), _ptr(exposure_dev),
+                                           _ptr(histogram_dev), self.stream), "oxc_eye_adaptation")
+
+    def bloom(self, frame_dev, w, h, settings, exposure_dev, downsampled_dev, upsampled_dev):
+        """oxc_bloom: the prefilter, downsample and upsample chains of a w x h float4 frame into the two chains (abi.bloom_levels layout,
+        abi.bloom_chain_texels float4 each); the bloom image is upsampled level 0.  settings: abi.BloomSettings; exposure_dev is read
+        under SCENE_HAS_EYE_ADAPTATION only"""
+        t = abi.BloomTargets(*[None if a is None else int(a) for a in (downsampled_dev, upsampled_dev)])
+        _check(self.lib.oxc_bloom(self.h, _ptr(frame_dev), w, h, C.byref(settings), _ptr(exposure_dev), C.byref(t), self.stream), "oxc_bloom")
+
     def atmosphere_transmittance(self, atmosphere, lut_dev):
         """oxc_atmosphere_transmittance: the transmittance LUT (binary16 RGBA, atmosphere.transmittance_lut_size) into lut_dev"""
         _check(self.lib.oxc_atmosphere_transmittance(self.h, C.byref(atmosphere), _ptr(lut_dev), self.stream), "oxc_atmosphere_transmittance")
@@ -859,6 +879,20 @@ class Renderer:
                                                  C.cast(lights, C.c_void_p) if n else None, int(bool(cast_shadows)), opt(gtao_camera),
                                                  opt(gtao_settings), opt(contact_camera), opt(contact_settings), _ptr(out)),
                "oxr_apply_pbr_atmosphere")
+        return out
+
+    def eye_adaptation(self, settings, delta_time):
+        """oxr_eye_adaptation: eye adaptation on the lit plane of the last apply_pbr* call, into the renderer's persistent exposure record
+        ((1, 1) at the first call); returns the record after the call (abi.Exposure)"""
+        rec = abi.Exposure()
+        _check(self.lib.oxr_eye_adaptation(self.h, C.byref(settings), float(np.float32(delta_time)), C.byref(rec)), "oxr_eye_adaptation")
+        return rec
+
+    def bloom(self, settings):
+        """oxr_bloom: the bloom image (upsampled level 0, float32 [height // 2, width // 2, 4]) of the lit plane of the last apply_pbr* call,
+        with the renderer's exposure record under SCENE_HAS_EYE_ADAPTATION"""
+        out = np.zeros((self.scene.height // 2, self.scene.width // 2, 4), dtype=np.float32)
+        _check(self.lib.oxr_bloom(self.h, C.byref(settings), _ptr(out)), "oxr_bloom")
         return out
 
     def apply_pbr(self, cam, settings, lights=None, cast_shadows=False, gtao_camera=None, gtao_settings=None, pbr_camera=None,

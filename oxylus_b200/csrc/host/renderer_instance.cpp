@@ -103,6 +103,7 @@ RendererInstance::~RendererInstance() {
   if (stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(stream_));
   cudaFree(d_vis64_); cudaFree(d_vis32_); cudaFree(d_depth_); cudaFree(d_occluder_); cudaFree(d_overdraw_); cudaFree(d_gbuffer_);
   cudaFree(d_uv_normal_); cudaFree(d_gtao_); cudaFree(d_pbr_); cudaFree(d_lights_); cudaFree(d_contact_); cudaFree(d_atmosphere_); cudaFree(d_sky_ibl_cube_);
+  cudaFree(d_post_); cudaFree(d_bloom_);
   if (h_pinned_) cudaFreeHost(h_pinned_);
   if (copy_stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(copy_stream_));
   for (auto& sl : slots_) {
@@ -513,6 +514,54 @@ auto RendererInstance::apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera
   }
   if (rc != OXC_OK) return fail(rc);
   if (cudaMemcpyAsync(rgba_host, d_pbr_, px * 16, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
+    return fail(OXC_E_CUDA);
+  pbr_lit_ = true;
+  return OXC_OK;
+}
+
+// eye adaptation on stream_, synchronous: the histogram and the record are allocated at the first call, the record filled with 1.0
+auto RendererInstance::eye_adaptation(const OxcEyeAdaptationSettings& settings, float delta_time, OxcExposure* exposure_host) -> int {
+  if (!ctx_ || !error_.empty()) return OXC_E_STATE;
+  if (!pbr_lit_) return OXC_E_INVALID; // no lit plane yet
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  const bool first = !d_post_;
+  if (first && cudaMalloc(reinterpret_cast<void**>(&d_post_), OXC_HISTOGRAM_BIN_COUNT * 4 + sizeof(OxcExposure)) != cudaSuccess) {
+    cudaGetLastError();
+    d_post_ = nullptr;
+    return OXC_E_CAPACITY; // an optional part: the camera path stays usable
+  }
+  OxcExposure* record = reinterpret_cast<OxcExposure*>(d_post_ + OXC_HISTOGRAM_BIN_COUNT);
+  const OxcExposure one{1.0f, 1.0f};
+  if (first && (cudaMemcpyAsync(record, &one, sizeof one, cudaMemcpyHostToDevice, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess))
+    return fail(OXC_E_CUDA);
+  int rc;
+  if ((rc = oxc_eye_adaptation(ctx_, d_pbr_, width_, height_, &settings, delta_time, record, d_post_, stream_)) != OXC_OK) return fail(rc);
+  if ((exposure_host && cudaMemcpyAsync(exposure_host, record, sizeof(OxcExposure), cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
+      cudaStreamSynchronize(s) != cudaSuccess)
+    return fail(OXC_E_CUDA);
+  return OXC_OK;
+}
+
+// bloom on stream_, synchronous: the two chains are allocated at the first call
+auto RendererInstance::bloom(const OxcBloomSettings& settings, float* bloom_host) -> int {
+  if (!ctx_ || !error_.empty()) return OXC_E_STATE;
+  if (!pbr_lit_ || width_ < 2 || height_ < 2) return OXC_E_INVALID;
+  const bool adapt = (settings.scene_flags & OXC_SCENE_HAS_EYE_ADAPTATION) != 0;
+  if (adapt && !d_post_) return OXC_E_STATE; // no exposure record before an eye_adaptation
+  const uint64_t texels = oxc_bloom_chain_texels(width_, height_);
+  if (!d_bloom_ && cudaMalloc(reinterpret_cast<void**>(&d_bloom_), texels * 32) != cudaSuccess) {
+    cudaGetLastError();
+    d_bloom_ = nullptr;
+    return OXC_E_CAPACITY; // an optional part: the camera path stays usable
+  }
+  const OxcBloomTargets targets{d_bloom_, d_bloom_ + texels * 4};
+  const OxcExposure* record = adapt ? reinterpret_cast<const OxcExposure*>(d_post_ + OXC_HISTOGRAM_BIN_COUNT) : nullptr;
+  int rc;
+  if ((rc = oxc_bloom(ctx_, d_pbr_, width_, height_, &settings, record, &targets, stream_)) != OXC_OK) return fail(rc);
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  if ((bloom_host && cudaMemcpyAsync(bloom_host, targets.upsampled, (size_t)(width_ / 2) * (height_ / 2) * 16, cudaMemcpyDeviceToHost, s) !=
+                         cudaSuccess) ||
+      cudaStreamSynchronize(s) != cudaSuccess)
     return fail(OXC_E_CUDA);
   return OXC_OK;
 }
@@ -1174,6 +1223,16 @@ int oxr_atmosphere_sky_ibl(OxrRenderer* r, const OxcAtmosphere* atmosphere, cons
                            float sun_intensity, uint16_t* cube_host) {
   if (!r || !atmosphere || !camera || !sun_direction) return OXC_E_INVALID;
   return r->impl.atmosphere_sky_ibl(*atmosphere, *camera, sun_direction, sun_intensity, cube_host);
+}
+
+int oxr_eye_adaptation(OxrRenderer* r, const OxcEyeAdaptationSettings* settings, float delta_time, OxcExposure* exposure_host) {
+  if (!r || !settings) return OXC_E_INVALID;
+  return r->impl.eye_adaptation(*settings, delta_time, exposure_host);
+}
+
+int oxr_bloom(OxrRenderer* r, const OxcBloomSettings* settings, float* bloom_host) {
+  if (!r || !settings) return OXC_E_INVALID;
+  return r->impl.bloom(*settings, bloom_host);
 }
 
 int oxr_contact_shadows(OxrRenderer* r, const OxcContactShadowCamera* contact_camera, const OxcContactShadowSettings* settings,

@@ -31,6 +31,8 @@
 #include "kernels_atmosphere.cuh"
 #include "kernels_sky_ibl.cuh"
 #include "kernels_pbr_atmosphere.cuh"
+#include "kernels_exposure.cuh"
+#include "kernels_bloom.cuh"
 
 using namespace oxc;
 
@@ -1654,6 +1656,82 @@ int oxc_apply_pbr_atmosphere(OxcContext* c, const OxcPbrCamera* cam, const OxcPb
   const dim3 grid((w + PBR_TILE_X - 1) / PBR_TILE_X, (h + PBR_TILE_Y - 1) / PBR_TILE_Y);
   k_apply_pbr_atmosphere<<<grid, PBR_THREADS, 0, s>>>(p);
   LAUNCHED();
+  return OXC_OK;
+}
+
+// [a, a + na) and [b, b + nb) share a byte
+static bool overlaps(const void* a, uint64_t na, const void* b, uint64_t nb) {
+  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+  return x < y + nb && y < x + na;
+}
+
+// the frame checks both post-processing calls make
+static int post_check_frame(const float* frame_dev, uint32_t w, uint32_t h) {
+  if (w == 0 || h == 0) return fail(OXC_E_INVALID, "empty extent %u x %u", w, h);
+  if (w > 32768u || h > 32768u) return fail(OXC_E_INVALID, "extent %u x %u above 32768", w, h);
+  if (reinterpret_cast<uintptr_t>(frame_dev) & 15u) return fail(OXC_E_INVALID, "frame_dev must be 16-byte aligned");
+  return OXC_OK;
+}
+
+int oxc_eye_adaptation(OxcContext* c, const float* frame_dev, uint32_t w, uint32_t h, const OxcEyeAdaptationSettings* settings, float delta_time,
+                       OxcExposure* exposure_dev, uint32_t* histogram_dev, void* stream) {
+  if (!c || !frame_dev || !settings || !exposure_dev || !histogram_dev) return fail(OXC_E_INVALID, "null argument");
+  int rc;
+  if ((rc = post_check_frame(frame_dev, w, h)) != OXC_OK) return rc;
+  if (reinterpret_cast<uintptr_t>(exposure_dev) & 7u) return fail(OXC_E_INVALID, "exposure_dev must be 8-byte aligned");
+  if (reinterpret_cast<uintptr_t>(histogram_dev) & 3u) return fail(OXC_E_INVALID, "histogram_dev must be 4-byte aligned");
+  const uint64_t frame_bytes = (uint64_t)w * h * 16, hist_bytes = OXC_HISTOGRAM_BIN_COUNT * 4;
+  if (overlaps(histogram_dev, hist_bytes, frame_dev, frame_bytes) || overlaps(exposure_dev, 8, frame_dev, frame_bytes) ||
+      overlaps(exposure_dev, 8, histogram_dev, hist_bytes))
+    return fail(OXC_E_INVALID, "histogram_dev, exposure_dev and frame_dev overlap");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  const EyeAdaptationParams p = eye_adaptation_make_params(frame_dev, w, h, *settings, delta_time, exposure_dev, histogram_dev);
+  CK(cudaMemsetAsync(histogram_dev, 0, hist_bytes, s));
+  const uint64_t ctas = std::min((p.pixels + HISTOGRAM_THREADS - 1) / HISTOGRAM_THREADS, (uint64_t)c->sm_count * HISTOGRAM_CTAS_PER_SM);
+  k_histogram<<<(unsigned)ctas, HISTOGRAM_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  k_exposure_average<<<1, HISTOGRAM_BINS, 0, s>>>(p);
+  LAUNCHED();
+  return OXC_OK;
+}
+
+uint32_t oxc_bloom_level_count(uint32_t width, uint32_t height) { return (uint32_t)bloom_level_count(width, height); }
+uint64_t oxc_bloom_chain_texels(uint32_t width, uint32_t height) { return bloom_chain_texels(width, height); }
+
+int oxc_bloom(OxcContext* c, const float* frame_dev, uint32_t w, uint32_t h, const OxcBloomSettings* settings, const OxcExposure* exposure_dev,
+              const OxcBloomTargets* targets, void* stream) {
+  if (!c || !frame_dev || !settings || !targets || !targets->downsampled || !targets->upsampled) return fail(OXC_E_INVALID, "null argument");
+  const bool adapt = (settings->scene_flags & OXC_SCENE_HAS_EYE_ADAPTATION) != 0;
+  if (adapt && !exposure_dev) return fail(OXC_E_INVALID, "null argument: HasEyeAdaptation reads exposure_dev");
+  int rc;
+  if ((rc = post_check_frame(frame_dev, w, h)) != OXC_OK) return rc;
+  if (w < 2 || h < 2) return fail(OXC_E_INVALID, "extent %u x %u below 2 x 2: the half extent is empty", w, h);
+  if (adapt && (reinterpret_cast<uintptr_t>(exposure_dev) & 7u)) return fail(OXC_E_INVALID, "exposure_dev must be 8-byte aligned");
+  if ((reinterpret_cast<uintptr_t>(targets->downsampled) | reinterpret_cast<uintptr_t>(targets->upsampled)) & 15u)
+    return fail(OXC_E_INVALID, "targets must be 16-byte aligned");
+  const uint64_t frame_bytes = (uint64_t)w * h * 16, chain_bytes = bloom_chain_texels(w, h) * 16;
+  const float *down = targets->downsampled, *up = targets->upsampled;
+  if (overlaps(down, chain_bytes, frame_dev, frame_bytes) || overlaps(up, chain_bytes, frame_dev, frame_bytes) ||
+      overlaps(down, chain_bytes, up, chain_bytes) ||
+      (adapt && (overlaps(down, chain_bytes, exposure_dev, 8) || overlaps(up, chain_bytes, exposure_dev, 8))))
+    return fail(OXC_E_INVALID, "targets overlap each other, frame_dev or exposure_dev");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  const BloomParams p = bloom_make_params(frame_dev, w, h, *settings, exposure_dev, *targets);
+  const int tail = bloom_tail_level(p);
+  k_bloom_prefilter<<<bloom_grid(p, 0), BLOOM_THREADS, 0, s>>>(p);
+  LAUNCHED();
+  for (int i = 1; i < tail; i++) {
+    k_bloom_downsample<<<bloom_grid(p, i), BLOOM_THREADS, 0, s>>>(p, i);
+    LAUNCHED();
+  }
+  k_bloom_tail<<<1, BLOOM_TAIL_THREADS, 0, s>>>(p, tail);
+  LAUNCHED();
+  for (int i = tail; i >= 1; i--) {
+    k_bloom_upsample<<<bloom_grid(p, i - 1), BLOOM_THREADS, 0, s>>>(p, i);
+    LAUNCHED();
+  }
   return OXC_OK;
 }
 
