@@ -37,11 +37,53 @@ struct Readback {
   uint32_t draw_index_count[2];
   unsigned long long raster_triangles;
 };
+
+// the atmosphere's LUTs at the reference's extents (RendererInstance.hpp: 256 x 64, 312 x 192, 32 x 32 x 32), binary16 RGBA
+constexpr uint32_t kTransmittanceLut[2] = {256, 64}, kSkyViewLut[2] = {312, 192}, kMultiscatteringLut[2] = {32, 32}, kAerialLut[3] = {32, 32, 32};
+constexpr size_t kTransmittanceTexels = (size_t)kTransmittanceLut[0] * kTransmittanceLut[1], kSkyViewTexels = (size_t)kSkyViewLut[0] * kSkyViewLut[1],
+                 kAerialTexels = (size_t)kAerialLut[0] * kAerialLut[1] * kAerialLut[2];
+
+// the three LUTs of the renderer's atmosphere block, in this order
+struct AtmosphereLuts {
+  uint16_t *transmittance, *sky_view, *aerial_perspective;
+};
+AtmosphereLuts lut_planes(uint16_t* block) {
+  return {block, block + kTransmittanceTexels * 4, block + (kTransmittanceTexels + kSkyViewTexels) * 4};
+}
+
+// the caller's record with the sizes of those LUTs
+OxcAtmosphere sized_atmosphere(const OxcAtmosphere& atmosphere) {
+  OxcAtmosphere sized = atmosphere;
+  for (int i = 0; i < 3; i++) {
+    sized.transmittance_lut_size[i] = i < 2 ? kTransmittanceLut[i] : 1; sized.sky_view_lut_size[i] = i < 2 ? kSkyViewLut[i] : 1;
+    sized.multiscattering_lut_size[i] = i < 2 ? kMultiscatteringLut[i] : 1; sized.aerial_perspective_lut_size[i] = kAerialLut[i];
+  }
+  return sized;
+}
 } // namespace
 
 int RendererInstance::fail(int rc) {
   if (rc != OXC_OK && error_.empty()) error_ = oxc_last_error();
   return rc;
+}
+
+template <typename T>
+int RendererInstance::optional_plane(T** p, size_t bytes) {
+  if (*p) return OXC_OK;
+  if (cudaMalloc(reinterpret_cast<void**>(p), bytes) != cudaSuccess) {
+    cudaGetLastError(); // clear the allocation error so that the next launch check does not report it
+    *p = nullptr;
+    return OXC_E_CAPACITY;
+  }
+  return OXC_OK;
+}
+
+int RendererInstance::copy_to_host(std::initializer_list<HostCopy> copies) {
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  for (const HostCopy& c : copies)
+    if (c.host && cudaMemcpyAsync(c.host, c.dev, c.bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess) return fail(OXC_E_CUDA);
+  if (cudaStreamSynchronize(s) != cudaSuccess) return fail(OXC_E_CUDA);
+  return OXC_OK;
 }
 
 RendererInstance::RendererInstance(int device, const OxcCreateInfo& info, uint32_t width, uint32_t height)
@@ -293,30 +335,16 @@ auto RendererInstance::resolve_shadowmap(const OxcCullCamera& camera, float* sha
   if (!ctx_ || !error_.empty()) return OXC_E_STATE;
   if (!shadow_host) return OXC_E_INVALID;
   if (!vsm_.updated) return OXC_E_STATE;
-  cudaStream_t s = static_cast<cudaStream_t>(stream_);
   const size_t px = (size_t)width_ * height_;
-  // the resolve's own planes are an optional part, as the shadow draw's context is: without room for them the camera path stays
-  // usable and this call returns OXC_E_CAPACITY (the sticky error is not set)
-  if (uv_normal_plane() != OXC_OK || shadow_plane() != OXC_OK) return OXC_E_CAPACITY;
+  // the resolve's own planes are an optional part, as the shadow draw's context is
+  if (optional_plane(&d_uv_normal_, px * 16) != OXC_OK || optional_plane(&vsm_.d_shadow, px * 4) != OXC_OK) return OXC_E_CAPACITY;
   int rc;
   if ((rc = oxc_bind_camera_buffer(ctx_, nullptr)) != OXC_OK) return fail(rc); // as render(): the camera comes from the argument
   OxcDecodeTargets targets{};
   targets.uv_normal = d_uv_normal_;
   if ((rc = oxc_decode_visbuffer(ctx_, &camera, d_vis64_, nullptr, width_, height_, &targets, stream_)) != OXC_OK) return fail(rc);
   if ((rc = resolve_shadowmap_device(d_uv_normal_)) != OXC_OK) return rc;
-  if (cudaMemcpyAsync(shadow_host, vsm_.d_shadow, px * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
-    return fail(OXC_E_CUDA);
-  return OXC_OK;
-}
-
-int RendererInstance::shadow_plane() {
-  if (vsm_.d_shadow) return OXC_OK;
-  if (cudaMalloc(reinterpret_cast<void**>(&vsm_.d_shadow), (size_t)width_ * height_ * 4) != cudaSuccess) {
-    cudaGetLastError(); // clear the allocation error so that the next launch check does not report it
-    vsm_.d_shadow = nullptr;
-    return OXC_E_CAPACITY;
-  }
-  return OXC_OK;
+  return copy_to_host({{shadow_host, vsm_.d_shadow, px * 4}});
 }
 
 // the frame's depth, then the fullscreen resolve into vsm_.d_shadow with the VSM state of the last update, from `normals` (float4 per
@@ -335,30 +363,16 @@ int RendererInstance::resolve_shadowmap_device(const float* normals) {
 auto RendererInstance::decode_visbuffer(const OxcCullCamera& camera, float* albedo_host, float* normal_host, float* emissive_host, float* mro_host)
     -> int {
   if (!ctx_ || !error_.empty()) return OXC_E_STATE;
-  cudaStream_t s = static_cast<cudaStream_t>(stream_);
   const size_t px = (size_t)width_ * height_;
-  // the planes are an optional part, as the resolve's are: without room for them the camera path stays usable
-  if (gbuffer_planes() != OXC_OK) return OXC_E_CAPACITY;
+  if (optional_plane(&d_gbuffer_, px * 64) != OXC_OK) return OXC_E_CAPACITY;
   float* const host[4] = {albedo_host, normal_host, emissive_host, mro_host};
   OxcGBufferTargets targets{};
   float** const dev[4] = {&targets.albedo, &targets.normal, &targets.emissive, &targets.metallic_roughness_occlusion};
   for (int k = 0; k < 4; k++) *dev[k] = host[k] ? d_gbuffer_ + (size_t)k * px * 4 : nullptr;
   const int rc = decode_gbuffer_device(camera, targets);
   if (rc != OXC_OK) return rc;
-  for (int k = 0; k < 4; k++)
-    if (host[k] && cudaMemcpyAsync(host[k], *dev[k], px * 16, cudaMemcpyDeviceToHost, s) != cudaSuccess) return fail(OXC_E_CUDA);
-  if (cudaStreamSynchronize(s) != cudaSuccess) return fail(OXC_E_CUDA);
-  return OXC_OK;
-}
-
-int RendererInstance::gbuffer_planes() {
-  if (d_gbuffer_) return OXC_OK;
-  if (cudaMalloc(reinterpret_cast<void**>(&d_gbuffer_), (size_t)width_ * height_ * 64) != cudaSuccess) {
-    cudaGetLastError(); // clear the allocation error so that the next launch check does not report it
-    d_gbuffer_ = nullptr;
-    return OXC_E_CAPACITY;
-  }
-  return OXC_OK;
+  return copy_to_host({{albedo_host, targets.albedo, px * 16}, {normal_host, targets.normal, px * 16}, {emissive_host, targets.emissive, px * 16},
+                       {mro_host, targets.metallic_roughness_occlusion, px * 16}});
 }
 
 // the cleared attachments, then the G-buffer decode of the last frame into `targets` (planes of d_gbuffer_), enqueued on stream_
@@ -373,26 +387,15 @@ int RendererInstance::decode_gbuffer_device(const OxcCullCamera& camera, const O
   return OXC_OK;
 }
 
-int RendererInstance::uv_normal_plane() {
-  if (d_uv_normal_) return OXC_OK;
-  if (cudaMalloc(reinterpret_cast<void**>(&d_uv_normal_), (size_t)width_ * height_ * 16) != cudaSuccess) {
-    cudaGetLastError(); // clear the allocation error so that the next launch check does not report it
-    d_uv_normal_ = nullptr;
-    return OXC_E_CAPACITY;
-  }
-  return OXC_OK;
-}
-
 // PBR.cpp:143-311 generate_ambient_occlusion on stream_, synchronous: the vis decode's normals of the last frame (the reference's
 // normal_attachment .zw), its depth, then prefilter, sector pass and denoise into the renderer's own planes
 auto RendererInstance::generate_ambient_occlusion(const OxcCullCamera& camera, const OxcGtaoCamera& gtao_camera, const OxcGtaoSettings& settings,
                                                   float* ao_host) -> int {
   if (!ctx_ || !error_.empty()) return OXC_E_STATE;
   if (!ao_host) return OXC_E_INVALID;
-  cudaStream_t s = static_cast<cudaStream_t>(stream_);
   const size_t px = (size_t)width_ * height_;
-  // the planes are an optional part, as the resolve's are: without room for them the camera path stays usable
-  if (uv_normal_plane() != OXC_OK || gtao_planes() != OXC_OK) return OXC_E_CAPACITY;
+  if (optional_plane(&d_uv_normal_, px * 16) != OXC_OK || optional_plane(&d_gtao_, gtao_mip_texels() * 4 + px * 10) != OXC_OK)
+    return OXC_E_CAPACITY;
   int rc;
   if ((rc = oxc_bind_camera_buffer(ctx_, nullptr)) != OXC_OK) return fail(rc); // as render(): the camera comes from the argument
   OxcDecodeTargets decode{};
@@ -400,25 +403,13 @@ auto RendererInstance::generate_ambient_occlusion(const OxcCullCamera& camera, c
   if ((rc = oxc_decode_visbuffer(ctx_, &camera, d_vis64_, nullptr, width_, height_, &decode, stream_)) != OXC_OK) return fail(rc);
   OxcGtaoTargets targets;
   if ((rc = generate_ambient_occlusion_device(gtao_camera, settings, d_uv_normal_, &targets)) != OXC_OK) return rc;
-  if (cudaMemcpyAsync(ao_host, targets.ambient_occlusion, px * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
-    return fail(OXC_E_CUDA);
-  return OXC_OK;
+  return copy_to_host({{ao_host, targets.ambient_occlusion, px * 4}});
 }
 
 size_t RendererInstance::gtao_mip_texels() const {
   size_t mip_texels = 0;
   for (uint32_t k = 0; k < 5; k++) mip_texels += (size_t)std::max(1u, width_ >> k) * std::max(1u, height_ >> k);
   return mip_texels;
-}
-
-int RendererInstance::gtao_planes() {
-  if (d_gtao_) return OXC_OK;
-  if (cudaMalloc(&d_gtao_, gtao_mip_texels() * 4 + (size_t)width_ * height_ * 10) != cudaSuccess) {
-    cudaGetLastError();
-    d_gtao_ = nullptr;
-    return OXC_E_CAPACITY;
-  }
-  return OXC_OK;
 }
 
 // the frame's depth, then prefilter, sector pass and denoise into the renderer's own planes from `normals` (float4 per pixel, oct(world
@@ -462,26 +453,17 @@ auto RendererInstance::apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera
   if (cast_shadows && !vsm_.updated) return OXC_E_STATE;
   cudaStream_t s = static_cast<cudaStream_t>(stream_);
   const size_t px = (size_t)width_ * height_;
-  // the planes are an optional part, as the other passes' are: without room for them the camera path stays usable
-  if (gbuffer_planes() != OXC_OK || (cast_shadows && shadow_plane() != OXC_OK) || (gtao && gtao_planes() != OXC_OK) ||
-      (contact && contact_plane() != OXC_OK))
+  if (optional_plane(&d_gbuffer_, px * 64) != OXC_OK || (cast_shadows && optional_plane(&vsm_.d_shadow, px * 4) != OXC_OK) ||
+      (gtao && optional_plane(&d_gtao_, gtao_mip_texels() * 4 + px * 10) != OXC_OK) || (contact && optional_plane(&d_contact_, px * 4) != OXC_OK))
     return OXC_E_CAPACITY;
-  if (!d_pbr_ && (cudaMalloc(reinterpret_cast<void**>(&d_pbr_), px * 16) != cudaSuccess ||
-                  cudaMalloc(reinterpret_cast<void**>(&d_lights_), OXC_MAX_LIGHTS * sizeof(OxcLight)) != cudaSuccess)) {
-    cudaGetLastError();
+  // the output plane and the lights buffer: both or neither
+  if (optional_plane(&d_pbr_, px * 16) != OXC_OK || optional_plane(&d_lights_, OXC_MAX_LIGHTS * sizeof(OxcLight)) != OXC_OK) {
     cudaFree(d_pbr_); d_pbr_ = nullptr;
     return OXC_E_CAPACITY;
   }
   int rc;
-  OxcAtmosphere sized{};
-  if (atmosphere) { // RendererInstance.cpp:1022: the per-frame LUTs and the cube update before the geometry's lighting chain
-    if ((rc = sky_ibl_device(*atmosphere, pbr_camera, settings.sun_direction, settings.sun_intensity)) != OXC_OK) return rc;
-    sized = *atmosphere;
-    for (int i = 0; i < 3; i++) {
-      sized.transmittance_lut_size[i] = i < 2 ? kTransmittanceLut[i] : 1; sized.sky_view_lut_size[i] = i < 2 ? kSkyViewLut[i] : 1;
-      sized.multiscattering_lut_size[i] = i < 2 ? kMultiscatteringLut[i] : 1; sized.aerial_perspective_lut_size[i] = kAerialLut[i];
-    }
-  }
+  // RendererInstance.cpp:1022: the per-frame LUTs and the cube update before the geometry's lighting chain
+  if (atmosphere && (rc = sky_ibl_device(*atmosphere, pbr_camera, settings.sun_direction, settings.sun_intensity)) != OXC_OK) return rc;
   OxcGBufferTargets gb{};
   gb.albedo = d_gbuffer_; gb.normal = d_gbuffer_ + px * 4; gb.emissive = d_gbuffer_ + px * 8; gb.metallic_roughness_occlusion = d_gbuffer_ + px * 12;
   if ((rc = decode_gbuffer_device(camera, gb)) != OXC_OK) return rc;
@@ -506,15 +488,15 @@ auto RendererInstance::apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera
       cudaMemcpyAsync(d_lights_, lights_host, settings.light_count * sizeof(OxcLight), cudaMemcpyHostToDevice, s) != cudaSuccess)
     return fail(OXC_E_CUDA);
   if (atmosphere) {
-    const size_t t_texels = (size_t)kTransmittanceLut[0] * kTransmittanceLut[1], sv_texels = (size_t)kSkyViewLut[0] * kSkyViewLut[1];
-    const OxcPbrSky sky{d_atmosphere_, d_atmosphere_ + t_texels * 4, d_atmosphere_ + (t_texels + sv_texels) * 4, d_sky_ibl_cube_};
+    const AtmosphereLuts luts = lut_planes(d_atmosphere_);
+    const OxcPbrSky sky{luts.transmittance, luts.sky_view, luts.aerial_perspective, d_sky_ibl_cube_};
+    const OxcAtmosphere sized = sized_atmosphere(*atmosphere);
     rc = oxc_apply_pbr_atmosphere(ctx_, &pbr_camera, &settings, &sized, d_lights_, &in, &sky, width_, height_, d_pbr_, stream_);
   } else {
     rc = oxc_apply_pbr(ctx_, &pbr_camera, &settings, d_lights_, &in, width_, height_, d_pbr_, stream_);
   }
   if (rc != OXC_OK) return fail(rc);
-  if (cudaMemcpyAsync(rgba_host, d_pbr_, px * 16, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
-    return fail(OXC_E_CUDA);
+  if ((rc = copy_to_host({{rgba_host, d_pbr_, px * 16}})) != OXC_OK) return rc;
   pbr_lit_ = true;
   return OXC_OK;
 }
@@ -525,21 +507,14 @@ auto RendererInstance::eye_adaptation(const OxcEyeAdaptationSettings& settings, 
   if (!pbr_lit_) return OXC_E_INVALID; // no lit plane yet
   cudaStream_t s = static_cast<cudaStream_t>(stream_);
   const bool first = !d_post_;
-  if (first && cudaMalloc(reinterpret_cast<void**>(&d_post_), OXC_HISTOGRAM_BIN_COUNT * 4 + sizeof(OxcExposure)) != cudaSuccess) {
-    cudaGetLastError();
-    d_post_ = nullptr;
-    return OXC_E_CAPACITY; // an optional part: the camera path stays usable
-  }
+  if (optional_plane(&d_post_, OXC_HISTOGRAM_BIN_COUNT * 4 + sizeof(OxcExposure)) != OXC_OK) return OXC_E_CAPACITY;
   OxcExposure* record = reinterpret_cast<OxcExposure*>(d_post_ + OXC_HISTOGRAM_BIN_COUNT);
   const OxcExposure one{1.0f, 1.0f};
   if (first && (cudaMemcpyAsync(record, &one, sizeof one, cudaMemcpyHostToDevice, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess))
     return fail(OXC_E_CUDA);
   int rc;
   if ((rc = oxc_eye_adaptation(ctx_, d_pbr_, width_, height_, &settings, delta_time, record, d_post_, stream_)) != OXC_OK) return fail(rc);
-  if ((exposure_host && cudaMemcpyAsync(exposure_host, record, sizeof(OxcExposure), cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
-      cudaStreamSynchronize(s) != cudaSuccess)
-    return fail(OXC_E_CUDA);
-  return OXC_OK;
+  return copy_to_host({{exposure_host, record, sizeof(OxcExposure)}});
 }
 
 // bloom on stream_, synchronous: the two chains are allocated at the first call
@@ -549,21 +524,12 @@ auto RendererInstance::bloom(const OxcBloomSettings& settings, float* bloom_host
   const bool adapt = (settings.scene_flags & OXC_SCENE_HAS_EYE_ADAPTATION) != 0;
   if (adapt && !d_post_) return OXC_E_STATE; // no exposure record before an eye_adaptation
   const uint64_t texels = oxc_bloom_chain_texels(width_, height_);
-  if (!d_bloom_ && cudaMalloc(reinterpret_cast<void**>(&d_bloom_), texels * 32) != cudaSuccess) {
-    cudaGetLastError();
-    d_bloom_ = nullptr;
-    return OXC_E_CAPACITY; // an optional part: the camera path stays usable
-  }
+  if (optional_plane(&d_bloom_, texels * 32) != OXC_OK) return OXC_E_CAPACITY;
   const OxcBloomTargets targets{d_bloom_, d_bloom_ + texels * 4};
   const OxcExposure* record = adapt ? reinterpret_cast<const OxcExposure*>(d_post_ + OXC_HISTOGRAM_BIN_COUNT) : nullptr;
   int rc;
   if ((rc = oxc_bloom(ctx_, d_pbr_, width_, height_, &settings, record, &targets, stream_)) != OXC_OK) return fail(rc);
-  cudaStream_t s = static_cast<cudaStream_t>(stream_);
-  if ((bloom_host && cudaMemcpyAsync(bloom_host, targets.upsampled, (size_t)(width_ / 2) * (height_ / 2) * 16, cudaMemcpyDeviceToHost, s) !=
-                         cudaSuccess) ||
-      cudaStreamSynchronize(s) != cudaSuccess)
-    return fail(OXC_E_CUDA);
-  return OXC_OK;
+  return copy_to_host({{bloom_host, targets.upsampled, (size_t)(width_ / 2) * (height_ / 2) * 16}});
 }
 
 // the contact_shadows pass (RendererInstance.cpp:990-1020) on stream_, synchronous: the last frame's depth, the pass into the renderer's
@@ -572,40 +538,22 @@ auto RendererInstance::contact_shadows(const OxcContactShadowCamera& contact_cam
     -> int {
   if (!ctx_ || !error_.empty()) return OXC_E_STATE;
   if (!contact_host) return OXC_E_INVALID;
-  // the plane is an optional part, as the other passes' are: without room for it the camera path stays usable
-  if (contact_plane() != OXC_OK) return OXC_E_CAPACITY;
+  const size_t px = (size_t)width_ * height_;
+  if (optional_plane(&d_contact_, px * 4) != OXC_OK) return OXC_E_CAPACITY;
   int rc;
   if ((rc = contact_shadows_device(contact_camera, settings)) != OXC_OK) return rc;
-  cudaStream_t s = static_cast<cudaStream_t>(stream_);
-  if (cudaMemcpyAsync(contact_host, d_contact_, (size_t)width_ * height_ * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-      cudaStreamSynchronize(s) != cudaSuccess)
-    return fail(OXC_E_CUDA);
-  return OXC_OK;
+  return copy_to_host({{contact_host, d_contact_, px * 4}});
 }
 
 // the atmosphere's LUTs on stream_, without a copy: the bake once with the default record (RendererInstance.cpp:203-226), then the two
-// per-frame LUTs with the caller's record at the renderer's extents (:1456-1459, PBR.cpp:11-50 and :96-140); *sized receives that record
+// per-frame LUTs with the caller's record at the renderer's extents (:1456-1459, PBR.cpp:11-50 and :96-140)
 int RendererInstance::atmosphere_luts_device(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3],
-                                             float sun_intensity, OxcAtmosphere* sized_out) {
+                                             float sun_intensity) {
   if (!ctx_ || !error_.empty()) return OXC_E_STATE;
   if (!sun_direction) return OXC_E_INVALID;
-  const size_t t_texels = (size_t)kTransmittanceLut[0] * kTransmittanceLut[1], sv_texels = (size_t)kSkyViewLut[0] * kSkyViewLut[1];
-  const size_t ap_texels = (size_t)kAerialLut[0] * kAerialLut[1] * kAerialLut[2];
-  if (!d_atmosphere_ && cudaMalloc(reinterpret_cast<void**>(&d_atmosphere_), (t_texels + sv_texels + ap_texels) * 8) != cudaSuccess) {
-    cudaGetLastError();
-    d_atmosphere_ = nullptr;
-    return OXC_E_CAPACITY; // an optional part: the camera path stays usable
-  }
-  uint16_t* d_t = d_atmosphere_;
-  uint16_t* d_sv = d_t + t_texels * 4;
-  uint16_t* d_ap = d_sv + sv_texels * 4;
-  OxcAtmosphere sized = atmosphere;
-  sized.transmittance_lut_size[0] = kTransmittanceLut[0]; sized.transmittance_lut_size[1] = kTransmittanceLut[1];
-  sized.transmittance_lut_size[2] = 1;
-  sized.sky_view_lut_size[0] = kSkyViewLut[0]; sized.sky_view_lut_size[1] = kSkyViewLut[1]; sized.sky_view_lut_size[2] = 1;
-  sized.multiscattering_lut_size[0] = kMultiscatteringLut[0]; sized.multiscattering_lut_size[1] = kMultiscatteringLut[1];
-  sized.multiscattering_lut_size[2] = 1;
-  for (int i = 0; i < 3; i++) sized.aerial_perspective_lut_size[i] = kAerialLut[i];
+  if (optional_plane(&d_atmosphere_, (kTransmittanceTexels + kSkyViewTexels + kAerialTexels) * 8) != OXC_OK) return OXC_E_CAPACITY;
+  const AtmosphereLuts luts = lut_planes(d_atmosphere_);
+  const OxcAtmosphere sized = sized_atmosphere(atmosphere);
   int rc;
   if (!transmittance_baked_) {
     // GPU::Atmosphere{} with only the transmittance and multiple-scattering sizes set, as the reference's init bakes it
@@ -613,11 +561,12 @@ int RendererInstance::atmosphere_luts_device(const OxcAtmosphere& atmosphere, co
                          {0.000650f, 0.001881f, 0.000085f}, 25.0f, 15.0f, {0.3f, 0.3f, 0.3f}, 6360.0f, 6460.0f, 8.0f, 1.0f,
                          {kTransmittanceLut[0], kTransmittanceLut[1], 1}, {0, 0, 0}, {kMultiscatteringLut[0], kMultiscatteringLut[1], 1},
                          {0, 0, 0}};
-    if ((rc = oxc_atmosphere_transmittance(ctx_, &def, d_t, stream_)) != OXC_OK) return fail(rc);
+    if ((rc = oxc_atmosphere_transmittance(ctx_, &def, luts.transmittance, stream_)) != OXC_OK) return fail(rc);
     transmittance_baked_ = true;
   }
-  if ((rc = oxc_atmosphere_sky_luts(ctx_, &sized, &camera, sun_direction, sun_intensity, d_t, d_sv, d_ap, stream_)) != OXC_OK) return fail(rc);
-  if (sized_out) *sized_out = sized;
+  if ((rc = oxc_atmosphere_sky_luts(ctx_, &sized, &camera, sun_direction, sun_intensity, luts.transmittance, luts.sky_view, luts.aerial_perspective,
+                                    stream_)) != OXC_OK)
+    return fail(rc);
   return OXC_OK;
 }
 
@@ -626,43 +575,26 @@ auto RendererInstance::atmosphere_luts(const OxcAtmosphere& atmosphere, const Ox
                                        float sun_intensity, uint16_t* transmittance_host, uint16_t* sky_view_host,
                                        uint16_t* aerial_perspective_host) -> int {
   int rc;
-  if ((rc = atmosphere_luts_device(atmosphere, camera, sun_direction, sun_intensity, nullptr)) != OXC_OK) return rc;
-  const size_t t_texels = (size_t)kTransmittanceLut[0] * kTransmittanceLut[1], sv_texels = (size_t)kSkyViewLut[0] * kSkyViewLut[1];
-  const size_t ap_texels = (size_t)kAerialLut[0] * kAerialLut[1] * kAerialLut[2];
-  uint16_t* d_t = d_atmosphere_;
-  uint16_t* d_sv = d_t + t_texels * 4;
-  uint16_t* d_ap = d_sv + sv_texels * 4;
-  cudaStream_t s = static_cast<cudaStream_t>(stream_);
-  if ((transmittance_host && cudaMemcpyAsync(transmittance_host, d_t, t_texels * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
-      (sky_view_host && cudaMemcpyAsync(sky_view_host, d_sv, sv_texels * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
-      (aerial_perspective_host && cudaMemcpyAsync(aerial_perspective_host, d_ap, ap_texels * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
-      cudaStreamSynchronize(s) != cudaSuccess)
-    return fail(OXC_E_CUDA);
-  return OXC_OK;
+  if ((rc = atmosphere_luts_device(atmosphere, camera, sun_direction, sun_intensity)) != OXC_OK) return rc;
+  const AtmosphereLuts luts = lut_planes(d_atmosphere_);
+  return copy_to_host({{transmittance_host, luts.transmittance, kTransmittanceTexels * 8}, {sky_view_host, luts.sky_view, kSkyViewTexels * 8},
+                       {aerial_perspective_host, luts.aerial_perspective, kAerialTexels * 8}});
 }
 
 // the per-frame LUTs as atmosphere_luts makes them, then the sky IBL cube (PBR.cpp:52-94) into the renderer's cube with
 // sun_ambient_strength 0.15 and frame_index = the count of earlier calls, on stream_ without a copy
 int RendererInstance::sky_ibl_device(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3],
                                      float sun_intensity) {
-  OxcAtmosphere sized;
   int rc;
-  if ((rc = atmosphere_luts_device(atmosphere, camera, sun_direction, sun_intensity, &sized)) != OXC_OK) return rc;
-  cudaStream_t s = static_cast<cudaStream_t>(stream_);
-  if (!d_sky_ibl_cube_) {
-    if (cudaMalloc(reinterpret_cast<void**>(&d_sky_ibl_cube_), OXC_SKY_IBL_CUBE_BYTES) != cudaSuccess) {
-      cudaGetLastError();
-      d_sky_ibl_cube_ = nullptr;
-      return OXC_E_CAPACITY; // an optional part: the camera path stays usable
-    }
-    // cleared to black, as RendererInstance.cpp:197-201 clears the reference's: no texel has history
-    if (cudaMemsetAsync(d_sky_ibl_cube_, 0, OXC_SKY_IBL_CUBE_BYTES, s) != cudaSuccess) return fail(OXC_E_CUDA);
-  }
-  const size_t t_texels = (size_t)kTransmittanceLut[0] * kTransmittanceLut[1];
-  const uint16_t* d_t = d_atmosphere_;
-  const uint16_t* d_sv = d_t + t_texels * 4;
-  if ((rc = oxc_atmosphere_sky_ibl(ctx_, &sized, &camera, sun_direction, sun_intensity, 0.15f, sky_ibl_calls_, d_t, d_sv, d_sky_ibl_cube_,
-                                   stream_)) != OXC_OK)
+  if ((rc = atmosphere_luts_device(atmosphere, camera, sun_direction, sun_intensity)) != OXC_OK) return rc;
+  const bool first = !d_sky_ibl_cube_;
+  if (optional_plane(&d_sky_ibl_cube_, OXC_SKY_IBL_CUBE_BYTES) != OXC_OK) return OXC_E_CAPACITY;
+  // cleared to black, as RendererInstance.cpp:197-201 clears the reference's: no texel has history
+  if (first && cudaMemsetAsync(d_sky_ibl_cube_, 0, OXC_SKY_IBL_CUBE_BYTES, static_cast<cudaStream_t>(stream_)) != cudaSuccess) return fail(OXC_E_CUDA);
+  const AtmosphereLuts luts = lut_planes(d_atmosphere_);
+  const OxcAtmosphere sized = sized_atmosphere(atmosphere);
+  if ((rc = oxc_atmosphere_sky_ibl(ctx_, &sized, &camera, sun_direction, sun_intensity, 0.15f, sky_ibl_calls_, luts.transmittance, luts.sky_view,
+                                   d_sky_ibl_cube_, stream_)) != OXC_OK)
     return fail(rc);
   sky_ibl_calls_++;
   return OXC_OK;
@@ -673,21 +605,7 @@ auto RendererInstance::atmosphere_sky_ibl(const OxcAtmosphere& atmosphere, const
                                           float sun_intensity, uint16_t* cube_host) -> int {
   int rc;
   if ((rc = sky_ibl_device(atmosphere, camera, sun_direction, sun_intensity)) != OXC_OK) return rc;
-  cudaStream_t s = static_cast<cudaStream_t>(stream_);
-  if ((cube_host && cudaMemcpyAsync(cube_host, d_sky_ibl_cube_, OXC_SKY_IBL_CUBE_BYTES, cudaMemcpyDeviceToHost, s) != cudaSuccess) ||
-      cudaStreamSynchronize(s) != cudaSuccess)
-    return fail(OXC_E_CUDA);
-  return OXC_OK;
-}
-
-int RendererInstance::contact_plane() {
-  if (d_contact_) return OXC_OK;
-  if (cudaMalloc(reinterpret_cast<void**>(&d_contact_), (size_t)width_ * height_ * 4) != cudaSuccess) {
-    cudaGetLastError();
-    d_contact_ = nullptr;
-    return OXC_E_CAPACITY;
-  }
-  return OXC_OK;
+  return copy_to_host({{cube_host, d_sky_ibl_cube_, OXC_SKY_IBL_CUBE_BYTES}});
 }
 
 int RendererInstance::contact_shadows_device(const OxcContactShadowCamera& contact_camera, const OxcContactShadowSettings& settings) {
@@ -726,9 +644,7 @@ auto RendererInstance::overdraw(const OxcCullCamera& camera, uint32_t* overdraw_
   if ((rc = oxc_clear_overdraw(ctx_, d_overdraw_, width_, height_, s)) != OXC_OK) return fail(rc);
   if ((rc = oxc_raster_overdraw(ctx_, &camera, OXC_CULL_TEST_ALL, width_, height_, d_overdraw_, /*after_frame=*/1, s)) != OXC_OK) return fail(rc);
   if ((rc = oxc_raster_overdraw(ctx_, &camera, OXC_CULL_TEST_ALL | OXC_CULL_LATE_PASS, width_, height_, d_overdraw_, /*after_frame=*/1, s)) != OXC_OK) return fail(rc);
-  if (cudaMemcpyAsync(overdraw_host, d_overdraw_, px * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
-    return fail(OXC_E_CUDA);
-  return OXC_OK;
+  return copy_to_host({{overdraw_host, d_overdraw_, px * 4}});
 }
 
 // the reference uploads its material table with the scene (RendererInstance.cpp:1333-1788); the vis-buffer encode reads it for

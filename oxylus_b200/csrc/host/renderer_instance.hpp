@@ -10,6 +10,7 @@
 // pointers owned by this object; "recording a pass" becomes enqueuing liboxcull kernels on one stream.
 #pragma once
 #include <cstdint>
+#include <initializer_list>
 #include <string>
 #include <vector>
 
@@ -126,6 +127,12 @@ public:
 
 private:
   int fail(int rc);
+  // allocates `bytes` at *p unless *p is set.  The passes' planes are optional parts: without room for one the camera path stays
+  // usable, so a failed allocation clears the CUDA error, leaves *p null and returns OXC_E_CAPACITY without setting the sticky error
+  template <typename T> int optional_plane(T** p, size_t bytes);
+  // the copies whose host pointer is set, device to host on stream_, then the end of the stream: OXC_OK, else the sticky OXC_E_CUDA
+  struct HostCopy { void* host; const void* dev; size_t bytes; };
+  int copy_to_host(std::initializer_list<HostCopy> copies);
   int run_frame(const OxcCullCamera& camera, const float* occluder_depth_host, void* readback_draw_counts, bool readback_on_device);
   int frame_head(const OxcCullCamera& camera, const float* occluder_depth_host, void* readback_draw_counts, bool readback_on_device);
   int frame_tail(const OxcCullCamera& camera, void* readback_draw_counts);
@@ -180,10 +187,6 @@ private:
   float* d_uv_normal_ = nullptr;    // uv_normal plane (float4 per pixel) the shadow resolve and the GTAO decode into, allocated by the
                                     // first of them; kept for the renderer's lifetime
   void* d_gtao_ = nullptr;          // generate_ambient_occlusion's planes (mips, edges, noisy and final occlusion), allocated by its first call
-  int uv_normal_plane();            // allocates d_uv_normal_ when missing: OXC_OK or OXC_E_CAPACITY
-  int gbuffer_planes();             // allocates d_gbuffer_ when missing: OXC_OK or OXC_E_CAPACITY
-  int shadow_plane();               // allocates vsm_.d_shadow when missing: OXC_OK or OXC_E_CAPACITY
-  int gtao_planes();                // allocates d_gtao_ when missing: OXC_OK or OXC_E_CAPACITY
   size_t gtao_mip_texels() const;   // texels of the five depth mips at the renderer's extent
   // the device parts of decode_visbuffer, resolve_shadowmap and generate_ambient_occlusion, enqueued on stream_ without a copy; the
   // two last read the given normal plane (oct(world normal) in .zw)
@@ -193,18 +196,14 @@ private:
                                         OxcGtaoTargets* targets);
   float* d_pbr_ = nullptr;          // apply_pbr's output plane (float4 per pixel), allocated by its first call
   float* d_contact_ = nullptr;      // the contact-shadow plane (f32 per pixel), allocated by the first call that runs the pass
-  int contact_plane();              // allocates d_contact_ when missing: OXC_OK or OXC_E_CAPACITY
   // the frame's depth, then the contact-shadow pass into d_contact_, enqueued on stream_ without a copy
   int contact_shadows_device(const OxcContactShadowCamera& contact_camera, const OxcContactShadowSettings& settings);
-  // the atmosphere's LUTs at the reference's extents (RendererInstance.hpp: 256 x 64, 312 x 192, 32 x 32 x 32), binary16 RGBA, allocated
-  // by the first atmosphere_luts; the transmittance LUT is baked once, with the default record
-  static constexpr uint32_t kTransmittanceLut[2] = {256, 64}, kSkyViewLut[2] = {312, 192}, kMultiscatteringLut[2] = {32, 32},
-                            kAerialLut[3] = {32, 32, 32};
-  uint16_t* d_atmosphere_ = nullptr; // transmittance, then sky view, then aerial perspective
+  // the atmosphere's LUTs at the reference's extents in one block (renderer_instance.cpp: lut_planes), allocated by the first
+  // atmosphere_luts; the transmittance LUT is baked once, with the default record
+  uint16_t* d_atmosphere_ = nullptr;
   bool transmittance_baked_ = false;
-  // the bake when missing and the per-frame LUTs on stream_, without a copy; sized_out (may be null) receives the record they used
-  int atmosphere_luts_device(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3], float sun_intensity,
-                             OxcAtmosphere* sized_out);
+  // the bake when missing and the per-frame LUTs on stream_, without a copy
+  int atmosphere_luts_device(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3], float sun_intensity);
   uint16_t* d_sky_ibl_cube_ = nullptr; // the sky IBL cube, allocated and zeroed by the first atmosphere_sky_ibl
   uint32_t sky_ibl_calls_ = 0;         // atmosphere_sky_ibl calls so far: the frame_index of the next one
   bool pbr_lit_ = false;               // d_pbr_ holds the output of a successful apply_pbr

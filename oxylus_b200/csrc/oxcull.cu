@@ -230,6 +230,29 @@ uint32_t capped_grid(const OxcContext* c, size_t n) {
   return grid ? (uint32_t)grid : 1u;
 }
 
+// Grid of a w x h pixel pass in tx x ty pixel tiles.
+dim3 tiles(uint32_t w, uint32_t h, uint32_t tx, uint32_t ty) { return dim3((w + tx - 1) / tx, (h + ty - 1) / ty); }
+
+// [a, a + na) and [b, b + nb) share a byte
+bool overlaps(const void* a, uint64_t na, const void* b, uint64_t nb) {
+  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+  return x < y + nb && y < x + na;
+}
+
+// some pointer is not a multiple of `bytes` (a power of two)
+template <typename... T>
+bool misaligned(uintptr_t bytes, const T*... p) {
+  return ((reinterpret_cast<uintptr_t>(p) | ...) & (bytes - 1)) != 0;
+}
+
+// The extent the screen-space passes accept (the G-buffer decode has no upper bound): 1..MAX_EXTENT on each side.
+constexpr uint32_t MAX_EXTENT = 32768;
+int check_extent(uint32_t w, uint32_t h) {
+  if (w == 0 || h == 0) return fail(OXC_E_INVALID, "empty extent %u x %u", w, h);
+  if (w > MAX_EXTENT || h > MAX_EXTENT) return fail(OXC_E_INVALID, "extent %u x %u above %u", w, h, MAX_EXTENT);
+  return OXC_OK;
+}
+
 int check_vis_id_bits(const OxcContext* c) {
   if (c->scene_id_bound > (1ull << (32u - c->prim_bits)))
     return fail(OXC_E_CAPACITY, "the scene can emit %llu meshlet instances: ids overflow the %u id bits of the vis-buffer word (visbuffer.slang:9-10)%s",
@@ -1191,8 +1214,7 @@ int oxc_decode_visbuffer(OxcContext* c, const OxcCullCamera* cam, const uint64_t
   decode_params(c, cam, vis64_dev, vis32_dev, w, h, &p);
   p.lambda = reinterpret_cast<float4*>(t->lambda); p.ddx = reinterpret_cast<float4*>(t->ddx); p.ddy = reinterpret_cast<float4*>(t->ddy);
   p.uv_normal = reinterpret_cast<float4*>(t->uv_normal); p.uv_grad = reinterpret_cast<float4*>(t->uv_grad);
-  const dim3 grid((w + DECODE_TX - 1) / DECODE_TX, (h + DECODE_TY - 1) / DECODE_TY);
-  k_decode_visbuffer<<<grid, dim3(DECODE_TX, DECODE_TY), 0, s>>>(p);
+  k_decode_visbuffer<<<tiles(w, h, DECODE_TX, DECODE_TY), dim3(DECODE_TX, DECODE_TY), 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }
@@ -1205,7 +1227,7 @@ int oxc_decode_gbuffer(OxcContext* c, const OxcCullCamera* cam, const uint64_t* 
   float* const planes[4] = {t->albedo, t->normal, t->emissive, t->metallic_roughness_occlusion};
   static const char* const plane_name[4] = {"albedo", "normal", "emissive", "metallic_roughness_occlusion"};
   for (int k = 0; k < 4; k++)
-    if (reinterpret_cast<uintptr_t>(planes[k]) & 15u) return fail(OXC_E_INVALID, "target %s is not 16-byte aligned (float4 per pixel)", plane_name[k]);
+    if (misaligned(16, planes[k])) return fail(OXC_E_INVALID, "target %s is not 16-byte aligned (float4 per pixel)", plane_name[k]);
   if (!c->scene_set) return fail(OXC_E_STATE, "oxc_set_scene first");
   if (c->gbuf_material_count == 0) return fail(OXC_E_STATE, "oxc_set_materials first: the decode reads the material table");
   if (!c->gbuf_error.empty()) return fail(OXC_E_INVALID, "material table: %s", c->gbuf_error.c_str());
@@ -1226,8 +1248,7 @@ int oxc_decode_gbuffer(OxcContext* c, const OxcCullCamera* cam, const uint64_t* 
   p.albedo = reinterpret_cast<float4*>(t->albedo); p.normal = reinterpret_cast<float4*>(t->normal);
   p.emissive = reinterpret_cast<float4*>(t->emissive); p.mro = reinterpret_cast<float4*>(t->metallic_roughness_occlusion);
   p.status = c->d_status;
-  const dim3 grid((w + DECODE_TX - 1) / DECODE_TX, (h + DECODE_TY - 1) / DECODE_TY);
-  k_decode_gbuffer<<<grid, dim3(DECODE_TX, DECODE_TY), 0, s>>>(p);
+  k_decode_gbuffer<<<tiles(w, h, DECODE_TX, DECODE_TY), dim3(DECODE_TX, DECODE_TY), 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }
@@ -1378,7 +1399,7 @@ int oxc_vsm_clear_dirty_pages(OxcContext* c, const OxcVsmContext* vsm, const Oxc
   VsmClearParams p{};
   p.allocator = allocator_dev; p.dirty_coords = reinterpret_cast<const uint2*>(dirty_coords_dev); p.atlas = physical_atlas_dev;
   p.page_size = (uint32_t)vsm->page_size; p.atlas_size = (uint32_t)vsm->physical_page_table_size; p.phys_per_row = p.atlas_size / p.page_size;
-  p.vec4 = (p.page_size % 4u == 0u && (reinterpret_cast<uintptr_t>(physical_atlas_dev) & 15u) == 0u) ? 1 : 0;
+  p.vec4 = (p.page_size % 4u == 0u && !misaligned(16, physical_atlas_dev)) ? 1 : 0;
   p.row_shift = -1;
   if (p.vec4 && is_pow2(p.page_size / 4u)) p.row_shift = (int)ilog2(p.page_size / 4u);
   // up to 8 CTAs per SM, never more than there can be dirty pages: a frame with few dirty pages costs a short, mostly idle launch
@@ -1463,13 +1484,12 @@ int oxc_vsm_resolve_shadows(OxcContext* c, const OxcVsmContext* vsm, const float
   if (rc != OXC_OK) return rc;
   if (vsm->depth_extent[0] < 1 || vsm->depth_extent[1] < 1)
     return fail(OXC_E_INVALID, "depth_extent %d x %d is empty", vsm->depth_extent[0], vsm->depth_extent[1]);
-  if (reinterpret_cast<uintptr_t>(normals_dev) & 15u) return fail(OXC_E_INVALID, "normals_dev is not 16-byte aligned (float4 per pixel)");
+  if (misaligned(16, normals_dev)) return fail(OXC_E_INVALID, "normals_dev is not 16-byte aligned (float4 per pixel)");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
   const VsmResolveParams p = vsm_resolve_make_params(*vsm, inv_pv, resolution, clipmaps, depth_dev, normals_dev, page_tables_dev,
                                                       physical_atlas_dev, shadow_dev);
-  const dim3 grid((p.width + VSM_RESOLVE_TILE_X - 1) / VSM_RESOLVE_TILE_X, (p.height + VSM_RESOLVE_TILE_Y - 1) / VSM_RESOLVE_TILE_Y);
-  k_vsm_resolve_shadows<<<grid, VSM_RESOLVE_THREADS, 0, s>>>(p);
+  k_vsm_resolve_shadows<<<tiles(p.width, p.height, VSM_RESOLVE_TILE_X, VSM_RESOLVE_TILE_Y), VSM_RESOLVE_THREADS, 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }
@@ -1478,24 +1498,22 @@ int oxc_generate_ambient_occlusion(OxcContext* c, const OxcGtaoCamera* cam, cons
                                    const float* normals_dev, uint32_t w, uint32_t h, const OxcGtaoTargets* t, void* stream) {
   if (!c || !cam || !st || !depth_dev || !normals_dev || !t) return fail(OXC_E_INVALID, "null argument");
   if (!t->depth_mips || !t->edges || !t->noisy_occlusion || !t->ambient_occlusion) return fail(OXC_E_INVALID, "null target");
-  if (w == 0 || h == 0) return fail(OXC_E_INVALID, "empty extent %u x %u", w, h);
-  if (w > 32768u || h > 32768u) return fail(OXC_E_INVALID, "extent %u x %u above 32768", w, h);
+  int rc;
+  if ((rc = check_extent(w, h)) != OXC_OK) return rc;
   if (st->slice_count < 1u || st->slice_count > OXC_GTAO_MAX_SLICES)
     return fail(OXC_E_INVALID, "slice_count %u outside 1..%u", st->slice_count, OXC_GTAO_MAX_SLICES);
   if (st->samples_per_slice_side < 1u || st->samples_per_slice_side > OXC_GTAO_MAX_SAMPLES_PER_SIDE)
     return fail(OXC_E_INVALID, "samples_per_slice_side %u outside 1..%u", st->samples_per_slice_side, OXC_GTAO_MAX_SAMPLES_PER_SIDE);
-  if (reinterpret_cast<uintptr_t>(normals_dev) & 15u) return fail(OXC_E_INVALID, "normals_dev is not 16-byte aligned (float4 per pixel)");
-  if ((reinterpret_cast<uintptr_t>(depth_dev) | reinterpret_cast<uintptr_t>(t->depth_mips) | reinterpret_cast<uintptr_t>(t->edges) |
-       reinterpret_cast<uintptr_t>(t->ambient_occlusion)) & 3u)
+  if (misaligned(16, normals_dev)) return fail(OXC_E_INVALID, "normals_dev is not 16-byte aligned (float4 per pixel)");
+  if (misaligned(4, depth_dev, t->depth_mips, t->edges, t->ambient_occlusion))
     return fail(OXC_E_INVALID, "depth_dev, depth_mips, edges and ambient_occlusion must be 4-byte aligned");
-  if (reinterpret_cast<uintptr_t>(t->noisy_occlusion) & 1u) return fail(OXC_E_INVALID, "noisy_occlusion is not 2-byte aligned");
+  if (misaligned(2, t->noisy_occlusion)) return fail(OXC_E_INVALID, "noisy_occlusion is not 2-byte aligned");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
   const GtaoParams p = gtao_make_params(*cam, *st, depth_dev, normals_dev, w, h, *t);
-  const dim3 pre((w + 2 * GTAO_PREFILTER_SIDE - 1) / (2 * GTAO_PREFILTER_SIDE), (h + 2 * GTAO_PREFILTER_SIDE - 1) / (2 * GTAO_PREFILTER_SIDE));
-  k_gtao_prefilter<<<pre, dim3(GTAO_PREFILTER_SIDE, GTAO_PREFILTER_SIDE), 0, s>>>(p);
+  k_gtao_prefilter<<<tiles(w, h, 2 * GTAO_PREFILTER_SIDE, 2 * GTAO_PREFILTER_SIDE), dim3(GTAO_PREFILTER_SIDE, GTAO_PREFILTER_SIDE), 0, s>>>(p);
   LAUNCHED();
-  const dim3 grid((w + GTAO_TILE_X - 1) / GTAO_TILE_X, (h + GTAO_TILE_Y - 1) / GTAO_TILE_Y);
+  const dim3 grid = tiles(w, h, GTAO_TILE_X, GTAO_TILE_Y);
   k_gtao_main<<<grid, GTAO_THREADS, 0, s>>>(p);
   LAUNCHED();
   k_gtao_denoise<<<grid, GTAO_THREADS, 0, s>>>(p);
@@ -1503,7 +1521,7 @@ int oxc_generate_ambient_occlusion(OxcContext* c, const OxcGtaoCamera* cam, cons
   return OXC_OK;
 }
 
-// what oxc_apply_pbr and oxc_apply_pbr_atmosphere both refuse: the planes, lights, extent and alignment: the planes, lights, extent and alignment
+// what oxc_apply_pbr and oxc_apply_pbr_atmosphere both refuse: the planes, lights, extent and alignment
 static int pbr_check_inputs(const OxcPbrSettings& st, const OxcLight* lights_dev, const OxcPbrInputs& in, uint32_t w, uint32_t h,
                             const float* out_dev) {
   if (!in.depth || !in.albedo || !in.normal || !in.emissive || !in.metallic_roughness_occlusion) return fail(OXC_E_INVALID, "null input plane");
@@ -1511,14 +1529,11 @@ static int pbr_check_inputs(const OxcPbrSettings& st, const OxcLight* lights_dev
   if (st.light_count > 0 && !lights_dev) return fail(OXC_E_INVALID, "null lights with light_count %u", st.light_count);
   if ((st.scene_flags & OXC_SCENE_HAS_CONTACT_SHADOWS) && !in.contact_shadow)
     return fail(OXC_E_INVALID, "null contact_shadow plane under HasContactShadows");
-  if (w == 0 || h == 0) return fail(OXC_E_INVALID, "empty extent %u x %u", w, h);
-  if (w > 32768u || h > 32768u) return fail(OXC_E_INVALID, "extent %u x %u above 32768", w, h);
-  if ((reinterpret_cast<uintptr_t>(in.albedo) | reinterpret_cast<uintptr_t>(in.normal) | reinterpret_cast<uintptr_t>(in.emissive) |
-       reinterpret_cast<uintptr_t>(in.metallic_roughness_occlusion) | reinterpret_cast<uintptr_t>(out_dev) |
-       reinterpret_cast<uintptr_t>(lights_dev)) & 15u)
+  int rc;
+  if ((rc = check_extent(w, h)) != OXC_OK) return rc;
+  if (misaligned(16, in.albedo, in.normal, in.emissive, in.metallic_roughness_occlusion, out_dev, lights_dev))
     return fail(OXC_E_INVALID, "float4 planes, out_dev and lights_dev must be 16-byte aligned");
-  if ((reinterpret_cast<uintptr_t>(in.depth) | reinterpret_cast<uintptr_t>(in.ambient_occlusion) | reinterpret_cast<uintptr_t>(in.shadow) |
-       reinterpret_cast<uintptr_t>(in.contact_shadow)) & 3u)
+  if (misaligned(4, in.depth, in.ambient_occlusion, in.shadow, in.contact_shadow))
     return fail(OXC_E_INVALID, "depth, ambient_occlusion, shadow and contact_shadow must be 4-byte aligned");
   return OXC_OK;
 }
@@ -1532,8 +1547,7 @@ int oxc_apply_pbr(OxcContext* c, const OxcPbrCamera* cam, const OxcPbrSettings* 
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
   const PbrParams p = pbr_make_params(*cam, *st, lights_dev, *in, w, h, out_dev);
-  const dim3 grid((w + PBR_TILE_X - 1) / PBR_TILE_X, (h + PBR_TILE_Y - 1) / PBR_TILE_Y);
-  k_apply_pbr<<<grid, PBR_THREADS, 0, s>>>(p);
+  k_apply_pbr<<<tiles(w, h, PBR_TILE_X, PBR_TILE_Y), PBR_THREADS, 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }
@@ -1541,17 +1555,15 @@ int oxc_apply_pbr(OxcContext* c, const OxcPbrCamera* cam, const OxcPbrSettings* 
 int oxc_contact_shadows(OxcContext* c, const OxcContactShadowCamera* cam, const OxcContactShadowSettings* st, const float* depth_dev, uint32_t w,
                         uint32_t h, float* out_dev, void* stream) {
   if (!c || !cam || !st || !depth_dev || !out_dev) return fail(OXC_E_INVALID, "null argument");
-  if (w == 0 || h == 0) return fail(OXC_E_INVALID, "empty extent %u x %u", w, h);
-  if (w > 32768u || h > 32768u) return fail(OXC_E_INVALID, "extent %u x %u above 32768", w, h);
+  int rc;
+  if ((rc = check_extent(w, h)) != OXC_OK) return rc;
   if (st->steps < 1u || st->steps > OXC_CONTACT_SHADOW_MAX_STEPS)
     return fail(OXC_E_INVALID, "steps %u outside 1..%u", st->steps, OXC_CONTACT_SHADOW_MAX_STEPS);
-  if ((reinterpret_cast<uintptr_t>(depth_dev) | reinterpret_cast<uintptr_t>(out_dev)) & 3u)
-    return fail(OXC_E_INVALID, "depth_dev and out_dev must be 4-byte aligned");
+  if (misaligned(4, depth_dev, out_dev)) return fail(OXC_E_INVALID, "depth_dev and out_dev must be 4-byte aligned");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
   const ContactShadowParams p = cs_make_params(*cam, *st, depth_dev, w, h, out_dev);
-  const dim3 grid((w + CONTACT_TILE_X - 1) / CONTACT_TILE_X, (h + CONTACT_TILE_Y - 1) / CONTACT_TILE_Y);
-  k_contact_shadows<<<grid, CONTACT_THREADS, 0, s>>>(p);
+  k_contact_shadows<<<tiles(w, h, CONTACT_TILE_X, CONTACT_TILE_Y), CONTACT_THREADS, 0, s>>>(p);
   LAUNCHED();
   return OXC_OK;
 }
@@ -1577,7 +1589,7 @@ static int atmosphere_check_sizes(const OxcAtmosphere& a, bool sky_view, bool ae
 
 int oxc_atmosphere_transmittance(OxcContext* c, const OxcAtmosphere* atmosphere, uint16_t* lut_dev, void* stream) {
   if (!c || !atmosphere || !lut_dev) return fail(OXC_E_INVALID, "null argument");
-  if (reinterpret_cast<uintptr_t>(lut_dev) & 7u) return fail(OXC_E_INVALID, "lut_dev must be 8-byte aligned");
+  if (misaligned(8, lut_dev)) return fail(OXC_E_INVALID, "lut_dev must be 8-byte aligned");
   int rc;
   if ((rc = atmosphere_check_sizes(*atmosphere, false, false)) != OXC_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1594,8 +1606,7 @@ int oxc_atmosphere_sky_luts(OxcContext* c, const OxcAtmosphere* atmosphere, cons
                             void* stream) {
   if (!c || !atmosphere || !camera || !sun_direction || !transmittance_dev || !sky_view_dev || !aerial_perspective_dev)
     return fail(OXC_E_INVALID, "null argument");
-  if ((reinterpret_cast<uintptr_t>(transmittance_dev) | reinterpret_cast<uintptr_t>(sky_view_dev) |
-       reinterpret_cast<uintptr_t>(aerial_perspective_dev)) & 7u)
+  if (misaligned(8, transmittance_dev, sky_view_dev, aerial_perspective_dev))
     return fail(OXC_E_INVALID, "transmittance_dev, sky_view_dev and aerial_perspective_dev must be 8-byte aligned");
   int rc;
   if ((rc = atmosphere_check_sizes(*atmosphere, true, true)) != OXC_OK) return rc;
@@ -1618,16 +1629,14 @@ int oxc_atmosphere_sky_ibl(OxcContext* c, const OxcAtmosphere* atmosphere, const
                            const uint16_t* sky_view_dev, uint16_t* cube_dev, void* stream) {
   if (!c || !atmosphere || !camera || !sun_direction || !transmittance_dev || !sky_view_dev || !cube_dev)
     return fail(OXC_E_INVALID, "null argument");
-  if ((reinterpret_cast<uintptr_t>(transmittance_dev) | reinterpret_cast<uintptr_t>(sky_view_dev) | reinterpret_cast<uintptr_t>(cube_dev)) & 7u)
+  if (misaligned(8, transmittance_dev, sky_view_dev, cube_dev))
     return fail(OXC_E_INVALID, "transmittance_dev, sky_view_dev and cube_dev must be 8-byte aligned");
   int rc;
   if ((rc = atmosphere_check_sizes(*atmosphere, true, false)) != OXC_OK) return rc;
   const OxcAtmosphere& a = *atmosphere;
   // the cube is written while both LUTs are read: it may not share a byte with either
-  const uintptr_t cube = reinterpret_cast<uintptr_t>(cube_dev), cube_end = cube + (uintptr_t)OXC_SKY_IBL_CUBE_BYTES;
-  const uintptr_t t = reinterpret_cast<uintptr_t>(transmittance_dev), t_end = t + (uintptr_t)a.transmittance_lut_size[0] * a.transmittance_lut_size[1] * 8;
-  const uintptr_t sv = reinterpret_cast<uintptr_t>(sky_view_dev), sv_end = sv + (uintptr_t)a.sky_view_lut_size[0] * a.sky_view_lut_size[1] * 8;
-  if ((cube < t_end && t < cube_end) || (cube < sv_end && sv < cube_end))
+  if (overlaps(cube_dev, OXC_SKY_IBL_CUBE_BYTES, transmittance_dev, (uint64_t)a.transmittance_lut_size[0] * a.transmittance_lut_size[1] * 8) ||
+      overlaps(cube_dev, OXC_SKY_IBL_CUBE_BYTES, sky_view_dev, (uint64_t)a.sky_view_lut_size[0] * a.sky_view_lut_size[1] * 8))
     return fail(OXC_E_INVALID, "cube_dev overlaps transmittance_dev or sky_view_dev");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
@@ -1646,30 +1655,14 @@ int oxc_apply_pbr_atmosphere(OxcContext* c, const OxcPbrCamera* cam, const OxcPb
   int rc;
   if ((rc = pbr_check_inputs(*st, lights_dev, *in, w, h, out_dev)) != OXC_OK) return rc;
   if (!sky->transmittance || !sky->sky_view || !sky->aerial_perspective || !sky->sky_cube) return fail(OXC_E_INVALID, "null sky plane");
-  if ((reinterpret_cast<uintptr_t>(sky->transmittance) | reinterpret_cast<uintptr_t>(sky->sky_view) |
-       reinterpret_cast<uintptr_t>(sky->aerial_perspective) | reinterpret_cast<uintptr_t>(sky->sky_cube)) & 7u)
+  if (misaligned(8, sky->transmittance, sky->sky_view, sky->aerial_perspective, sky->sky_cube))
     return fail(OXC_E_INVALID, "sky planes must be 8-byte aligned");
   if ((rc = atmosphere_check_sizes(*atmosphere, true, true)) != OXC_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CK(cudaSetDevice(c->device));
   const PbrAtmParams p = pbr_atmosphere_make_params(*cam, *st, *atmosphere, lights_dev, *in, *sky, w, h, out_dev);
-  const dim3 grid((w + PBR_TILE_X - 1) / PBR_TILE_X, (h + PBR_TILE_Y - 1) / PBR_TILE_Y);
-  k_apply_pbr_atmosphere<<<grid, PBR_THREADS, 0, s>>>(p);
+  k_apply_pbr_atmosphere<<<tiles(w, h, PBR_TILE_X, PBR_TILE_Y), PBR_THREADS, 0, s>>>(p);
   LAUNCHED();
-  return OXC_OK;
-}
-
-// [a, a + na) and [b, b + nb) share a byte
-static bool overlaps(const void* a, uint64_t na, const void* b, uint64_t nb) {
-  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
-  return x < y + nb && y < x + na;
-}
-
-// the frame checks both post-processing calls make
-static int post_check_frame(const float* frame_dev, uint32_t w, uint32_t h) {
-  if (w == 0 || h == 0) return fail(OXC_E_INVALID, "empty extent %u x %u", w, h);
-  if (w > 32768u || h > 32768u) return fail(OXC_E_INVALID, "extent %u x %u above 32768", w, h);
-  if (reinterpret_cast<uintptr_t>(frame_dev) & 15u) return fail(OXC_E_INVALID, "frame_dev must be 16-byte aligned");
   return OXC_OK;
 }
 
@@ -1677,9 +1670,10 @@ int oxc_eye_adaptation(OxcContext* c, const float* frame_dev, uint32_t w, uint32
                        OxcExposure* exposure_dev, uint32_t* histogram_dev, void* stream) {
   if (!c || !frame_dev || !settings || !exposure_dev || !histogram_dev) return fail(OXC_E_INVALID, "null argument");
   int rc;
-  if ((rc = post_check_frame(frame_dev, w, h)) != OXC_OK) return rc;
-  if (reinterpret_cast<uintptr_t>(exposure_dev) & 7u) return fail(OXC_E_INVALID, "exposure_dev must be 8-byte aligned");
-  if (reinterpret_cast<uintptr_t>(histogram_dev) & 3u) return fail(OXC_E_INVALID, "histogram_dev must be 4-byte aligned");
+  if ((rc = check_extent(w, h)) != OXC_OK) return rc;
+  if (misaligned(16, frame_dev)) return fail(OXC_E_INVALID, "frame_dev must be 16-byte aligned");
+  if (misaligned(8, exposure_dev)) return fail(OXC_E_INVALID, "exposure_dev must be 8-byte aligned");
+  if (misaligned(4, histogram_dev)) return fail(OXC_E_INVALID, "histogram_dev must be 4-byte aligned");
   const uint64_t frame_bytes = (uint64_t)w * h * 16, hist_bytes = OXC_HISTOGRAM_BIN_COUNT * 4;
   if (overlaps(histogram_dev, hist_bytes, frame_dev, frame_bytes) || overlaps(exposure_dev, 8, frame_dev, frame_bytes) ||
       overlaps(exposure_dev, 8, histogram_dev, hist_bytes))
@@ -1705,11 +1699,11 @@ int oxc_bloom(OxcContext* c, const float* frame_dev, uint32_t w, uint32_t h, con
   const bool adapt = (settings->scene_flags & OXC_SCENE_HAS_EYE_ADAPTATION) != 0;
   if (adapt && !exposure_dev) return fail(OXC_E_INVALID, "null argument: HasEyeAdaptation reads exposure_dev");
   int rc;
-  if ((rc = post_check_frame(frame_dev, w, h)) != OXC_OK) return rc;
+  if ((rc = check_extent(w, h)) != OXC_OK) return rc;
+  if (misaligned(16, frame_dev)) return fail(OXC_E_INVALID, "frame_dev must be 16-byte aligned");
   if (w < 2 || h < 2) return fail(OXC_E_INVALID, "extent %u x %u below 2 x 2: the half extent is empty", w, h);
-  if (adapt && (reinterpret_cast<uintptr_t>(exposure_dev) & 7u)) return fail(OXC_E_INVALID, "exposure_dev must be 8-byte aligned");
-  if ((reinterpret_cast<uintptr_t>(targets->downsampled) | reinterpret_cast<uintptr_t>(targets->upsampled)) & 15u)
-    return fail(OXC_E_INVALID, "targets must be 16-byte aligned");
+  if (adapt && misaligned(8, exposure_dev)) return fail(OXC_E_INVALID, "exposure_dev must be 8-byte aligned");
+  if (misaligned(16, targets->downsampled, targets->upsampled)) return fail(OXC_E_INVALID, "targets must be 16-byte aligned");
   const uint64_t frame_bytes = (uint64_t)w * h * 16, chain_bytes = bloom_chain_texels(w, h) * 16;
   const float *down = targets->downsampled, *up = targets->upsampled;
   if (overlaps(down, chain_bytes, frame_dev, frame_bytes) || overlaps(up, chain_bytes, frame_dev, frame_bytes) ||

@@ -118,6 +118,21 @@ GPU_MODULES = [
     # count and a box on a plane; the full-size cases, the CUDA graph and the renderer frames stay on the GPU
     ("test_gpu_contact_shadows", "1x1 or 17x9 or test_steps or random_settings or box_on_plane or argument_refusals", {}, ORDERS, 14,
      3000),
+    # both atmosphere launches (the bake's row-major texels, the per-frame launch's sky-view and aerial-perspective CTAs side by side),
+    # parameters and refusals at the odd and minimum sizes and every camera height; the reference sizes, the random and hostile
+    # records, the CUDA graph and the renderer case stay on the GPU
+    ("test_gpu_atmosphere", "odd or minimum or argument_refusals", {}, ORDERS, 7, 3000),
+    # the sky IBL's (texel, sample) launch with its shared-memory hand-off and barrier on the small cases (the history sequence at three
+    # camera heights, hostile cubes, random and hostile records) and the refusals; the reference sizes, the CUDA graph and the renderer
+    # stay on the GPU
+    ("test_gpu_sky_ibl", "small or argument_refusals", {}, ORDERS, 9, 3000),
+    # k_apply_pbr_atmosphere with its shared-memory light staging and barrier on the small cases (three camera heights and suns over
+    # oracle-made LUTs and cubes, the hostile frames) and the refusals; 1080p, 4K and the CUDA graph stay on the GPU
+    ("test_gpu_pbr_atmosphere", "small or argument_refusals", {}, ORDERS, 7, 3000),
+    # the histogram's warp-aggregated shared-memory atomics, the average's shuffles and barrier, the bloom's per-level launches and
+    # single-CTA tail on the small cases (hostile frames and settings, the uniform frame, the adaptation sequence, the caller's last
+    # upsampled level) and the refusals; the reference sizes, the wrapping frame, the CUDA graph and the renderer stay on the GPU
+    ("test_gpu_post", "small or argument_refusals", {}, ORDERS, 5, 3000),
     # all nine k_cull_meshlets instantiations over three pyramid states, every flag subset, the occlusion toggle, the mesh-level flags, the
     # shard id base and mixed cameras through the raster; its hostile frames are the torture script's (test_hostile_inputs_...)
     ("test_gpu_variants", "not hostile_frames", {}, ("default",), 18, 900),
