@@ -1288,6 +1288,80 @@ uint64_t oxc_bloom_chain_texels(uint32_t width, uint32_t height);
 int oxc_bloom(OxcContext* ctx, const float* frame_dev, uint32_t width, uint32_t height, const OxcBloomSettings* settings,
               const OxcExposure* exposure_dev, const OxcBloomTargets* targets, void* stream);
 
+/* Tonemap (PostProcess.cpp:205-247, passes/tonemap.slang fs_main, passes/lens.slang): the last step of the post chain, the HDR lit
+ * frame to the displayed colour.  One thread per pixel of a width x height frame: the exposure, the bloom composite, the curve, then the
+ * lens effects, into out_dev (float4 per pixel, row-major).  frame_dev: the lit frame as either PBR apply writes it, float4, 16-byte
+ * aligned.  exposure_dev: oxc_eye_adaptation's record, read and required only under OXC_SCENE_HAS_EYE_ADAPTATION (8-byte aligned).
+ * bloom_dev: the bloom image, upsampled level 0 of oxc_bloom's chain, (width / 2) x (height / 2) float4, read and required only under
+ * OXC_SCENE_HAS_BLOOM (16-byte aligned).  Flags read: HAS_EYE_ADAPTATION, HAS_BLOOM, HAS_CHROMATIC_ABERRATION, HAS_VIGNETTE,
+ * HAS_FILM_GRAIN, TRANSPARENT_BACKGROUND; the others are ignored.  No scratch, so the call is graph-capturable from its first call.
+ * Settings: the PostProcessSettings push constants, the pp.exposure cvar (1.0), pp.bloom_intensity (0.1), the component defaults
+ * (vignette 0.5, chromatic aberration 0.5, film grain amount 0.6 and scale 0.7), TonemappingComponent's AgX, seed = frame count % 16.
+ * Refused with OXC_E_INVALID, before anything is launched: a NULL required argument; a zero extent or one above 32768; frame_dev or
+ * out_dev not 16-byte aligned, a required bloom_dev not 16-byte or exposure_dev not 8-byte aligned; tonemap_type above OXC_TONEMAP_GT7;
+ * OXC_SCENE_HAS_BLOOM with width or height below 2 (no bloom image exists); out_dev sharing a byte with the frame or a required input
+ * (in place included: the chromatic aberration taps read other pixels).  NaN, Inf and denormal settings, records and pixels are
+ * accepted and follow the rules below.
+ * SPECIFICATION (oracle/oxc_oracle_tonemap.c orc_tonemap), the rules of oxc_eye_adaptation and oxc_bloom (binary32, no contraction,
+ * written order, max / min NaN rules, clamp(x, a, b) = min(max(x, a), b), saturate = clamp(x, 0, 1), lerp(a, b, t) = a + (b - a) * t,
+ * mul(M, v) = row . v with dot(a, b) = (a.x*b.x + a.y*b.y) + a.z*b.z, mul(A, B) likewise, a scalar times a vector per component,
+ * constants the binary32 roundings of the literals); every stored NaN is 0x7FFFFFFF.  Items 5-9 settle what the reference leaves open
+ * and are commitments:
+ *   1. taps: SampleLevel of a float4 plane through the pass's {linear, linear} sampler; its address mode is vuk's default, which is not
+ *      in the reference tree: committed to Repeat (Vulkan's zero value).  The bilinear rule of oxc_bloom item 1 on all four channels,
+ *      with texel indices wrapped into 0..n-1 (wrap_index): so column 0 blends with the last column at the left edge.  NaN-safe: the
+ *      floor goes through the saturating sat_i32 and a NaN coordinate gives NaN weights.
+ *   2. pixel (x, y): tex_coord uv = ((f32(x) + 0.5) / f32(width), (f32(y) + 0.5) / f32(height)) (bloom item 2's rule); source = the
+ *      frame's tap at uv.  u * width - 0.5 need not be the integer x, and the rule computes a00 + wx * (a10 - a00) even at wx = 0, so a
+ *      non-finite neighbour can reach a pixel.  color = source.rgb * exposure, the record's exposure under HasEyeAdaptation, else
+ *      settings->exposure; under HasBloom color += tap(bloom, uv).rgb * bloom_intensity (a bilinear upscale, wrapping at the edges).
+ *   3. curve, by tonemap_type: NONE none; ACES ACES_Fitted (ACESInputMat, RRTAndODTFit a = v * (v + 0.0245786) - 0.000090537, b = v *
+ *      (0.983729 * v + 0.4329510) + 0.238081, a / b, ACESOutputMat, saturate): outputs in [0, 1]; AGX AgX_DS (max(c, 0), the matrix,
+ *      clamp(DualSection(x, 0.1, 1), 0, 1) with DualSection = x < S ? x : peak - (peak - S) * exp((-C * (x - S)) / peak), desaturation
+ *      dot with (0.2126729, 0.7151522, 0.0721750), clamp(lerp(d, c, 1.3), 0, 1), the inverse matrix): not bounded, the inverse comes
+ *      after the last clamp; GT7 initializeAsSDR + applyToneMapping with the ICtCp UCS in Rec.2020 through com::rec709_to_rec2020 /
+ *      rec2020_to_rec709 (via XYZ, two mat . v each way): its Rec.2020 output lies in [0, 1] (min(blended, 2.5) * 0.4, NaN -> 1).
+ *   4. chromatic aberration (HasChromaticAberration) REPLACES the colour: its three taps read the raw frame, without exposure, bloom or
+ *      curve (reference behaviour).  rg = FfxLensGetRGMag(amount) per call; c = screen_size / 2 in integers; red / green tap at
+ *      ((f32(x - c.x) * mag + f32(c.x)) + 0.5) * (1 / f32(2 * c.x)) (y likewise), the .r / .g of the tap; the blue tap at f32(x) *
+ *      (1 / f32(2 * c.x)), the pixel's corner, without the + 0.5, its .b.  For an odd width 1 / f32(2 c) is not 1 / width.  At width or
+ *      height 1, c = 0 and the coordinates follow IEEE arithmetic (inf, NaN) and item 1's NaN rule; the call is not refused.
+ *   5. vignette (HasVignette), before the grain as fs_main calls them: m = canonical_cos((f32(|x - c.x|) / f32(c.x) * amount) * fl(PI
+ *      * 0.25)) per axis, squared twice, color *= clamp(m.x * m.y, 0, 1); exactly 1 at the centre pixel.
+ *   6. film grain (HasFilmGrain): d = sat_i32(scale / 8) (truncating, saturating, NaN -> 0); the quotient coord / d in i32, truncating,
+ *      converted to u32 (a negative one wraps); d = 0, which every scale in (-8, 8) gives (the component's 0.7 included) and which the
+ *      shader leaves undefined, gives the quotient -1, all ones, in both components (an explicit branch).  pcg3d16((q.x, q.y, seed)) in
+ *      u32 arithmetic mod 2^32; r = f32(v) * 2^-16 - 0.5; simplex(f32(coord) / scale + r) with round() = rint (ties to even, HLSL's
+ *      rule; GLSL.std.450 leaves halves open); grain = 1 - 2 * exp2(-length(p) * 3); color += (grain * min(color, 1 - color)) * amount.
+ *   7. alpha: the source tap's alpha under TransparentBackground, else 1.
+ *   8. transcendentals: exp canonical_exp, log2 canonical_log2, pow canonical_pow, exp2(x) canonical_pow(2, x), cos canonical_cos
+ *      (oxc_exact.cuh; the oracle's orc_*_canonical); sqrt and / are IEEE.
+ *   9. constants that do not depend on the call, formed once in binary32 in shader order with the same functions (the values the
+ *      library keeps as hex and the tests recompute): AgX's sRGB_to_adjusted = mul(sRGB_to_XYZ, XYZ_to_adjusted) as the code writes it
+ *      (color_PrimariesToMatrix, color_ComputeCompressionMatrix with compression 0.15, tonemap.slang's inverse) and its inverse; the
+ *      DualSection constants; GT7's kA, kB, kC, linearSection * peak, the target 2.5, its UCS intensity, the SDR factor 0.4, 1 - 0.6, 1 / m1,
+ *      1 / m2; simplex's F2 and G2.  The unused shader paths (agx_tonemapping, the Jzazbz UCS, initializeAsHDR) are not part of it.
+ *   10. output: binary32 RGBA, the value before the reference's store into the caller's attachment format (deviation: that conversion
+ *      is not bit-defined). */
+#define OXC_TONEMAP_NONE 0u /* TonemapType */
+#define OXC_TONEMAP_ACES 1u
+#define OXC_TONEMAP_AGX 2u
+#define OXC_TONEMAP_GT7 3u
+typedef struct OxcTonemapSettings {
+  uint32_t scene_flags;               /* OXC_SCENE_*: the six flags above are read */
+  uint32_t tonemap_type;              /* OXC_TONEMAP_* */
+  float exposure;                     /* pp.exposure, read without HasEyeAdaptation */
+  float bloom_intensity;              /* pp.bloom_intensity */
+  float chromatic_aberration_amount;
+  float vignette_amount;
+  float film_grain_scale;
+  float film_grain_amount;
+  uint32_t film_grain_seed;
+} OxcTonemapSettings;
+OXC_STATIC_ASSERT(sizeof(OxcTonemapSettings) == 36, "TonemapSettings");
+int oxc_tonemap(OxcContext* ctx, const float* frame_dev, uint32_t width, uint32_t height, const OxcTonemapSettings* settings,
+                const OxcExposure* exposure_dev, const float* bloom_dev, float* out_dev, void* stream);
+
 int oxc_get_outputs(OxcContext* ctx, OxcOutputs* out);
 /* Instrumentation hook: 128 u64 counters that builds with -DOXC_RASTER_STATS fill (tools/raster_stats.py); zero otherwise. */
 void* oxc_debug_stats_ptr(OxcContext* ctx);
@@ -1484,6 +1558,13 @@ int oxr_eye_adaptation(OxrRenderer* r, const OxcEyeAdaptationSettings* settings,
  * any oxr_apply_pbr* call or for a frame below 2 x 2; OXC_E_CAPACITY, with the camera path left usable, when the chains cannot be
  * allocated.  The frame's outputs and the lit plane are left as they were. */
 int oxr_bloom(OxrRenderer* r, const OxcBloomSettings* settings, float* bloom_host);
+/* Tonemap (PostProcess.cpp:205-247) of the same lit plane, on the renderer's stream, synchronous: oxc_tonemap into a plane the renderer
+ * owns (allocated at the first call), reading the renderer's exposure record under OXC_SCENE_HAS_EYE_ADAPTATION and its bloom image
+ * (upsampled level 0) under OXC_SCENE_HAS_BLOOM.  rgba_host (may be NULL) receives width x height float4.  OXC_E_INVALID before any
+ * oxr_apply_pbr* call; OXC_E_STATE under HasEyeAdaptation before an oxr_eye_adaptation and under HasBloom before an oxr_bloom;
+ * OXC_E_CAPACITY, with the camera path left usable, when the plane cannot be allocated.  The lit plane, the record and the bloom chains
+ * are left as they were. */
+int oxr_tonemap(OxrRenderer* r, const OxcTonemapSettings* settings, float* rgba_host);
 
 /* ------------------------------------------------------------------------------------------------
  * oxb_* — mesh builder (SURVEY §8f.2): host-side producer of the blob layout above, mirroring build_gltf_mesh

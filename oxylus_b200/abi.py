@@ -563,6 +563,28 @@ def bloom_chain_texels(width: int, height: int) -> int:
     return sum(w * h for w, h, _ in bloom_levels(width, height))
 
 
+TONEMAP_NONE, TONEMAP_ACES, TONEMAP_AGX, TONEMAP_GT7 = 0, 1, 2, 3
+
+
+class TonemapSettings(C.Structure):
+    """OxcTonemapSettings: the tonemap's scene flags and curve, the pp.* cvars and the lens components' settings"""
+    _fields_ = [("scene_flags", C.c_uint32), ("tonemap_type", C.c_uint32), ("exposure", C.c_float), ("bloom_intensity", C.c_float),
+                ("chromatic_aberration_amount", C.c_float), ("vignette_amount", C.c_float), ("film_grain_scale", C.c_float),
+                ("film_grain_amount", C.c_float), ("film_grain_seed", C.c_uint32)]
+
+
+assert C.sizeof(TonemapSettings) == 36
+
+
+def tonemap_settings(scene_flags=0, tonemap_type=TONEMAP_AGX, exposure=1.0, bloom_intensity=0.1, chromatic_aberration_amount=0.5,
+                     vignette_amount=0.5, film_grain_scale=0.7, film_grain_amount=0.6, film_grain_seed=0):
+    """TonemapSettings with the reference's defaults: TonemappingComponent's AgX, the pp.exposure and pp.bloom_intensity cvars, the
+    vignette, chromatic aberration and film grain components; the seed is the frame count % 16"""
+    f = [float(np.float32(v)) for v in (exposure, bloom_intensity, chromatic_aberration_amount, vignette_amount, film_grain_scale,
+                                        film_grain_amount)]
+    return TonemapSettings(int(scene_flags), int(tonemap_type), *f, int(film_grain_seed) & 0xFFFFFFFF)
+
+
 def atmosphere(**overrides):
     """Atmosphere with the GPU::Atmosphere{} defaults and the reference's LUT sizes; any field may be overridden by name"""
     a = Atmosphere()

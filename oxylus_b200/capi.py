@@ -24,6 +24,7 @@ SYMBOLS = [
     "oxc_vsm_draw_pages", "oxc_vsm_draw_stats", "oxc_vsm_resolve_shadows", "oxc_generate_ambient_occlusion", "oxc_apply_pbr",
     "oxc_contact_shadows", "oxc_atmosphere_transmittance", "oxc_atmosphere_sky_luts", "oxc_atmosphere_sky_ibl", "oxc_apply_pbr_atmosphere", "oxr_apply_pbr_atmosphere",
     "oxc_eye_adaptation", "oxc_bloom", "oxc_bloom_level_count", "oxc_bloom_chain_texels", "oxr_eye_adaptation", "oxr_bloom",
+    "oxc_tonemap", "oxr_tonemap",
     "oxc_get_outputs", "oxc_check_status", "oxc_mark_hiz_dirty", "oxc_bind_camera_buffer", "oxc_load_camera", "oxc_debug_stats_ptr",
     "oxc_mgpu_get_unique_id", "oxc_mgpu_init", "oxc_mgpu_init_with_comm", "oxc_mgpu_shutdown", "oxc_mgpu_info", "oxc_mgpu_exchange_hiz",
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
@@ -171,6 +172,8 @@ def load(build_if_missing=True):
     lib.oxc_bloom.argtypes = [vp, vp, u32, u32, C.POINTER(abi.BloomSettings), vp, C.POINTER(abi.BloomTargets), vp]
     lib.oxr_eye_adaptation.argtypes = [vp, C.POINTER(abi.EyeAdaptationSettings), C.c_float, C.POINTER(abi.Exposure)]
     lib.oxr_bloom.argtypes = [vp, C.POINTER(abi.BloomSettings), vp]
+    lib.oxc_tonemap.argtypes = [vp, vp, u32, u32, C.POINTER(abi.TonemapSettings), vp, vp, vp, vp]
+    lib.oxr_tonemap.argtypes = [vp, C.POINTER(abi.TonemapSettings), vp]
     lib.oxc_bloom_level_count.restype, lib.oxc_bloom_level_count.argtypes = u32, [u32, u32]
     lib.oxc_bloom_chain_texels.restype, lib.oxc_bloom_chain_texels.argtypes = C.c_uint64, [u32, u32]
     _LIB = lib
@@ -549,6 +552,13 @@ class Context:
         t = abi.BloomTargets(*[None if a is None else int(a) for a in (downsampled_dev, upsampled_dev)])
         _check(self.lib.oxc_bloom(self.h, _ptr(frame_dev), w, h, C.byref(settings), _ptr(exposure_dev), C.byref(t), self.stream), "oxc_bloom")
 
+    def tonemap(self, frame_dev, w, h, settings, exposure_dev, bloom_dev, out_dev):
+        """oxc_tonemap: the exposure, bloom composite, curve and lens effects of a w x h float4 frame into out_dev (w x h float4).
+        settings: abi.TonemapSettings; exposure_dev is read under SCENE_HAS_EYE_ADAPTATION only, bloom_dev ((w // 2) x (h // 2) float4,
+        upsampled level 0 of bloom's chain) under SCENE_HAS_BLOOM only"""
+        _check(self.lib.oxc_tonemap(self.h, _ptr(frame_dev), w, h, C.byref(settings), _ptr(exposure_dev), _ptr(bloom_dev), _ptr(out_dev),
+                                    self.stream), "oxc_tonemap")
+
     def atmosphere_transmittance(self, atmosphere, lut_dev):
         """oxc_atmosphere_transmittance: the transmittance LUT (binary16 RGBA, atmosphere.transmittance_lut_size) into lut_dev"""
         _check(self.lib.oxc_atmosphere_transmittance(self.h, C.byref(atmosphere), _ptr(lut_dev), self.stream), "oxc_atmosphere_transmittance")
@@ -893,6 +903,13 @@ class Renderer:
         with the renderer's exposure record under SCENE_HAS_EYE_ADAPTATION"""
         out = np.zeros((self.scene.height // 2, self.scene.width // 2, 4), dtype=np.float32)
         _check(self.lib.oxr_bloom(self.h, C.byref(settings), _ptr(out)), "oxr_bloom")
+        return out
+
+    def tonemap(self, settings):
+        """oxr_tonemap: the tonemapped frame (float32 [height, width, 4]) of the lit plane of the last apply_pbr* call, with the
+        renderer's exposure record under SCENE_HAS_EYE_ADAPTATION and its bloom image under SCENE_HAS_BLOOM"""
+        out = np.zeros((self.scene.height, self.scene.width, 4), dtype=np.float32)
+        _check(self.lib.oxr_tonemap(self.h, C.byref(settings), _ptr(out)), "oxr_tonemap")
         return out
 
     def apply_pbr(self, cam, settings, lights=None, cast_shadows=False, gtao_camera=None, gtao_settings=None, pbr_camera=None,

@@ -145,7 +145,7 @@ RendererInstance::~RendererInstance() {
   if (stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(stream_));
   cudaFree(d_vis64_); cudaFree(d_vis32_); cudaFree(d_depth_); cudaFree(d_occluder_); cudaFree(d_overdraw_); cudaFree(d_gbuffer_);
   cudaFree(d_uv_normal_); cudaFree(d_gtao_); cudaFree(d_pbr_); cudaFree(d_lights_); cudaFree(d_contact_); cudaFree(d_atmosphere_); cudaFree(d_sky_ibl_cube_);
-  cudaFree(d_post_); cudaFree(d_bloom_);
+  cudaFree(d_post_); cudaFree(d_bloom_); cudaFree(d_tonemap_);
   if (h_pinned_) cudaFreeHost(h_pinned_);
   if (copy_stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(copy_stream_));
   for (auto& sl : slots_) {
@@ -529,7 +529,24 @@ auto RendererInstance::bloom(const OxcBloomSettings& settings, float* bloom_host
   const OxcExposure* record = adapt ? reinterpret_cast<const OxcExposure*>(d_post_ + OXC_HISTOGRAM_BIN_COUNT) : nullptr;
   int rc;
   if ((rc = oxc_bloom(ctx_, d_pbr_, width_, height_, &settings, record, &targets, stream_)) != OXC_OK) return fail(rc);
-  return copy_to_host({{bloom_host, targets.upsampled, (size_t)(width_ / 2) * (height_ / 2) * 16}});
+  if ((rc = copy_to_host({{bloom_host, targets.upsampled, (size_t)(width_ / 2) * (height_ / 2) * 16}})) != OXC_OK) return rc;
+  bloomed_ = true;
+  return OXC_OK;
+}
+
+// tonemap on stream_, synchronous: the output plane is allocated at the first call
+auto RendererInstance::tonemap(const OxcTonemapSettings& settings, float* rgba_host) -> int {
+  if (!ctx_ || !error_.empty()) return OXC_E_STATE;
+  if (!pbr_lit_ || settings.tonemap_type > OXC_TONEMAP_GT7) return OXC_E_INVALID; // no lit plane yet, or no such curve
+  const bool adapt = (settings.scene_flags & OXC_SCENE_HAS_EYE_ADAPTATION) != 0, bloom = (settings.scene_flags & OXC_SCENE_HAS_BLOOM) != 0;
+  if ((adapt && !d_post_) || (bloom && !bloomed_)) return OXC_E_STATE; // no record before an eye_adaptation, no image before a bloom
+  const size_t px = (size_t)width_ * height_;
+  if (optional_plane(&d_tonemap_, px * 16) != OXC_OK) return OXC_E_CAPACITY;
+  const OxcExposure* record = adapt ? reinterpret_cast<const OxcExposure*>(d_post_ + OXC_HISTOGRAM_BIN_COUNT) : nullptr;
+  const float* image = bloom ? d_bloom_ + oxc_bloom_chain_texels(width_, height_) * 4 : nullptr; // upsampled level 0
+  int rc;
+  if ((rc = oxc_tonemap(ctx_, d_pbr_, width_, height_, &settings, record, image, d_tonemap_, stream_)) != OXC_OK) return fail(rc);
+  return copy_to_host({{rgba_host, d_tonemap_, px * 16}});
 }
 
 // the contact_shadows pass (RendererInstance.cpp:990-1020) on stream_, synchronous: the last frame's depth, the pass into the renderer's
@@ -1149,6 +1166,11 @@ int oxr_eye_adaptation(OxrRenderer* r, const OxcEyeAdaptationSettings* settings,
 int oxr_bloom(OxrRenderer* r, const OxcBloomSettings* settings, float* bloom_host) {
   if (!r || !settings) return OXC_E_INVALID;
   return r->impl.bloom(*settings, bloom_host);
+}
+
+int oxr_tonemap(OxrRenderer* r, const OxcTonemapSettings* settings, float* rgba_host) {
+  if (!r || !settings) return OXC_E_INVALID;
+  return r->impl.tonemap(*settings, rgba_host);
 }
 
 int oxr_contact_shadows(OxrRenderer* r, const OxcContactShadowCamera* contact_camera, const OxcContactShadowSettings* settings,

@@ -111,6 +111,9 @@ public:
   // bloom (PostProcess.cpp:79-203) of the same plane into the renderer's two chains, reading the record under HasEyeAdaptation;
   // upsampled level 0 ((width / 2) x (height / 2) float4) to the host when non-null
   auto bloom(const OxcBloomSettings& settings, float* bloom_host) -> int;
+  // the tonemap (PostProcess.cpp:205-247) of the same plane into the renderer's tonemap plane, reading the record under
+  // HasEyeAdaptation and upsampled level 0 of the bloom chain under HasBloom; width x height float4 to the host when non-null
+  auto tonemap(const OxcTonemapSettings& settings, float* rgba_host) -> int;
 
   // RendererInstance::render geometry section: run_geometry_pass(false) -> generate_hiz -> run_geometry_pass(true)
   auto render(const OxcCullCamera& camera, const float* occluder_depth_host, uint32_t* vis32_host, float* depth_host,
@@ -209,6 +212,8 @@ private:
   bool pbr_lit_ = false;               // d_pbr_ holds the output of a successful apply_pbr
   uint32_t* d_post_ = nullptr;         // the eye-adaptation histogram (256 u32), then the exposure record, from the first eye_adaptation
   float* d_bloom_ = nullptr;           // bloom's downsampled chain, then its upsampled chain, from the first bloom
+  bool bloomed_ = false;               // d_bloom_ holds the chains of a successful bloom
+  float* d_tonemap_ = nullptr;         // the tonemap's output plane (float4 per pixel), from the first tonemap
   int sky_ibl_device(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3], float sun_intensity);
   OxcLight* d_lights_ = nullptr;    // apply_pbr's lights buffer (OXC_MAX_LIGHTS records), allocated with d_pbr_
   bool has_external_depth_ = false;

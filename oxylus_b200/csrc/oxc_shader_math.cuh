@@ -25,6 +25,12 @@ OXC_DI int sat_i32(float f) { return !(f == f) ? 0 : (f >= 2147483648.0f ? INT_M
 OXC_DI uint32_t sat_u32(float f) { return !(f > 0.0f) ? 0u : (f >= 4294967296.0f ? 0xFFFFFFFFu : (uint32_t)f); }
 // a texel index clamped to the edge of an extent n >= 1
 OXC_DI int clamp_index(long long i, int n) { return (int)(i < 0 ? 0 : (i > n - 1 ? n - 1 : i)); }
+// a texel index wrapped into an extent n >= 1 (the Repeat address mode); an index already inside skips the division
+OXC_DI int wrap_index(long long i, int n) {
+  if (i >= 0 && i < n) return (int)i;
+  const long long r = i % n;
+  return (int)(r < 0 ? r + n : r);
+}
 
 // the blend of two mip levels' values: (1 - f) * lo + f * hi
 OXC_DI float lerp_levels(float f, float lo, float hi) { return fa(fm(fs(1.0f, f), lo), fm(f, hi)); }

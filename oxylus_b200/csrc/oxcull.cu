@@ -33,6 +33,7 @@
 #include "kernels_pbr_atmosphere.cuh"
 #include "kernels_exposure.cuh"
 #include "kernels_bloom.cuh"
+#include "kernels_tonemap.cuh"
 
 using namespace oxc;
 
@@ -1726,6 +1727,37 @@ int oxc_bloom(OxcContext* c, const float* frame_dev, uint32_t w, uint32_t h, con
     k_bloom_upsample<<<bloom_grid(p, i - 1), BLOOM_THREADS, 0, s>>>(p, i);
     LAUNCHED();
   }
+  return OXC_OK;
+}
+
+int oxc_tonemap(OxcContext* c, const float* frame_dev, uint32_t w, uint32_t h, const OxcTonemapSettings* settings, const OxcExposure* exposure_dev,
+                const float* bloom_dev, float* out_dev, void* stream) {
+  if (!c || !frame_dev || !settings || !out_dev) return fail(OXC_E_INVALID, "null argument");
+  const bool adapt = (settings->scene_flags & OXC_SCENE_HAS_EYE_ADAPTATION) != 0, bloom = (settings->scene_flags & OXC_SCENE_HAS_BLOOM) != 0;
+  if (adapt && !exposure_dev) return fail(OXC_E_INVALID, "null argument: HasEyeAdaptation reads exposure_dev");
+  if (bloom && !bloom_dev) return fail(OXC_E_INVALID, "null argument: HasBloom reads bloom_dev");
+  int rc;
+  if ((rc = check_extent(w, h)) != OXC_OK) return rc;
+  if (misaligned(16, frame_dev, out_dev)) return fail(OXC_E_INVALID, "frame_dev and out_dev must be 16-byte aligned");
+  if (adapt && misaligned(8, exposure_dev)) return fail(OXC_E_INVALID, "exposure_dev must be 8-byte aligned");
+  if (bloom && misaligned(16, bloom_dev)) return fail(OXC_E_INVALID, "bloom_dev must be 16-byte aligned");
+  if (settings->tonemap_type > OXC_TONEMAP_GT7) return fail(OXC_E_INVALID, "tonemap_type %u above OXC_TONEMAP_GT7", settings->tonemap_type);
+  if (bloom && (w < 2 || h < 2)) return fail(OXC_E_INVALID, "extent %u x %u below 2 x 2 under HasBloom: there is no bloom image", w, h);
+  const uint64_t frame_bytes = (uint64_t)w * h * 16, bloom_bytes = (uint64_t)(w / 2) * (h / 2) * 16;
+  if (overlaps(out_dev, frame_bytes, frame_dev, frame_bytes) || (adapt && overlaps(out_dev, frame_bytes, exposure_dev, 8)) ||
+      (bloom && overlaps(out_dev, frame_bytes, bloom_dev, bloom_bytes)))
+    return fail(OXC_E_INVALID, "out_dev overlaps frame_dev, exposure_dev or bloom_dev");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  const TonemapParams p = tonemap_make_params(frame_dev, w, h, *settings, exposure_dev, bloom_dev, out_dev);
+  const dim3 grid = tiles(w, h, TONEMAP_TILE_X, TONEMAP_TILE_Y);
+  switch (settings->tonemap_type) {
+  case OXC_TONEMAP_NONE: k_tonemap<OXC_TONEMAP_NONE><<<grid, TONEMAP_THREADS, 0, s>>>(p); break;
+  case OXC_TONEMAP_ACES: k_tonemap<OXC_TONEMAP_ACES><<<grid, TONEMAP_THREADS, 0, s>>>(p); break;
+  case OXC_TONEMAP_AGX: k_tonemap<OXC_TONEMAP_AGX><<<grid, TONEMAP_THREADS, 0, s>>>(p); break;
+  default: k_tonemap<OXC_TONEMAP_GT7><<<grid, TONEMAP_THREADS, 0, s>>>(p); break;
+  }
+  LAUNCHED();
   return OXC_OK;
 }
 
