@@ -1362,6 +1362,63 @@ OXC_STATIC_ASSERT(sizeof(OxcTonemapSettings) == 36, "TonemapSettings");
 int oxc_tonemap(OxcContext* ctx, const float* frame_dev, uint32_t width, uint32_t height, const OxcTonemapSettings* settings,
                 const OxcExposure* exposure_dev, const float* bloom_dev, float* out_dev, void* stream);
 
+/* FXAA (RendererInstance.cpp:1225-1255, passes/fxaa/fxaa.slang fs_main): the anti-aliasing pass between PBR apply and the post chain.
+ * The reference runs it under HasFXAA (OXC_SCENE_HAS_FXAA, the pp.fxaa cvar, on by default) on the HDR frame, before eye adaptation,
+ * bloom and the tonemap, and its output becomes the frame those three read (std::tie(final_attachment, ...) = fxaa_pass(...)).  The
+ * caller gates the call on HasFXAA, as the reference's `if` does.  One thread per pixel of a width x height frame: the 3 x 3 luma
+ * neighbourhood, the early exit, the walk along the edge, the sub-pixel term and one final tap, into out_dev (float4 per pixel,
+ * row-major).  frame_dev: the lit frame as either PBR apply writes it, float4, 16-byte aligned.  No settings: the reference has none.
+ * No scratch, so the call is graph-capturable from its first call.
+ * Refused with OXC_E_INVALID, before anything is launched: a NULL argument; a zero extent or one above 32768; frame_dev or out_dev not
+ * 16-byte aligned; out_dev sharing a byte with frame_dev (in place included: the taps read other pixels).  NaN, Inf, denormal and
+ * negative pixels are accepted and follow the rules below.
+ * SPECIFICATION (oracle/oxc_oracle_fxaa.c orc_fxaa), binary32, no contraction, each expression in the shader's written order, left to
+ * right; max / min with the NaN rules of oxc_apply_pbr (a NaN operand yields the other one, vmax / vmin); clamp(x, 0, 1) = min(max(x,
+ * 0), 1); sqrt and / are IEEE; abs is fabs; every stored NaN is 0x7FFFFFFF:
+ *   1. pixel and step: pixel (x, y) has tex_coord uv = ((f32(x) + 0.5) / f32(width), (f32(y) + 0.5) / f32(height)) (oxc_tonemap item 2's
+ *      rule); inv = (1 / f32(width), 1 / f32(height)), the push constant inverse_screen_size, formed once per call.
+ *   2. taps: Sample(uv) is oxc_bloom item 1's bilinear rule on all four channels with ClampToEdge (LinearSamplerClamped, the sampler of
+ *      bloom's upsample): x = u * W - 0.5, x0 = floor(x), wx = x - x0 (y likewise), texels x0, x0 + 1 / y0, y0 + 1 clamped into the
+ *      frame (NaN-safe: the floor goes through the saturating sat_i32, a NaN coordinate gives NaN weights).  The frame has one level, so
+ *      the implicit-LOD Sample reads level 0.  Sample(uv, int2(dx, dy)) adds the constant offset to the unnormalised coordinate before
+ *      the half-texel shift: x = (u * W + dx) - 0.5 (y likewise).  That is Vulkan's texel-offset order; the Vulkan specification is not
+ *      in the reference tree, so this order is a commitment.  u * W - 0.5 need not be the integer x, and the rule computes a00 + wx *
+ *      (a10 - a00) even at wx = 0: a centre or cross tap is a real bilinear tap, not a texel load, and a non-finite neighbour can reach
+ *      a pixel.
+ *   3. luma(c) = sqrt((c.r * 0.299 + c.g * 0.587) + c.b * 0.114) with bloom's binary32 weights (0x3E991687, 0x3F1645A2, 0x3DE978D5);
+ *      a negative sum gives NaN.
+ *   4. early exit: luma_center = luma(Sample(uv)); luma_down, _up, _left, _right of the offsets (0, -1), (0, 1), (-1, 0), (1, 0);
+ *      luma_min = min(center, min(min(down, up), min(left, right))), luma_max likewise with max, range = luma_max - luma_min.  If range <
+ *      max(0.0312, luma_max * 0.125) the output is the centre tap.  A NaN range fails the comparison and goes on to the walk.
+ *   5. the rest of fs_main, line by line: the corners (-1, -1), (1, 1), (-1, 1), (1, -1); down_up = down + up, left_right = left + right,
+ *      left_corners = down_left + up_left, down_corners = down_left + down_right, right_corners = down_right + up_right, up_corners =
+ *      up_right + up_left; edge_horizontal = (abs(-2 * left + left_corners) + abs(-2 * center + down_up) * 2) + abs(-2 * right +
+ *      right_corners), edge_vertical = (abs(-2 * up + up_corners) + abs(-2 * center + left_right) * 2) + abs(-2 * down + down_corners);
+ *      is_horizontal = edge_horizontal >= edge_vertical; step = is_horizontal ? inv.y : inv.x; luma1, luma2 = is_horizontal ? (down,
+ *      up) : (left, right); gradient1 = luma1 - center, gradient2 = luma2 - center; is1_steepest = abs(gradient1) >= abs(gradient2);
+ *      gradient_scaled = 0.25 * max(abs(gradient1), abs(gradient2)); if is1_steepest: step = -step, local_average = 0.5 * (luma1 +
+ *      center), else 0.5 * (luma2 + center); current = uv with current.y (horizontal) or .x += step * 0.5; offset = is_horizontal ?
+ *      (inv.x, 0) : (0, inv.y); uv1 = current - offset * QUALITY(0), uv2 = current + offset * QUALITY(0); end1 = luma(Sample(uv1)) -
+ *      local_average, end2 likewise; reached1 = abs(end1) >= gradient_scaled, reached2 likewise; uv1 -= offset * QUALITY(1) unless
+ *      reached1, uv2 += ... unless reached2; unless both are reached, for i = 2..11: end1 = luma(Sample(uv1)) - local_average unless
+ *      reached1, end2 likewise, both reached flags recomputed, uv1 -= offset * QUALITY(i) unless reached1, uv2 += ... unless reached2,
+ *      and then break when both are reached (the break comes after that step's advance).  end1 and end2 keep their last values for the
+ *      variation test.  QUALITY(i) = 1 for i <= 4, 1.5 at 5, 2 for 6..9, 4 at 10, 8 at 11.  distance1 = is_horizontal ? uv.x - uv1.x :
+ *      uv.y - uv1.y, distance2 = is_horizontal ? uv2.x - uv.x : uv2.y - uv.y; is_direction1 = distance1 < distance2; distance_final =
+ *      min(distance1, distance2); edge_thickness = distance1 + distance2; center_smaller = center < local_average; correct_variation =
+ *      is_direction1 ? ((end1 < 0) != center_smaller) : ((end2 < 0) != center_smaller); pixel_offset = (-distance_final /
+ *      edge_thickness) + 0.5; final_offset = correct_variation ? pixel_offset : 0; luma_average = (1 / 12) * (((2 * (down_up +
+ *      left_right)) + left_corners) + right_corners); sub1 = clamp(abs(luma_average - center) / range, 0, 1); sub2 = ((-2 * sub1 + 3) *
+ *      sub1) * sub1; sub_final = (sub2 * sub2) * 0.75; final_offset = max(final_offset, sub_final); final_uv = uv with final_uv.y
+ *      (horizontal) or .x += final_offset * step.  A uv component whose offset component is 0 stays bit-identical (uv - 0 * q = uv), so
+ *      an implementation may advance only the moving axis.  At most 32 bilinear taps per pixel (1 centre, 4 cross, 4 corners, 2 first
+ *      ends, 2 x 10 in the walk, 1 final); the farthest lies 18.5 texels along the edge.
+ *   6. constants, the binary32 roundings of the literals: 0.0312 = 0x3CFF9724, 0.125, 0.75, 1.0 / 12.0 = 0x3DAAAAAB (the binary32
+ *      quotient and the rounding of the binary64 quotient agree, so the literal's type does not matter).
+ *   7. output: Sample(final_uv), or the centre tap on the early exit, all four channels: alpha is filtered like the colour.  A binary32
+ *      float4 plane; deviation: it is not converted to the reference's hdr_format attachment (that conversion is not bit-defined). */
+int oxc_fxaa(OxcContext* ctx, const float* frame_dev, uint32_t width, uint32_t height, float* out_dev, void* stream);
+
 int oxc_get_outputs(OxcContext* ctx, OxcOutputs* out);
 /* Instrumentation hook: 128 u64 counters that builds with -DOXC_RASTER_STATS fill (tools/raster_stats.py); zero otherwise. */
 void* oxc_debug_stats_ptr(OxcContext* ctx);
@@ -1546,25 +1603,34 @@ int oxr_atmosphere_luts(OxrRenderer* r, const OxcAtmosphere* atmosphere, const O
  * planes cannot be allocated; a failed call does not advance the count. */
 int oxr_atmosphere_sky_ibl(OxrRenderer* r, const OxcAtmosphere* atmosphere, const OxcPbrCamera* camera, const float sun_direction[3],
                            float sun_intensity, uint16_t* cube_host);
-/* Eye adaptation (PostProcess.cpp:7-77) on the lit plane of the renderer's last oxr_apply_pbr* call, on the renderer's stream,
- * synchronous: oxc_eye_adaptation into the renderer's exposure record and histogram.  The first call allocates both and fills the record
+/* The post chain's source: oxr_eye_adaptation, oxr_bloom and oxr_tonemap read the lit plane of the renderer's last oxr_apply_pbr* call,
+ * or, after a successful oxr_fxaa, the FXAA plane, as the reference's final_attachment becomes FXAA's output.  The next oxr_apply_pbr*
+ * makes the lit plane the source again.
+ * Eye adaptation (PostProcess.cpp:7-77) on the post chain's source, on the renderer's stream, synchronous: oxc_eye_adaptation into the renderer's exposure record and histogram.  The first call allocates both and fills the record
  * with (1, 1), as the reference's vuk::fill does; the record persists across calls.  exposure_host (may be NULL) receives the record
  * after the call.  OXC_E_INVALID before any oxr_apply_pbr* call; OXC_E_CAPACITY, with the camera path left usable, when the record cannot
- * be allocated.  The frame's outputs and the lit plane are left as they were. */
+ * be allocated.  The frame's outputs and the source plane are left as they were. */
 int oxr_eye_adaptation(OxrRenderer* r, const OxcEyeAdaptationSettings* settings, float delta_time, OxcExposure* exposure_host);
-/* Bloom (PostProcess.cpp:79-203) of the same lit plane, on the renderer's stream, synchronous: oxc_bloom into the renderer's two chains
+/* Bloom (PostProcess.cpp:79-203) of the post chain's source, on the renderer's stream, synchronous: oxc_bloom into the renderer's two chains
  * (allocated at the first call), reading the renderer's exposure record under OXC_SCENE_HAS_EYE_ADAPTATION (OXC_E_STATE before an
  * oxr_eye_adaptation then).  bloom_host (may be NULL) receives upsampled level 0, (width / 2) x (height / 2) float4.  OXC_E_INVALID before
  * any oxr_apply_pbr* call or for a frame below 2 x 2; OXC_E_CAPACITY, with the camera path left usable, when the chains cannot be
- * allocated.  The frame's outputs and the lit plane are left as they were. */
+ * allocated.  The frame's outputs and the source plane are left as they were. */
 int oxr_bloom(OxrRenderer* r, const OxcBloomSettings* settings, float* bloom_host);
-/* Tonemap (PostProcess.cpp:205-247) of the same lit plane, on the renderer's stream, synchronous: oxc_tonemap into a plane the renderer
+/* Tonemap (PostProcess.cpp:205-247) of the post chain's source, on the renderer's stream, synchronous: oxc_tonemap into a plane the renderer
  * owns (allocated at the first call), reading the renderer's exposure record under OXC_SCENE_HAS_EYE_ADAPTATION and its bloom image
  * (upsampled level 0) under OXC_SCENE_HAS_BLOOM.  rgba_host (may be NULL) receives width x height float4.  OXC_E_INVALID before any
  * oxr_apply_pbr* call; OXC_E_STATE under HasEyeAdaptation before an oxr_eye_adaptation and under HasBloom before an oxr_bloom;
- * OXC_E_CAPACITY, with the camera path left usable, when the plane cannot be allocated.  The lit plane, the record and the bloom chains
- * are left as they were. */
+ * OXC_E_CAPACITY, with the camera path left usable, when the plane cannot be allocated.  The source plane, the record and the bloom
+ * chains are left as they were. */
 int oxr_tonemap(OxrRenderer* r, const OxcTonemapSettings* settings, float* rgba_host);
+/* FXAA (RendererInstance.cpp:1225-1255) of the lit plane of the renderer's last oxr_apply_pbr* call, on the renderer's stream,
+ * synchronous: oxc_fxaa into a plane the renderer owns (allocated at the first call), which then becomes the post chain's source until
+ * the next oxr_apply_pbr*.  It always reads the lit plane, so a second call gives the same plane.  The caller gates it on HasFXAA and
+ * runs it once per frame, between PBR apply and eye adaptation, as the reference does.  rgba_host (may be NULL) receives width x height
+ * float4.  OXC_E_INVALID before any oxr_apply_pbr* call; OXC_E_CAPACITY, with the camera path left usable, when the plane cannot be
+ * allocated.  The lit plane is left as it was. */
+int oxr_fxaa(OxrRenderer* r, float* rgba_host);
 
 /* ------------------------------------------------------------------------------------------------
  * oxb_* — mesh builder (SURVEY §8f.2): host-side producer of the blob layout above, mirroring build_gltf_mesh

@@ -24,7 +24,7 @@ SYMBOLS = [
     "oxc_vsm_draw_pages", "oxc_vsm_draw_stats", "oxc_vsm_resolve_shadows", "oxc_generate_ambient_occlusion", "oxc_apply_pbr",
     "oxc_contact_shadows", "oxc_atmosphere_transmittance", "oxc_atmosphere_sky_luts", "oxc_atmosphere_sky_ibl", "oxc_apply_pbr_atmosphere", "oxr_apply_pbr_atmosphere",
     "oxc_eye_adaptation", "oxc_bloom", "oxc_bloom_level_count", "oxc_bloom_chain_texels", "oxr_eye_adaptation", "oxr_bloom",
-    "oxc_tonemap", "oxr_tonemap",
+    "oxc_tonemap", "oxr_tonemap", "oxc_fxaa", "oxr_fxaa",
     "oxc_get_outputs", "oxc_check_status", "oxc_mark_hiz_dirty", "oxc_bind_camera_buffer", "oxc_load_camera", "oxc_debug_stats_ptr",
     "oxc_mgpu_get_unique_id", "oxc_mgpu_init", "oxc_mgpu_init_with_comm", "oxc_mgpu_shutdown", "oxc_mgpu_info", "oxc_mgpu_exchange_hiz",
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
@@ -174,6 +174,8 @@ def load(build_if_missing=True):
     lib.oxr_bloom.argtypes = [vp, C.POINTER(abi.BloomSettings), vp]
     lib.oxc_tonemap.argtypes = [vp, vp, u32, u32, C.POINTER(abi.TonemapSettings), vp, vp, vp, vp]
     lib.oxr_tonemap.argtypes = [vp, C.POINTER(abi.TonemapSettings), vp]
+    lib.oxc_fxaa.argtypes = [vp, vp, u32, u32, vp, vp]
+    lib.oxr_fxaa.argtypes = [vp, vp]
     lib.oxc_bloom_level_count.restype, lib.oxc_bloom_level_count.argtypes = u32, [u32, u32]
     lib.oxc_bloom_chain_texels.restype, lib.oxc_bloom_chain_texels.argtypes = C.c_uint64, [u32, u32]
     _LIB = lib
@@ -559,6 +561,10 @@ class Context:
         _check(self.lib.oxc_tonemap(self.h, _ptr(frame_dev), w, h, C.byref(settings), _ptr(exposure_dev), _ptr(bloom_dev), _ptr(out_dev),
                                     self.stream), "oxc_tonemap")
 
+    def fxaa(self, frame_dev, w, h, out_dev):
+        """oxc_fxaa: FXAA of a w x h float4 frame into out_dev (w x h float4, sharing no byte with the frame)"""
+        _check(self.lib.oxc_fxaa(self.h, _ptr(frame_dev), w, h, _ptr(out_dev), self.stream), "oxc_fxaa")
+
     def atmosphere_transmittance(self, atmosphere, lut_dev):
         """oxc_atmosphere_transmittance: the transmittance LUT (binary16 RGBA, atmosphere.transmittance_lut_size) into lut_dev"""
         _check(self.lib.oxc_atmosphere_transmittance(self.h, C.byref(atmosphere), _ptr(lut_dev), self.stream), "oxc_atmosphere_transmittance")
@@ -892,24 +898,32 @@ class Renderer:
         return out
 
     def eye_adaptation(self, settings, delta_time):
-        """oxr_eye_adaptation: eye adaptation on the lit plane of the last apply_pbr* call, into the renderer's persistent exposure record
-        ((1, 1) at the first call); returns the record after the call (abi.Exposure)"""
+        """oxr_eye_adaptation: eye adaptation on the post chain's source (the lit plane of the last apply_pbr* call, or the FXAA plane
+        after fxaa), into the renderer's persistent exposure record ((1, 1) at the first call); returns the record after the call
+        (abi.Exposure)"""
         rec = abi.Exposure()
         _check(self.lib.oxr_eye_adaptation(self.h, C.byref(settings), float(np.float32(delta_time)), C.byref(rec)), "oxr_eye_adaptation")
         return rec
 
     def bloom(self, settings):
-        """oxr_bloom: the bloom image (upsampled level 0, float32 [height // 2, width // 2, 4]) of the lit plane of the last apply_pbr* call,
-        with the renderer's exposure record under SCENE_HAS_EYE_ADAPTATION"""
+        """oxr_bloom: the bloom image (upsampled level 0, float32 [height // 2, width // 2, 4]) of the post chain's source, with the
+        renderer's exposure record under SCENE_HAS_EYE_ADAPTATION"""
         out = np.zeros((self.scene.height // 2, self.scene.width // 2, 4), dtype=np.float32)
         _check(self.lib.oxr_bloom(self.h, C.byref(settings), _ptr(out)), "oxr_bloom")
         return out
 
     def tonemap(self, settings):
-        """oxr_tonemap: the tonemapped frame (float32 [height, width, 4]) of the lit plane of the last apply_pbr* call, with the
-        renderer's exposure record under SCENE_HAS_EYE_ADAPTATION and its bloom image under SCENE_HAS_BLOOM"""
+        """oxr_tonemap: the tonemapped frame (float32 [height, width, 4]) of the post chain's source, with the renderer's exposure
+        record under SCENE_HAS_EYE_ADAPTATION and its bloom image under SCENE_HAS_BLOOM"""
         out = np.zeros((self.scene.height, self.scene.width, 4), dtype=np.float32)
         _check(self.lib.oxr_tonemap(self.h, C.byref(settings), _ptr(out)), "oxr_tonemap")
+        return out
+
+    def fxaa(self):
+        """oxr_fxaa: FXAA (float32 [height, width, 4]) of the lit plane of the last apply_pbr* call; the FXAA plane then becomes the
+        source of eye_adaptation, bloom and tonemap until the next apply_pbr*"""
+        out = np.zeros((self.scene.height, self.scene.width, 4), dtype=np.float32)
+        _check(self.lib.oxr_fxaa(self.h, _ptr(out)), "oxr_fxaa")
         return out
 
     def apply_pbr(self, cam, settings, lights=None, cast_shadows=False, gtao_camera=None, gtao_settings=None, pbr_camera=None,

@@ -145,7 +145,7 @@ RendererInstance::~RendererInstance() {
   if (stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(stream_));
   cudaFree(d_vis64_); cudaFree(d_vis32_); cudaFree(d_depth_); cudaFree(d_occluder_); cudaFree(d_overdraw_); cudaFree(d_gbuffer_);
   cudaFree(d_uv_normal_); cudaFree(d_gtao_); cudaFree(d_pbr_); cudaFree(d_lights_); cudaFree(d_contact_); cudaFree(d_atmosphere_); cudaFree(d_sky_ibl_cube_);
-  cudaFree(d_post_); cudaFree(d_bloom_); cudaFree(d_tonemap_);
+  cudaFree(d_post_); cudaFree(d_bloom_); cudaFree(d_tonemap_); cudaFree(d_fxaa_);
   if (h_pinned_) cudaFreeHost(h_pinned_);
   if (copy_stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(copy_stream_));
   for (auto& sl : slots_) {
@@ -497,14 +497,14 @@ auto RendererInstance::apply_pbr(const OxcCullCamera& camera, const OxcPbrCamera
   }
   if (rc != OXC_OK) return fail(rc);
   if ((rc = copy_to_host({{rgba_host, d_pbr_, px * 16}})) != OXC_OK) return rc;
-  pbr_lit_ = true;
+  post_source_ = d_pbr_;
   return OXC_OK;
 }
 
 // eye adaptation on stream_, synchronous: the histogram and the record are allocated at the first call, the record filled with 1.0
 auto RendererInstance::eye_adaptation(const OxcEyeAdaptationSettings& settings, float delta_time, OxcExposure* exposure_host) -> int {
   if (!ctx_ || !error_.empty()) return OXC_E_STATE;
-  if (!pbr_lit_) return OXC_E_INVALID; // no lit plane yet
+  if (!post_source_) return OXC_E_INVALID; // no lit plane yet
   cudaStream_t s = static_cast<cudaStream_t>(stream_);
   const bool first = !d_post_;
   if (optional_plane(&d_post_, OXC_HISTOGRAM_BIN_COUNT * 4 + sizeof(OxcExposure)) != OXC_OK) return OXC_E_CAPACITY;
@@ -513,14 +513,14 @@ auto RendererInstance::eye_adaptation(const OxcEyeAdaptationSettings& settings, 
   if (first && (cudaMemcpyAsync(record, &one, sizeof one, cudaMemcpyHostToDevice, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess))
     return fail(OXC_E_CUDA);
   int rc;
-  if ((rc = oxc_eye_adaptation(ctx_, d_pbr_, width_, height_, &settings, delta_time, record, d_post_, stream_)) != OXC_OK) return fail(rc);
+  if ((rc = oxc_eye_adaptation(ctx_, post_source_, width_, height_, &settings, delta_time, record, d_post_, stream_)) != OXC_OK) return fail(rc);
   return copy_to_host({{exposure_host, record, sizeof(OxcExposure)}});
 }
 
 // bloom on stream_, synchronous: the two chains are allocated at the first call
 auto RendererInstance::bloom(const OxcBloomSettings& settings, float* bloom_host) -> int {
   if (!ctx_ || !error_.empty()) return OXC_E_STATE;
-  if (!pbr_lit_ || width_ < 2 || height_ < 2) return OXC_E_INVALID;
+  if (!post_source_ || width_ < 2 || height_ < 2) return OXC_E_INVALID;
   const bool adapt = (settings.scene_flags & OXC_SCENE_HAS_EYE_ADAPTATION) != 0;
   if (adapt && !d_post_) return OXC_E_STATE; // no exposure record before an eye_adaptation
   const uint64_t texels = oxc_bloom_chain_texels(width_, height_);
@@ -528,7 +528,7 @@ auto RendererInstance::bloom(const OxcBloomSettings& settings, float* bloom_host
   const OxcBloomTargets targets{d_bloom_, d_bloom_ + texels * 4};
   const OxcExposure* record = adapt ? reinterpret_cast<const OxcExposure*>(d_post_ + OXC_HISTOGRAM_BIN_COUNT) : nullptr;
   int rc;
-  if ((rc = oxc_bloom(ctx_, d_pbr_, width_, height_, &settings, record, &targets, stream_)) != OXC_OK) return fail(rc);
+  if ((rc = oxc_bloom(ctx_, post_source_, width_, height_, &settings, record, &targets, stream_)) != OXC_OK) return fail(rc);
   if ((rc = copy_to_host({{bloom_host, targets.upsampled, (size_t)(width_ / 2) * (height_ / 2) * 16}})) != OXC_OK) return rc;
   bloomed_ = true;
   return OXC_OK;
@@ -537,7 +537,7 @@ auto RendererInstance::bloom(const OxcBloomSettings& settings, float* bloom_host
 // tonemap on stream_, synchronous: the output plane is allocated at the first call
 auto RendererInstance::tonemap(const OxcTonemapSettings& settings, float* rgba_host) -> int {
   if (!ctx_ || !error_.empty()) return OXC_E_STATE;
-  if (!pbr_lit_ || settings.tonemap_type > OXC_TONEMAP_GT7) return OXC_E_INVALID; // no lit plane yet, or no such curve
+  if (!post_source_ || settings.tonemap_type > OXC_TONEMAP_GT7) return OXC_E_INVALID; // no lit plane yet, or no such curve
   const bool adapt = (settings.scene_flags & OXC_SCENE_HAS_EYE_ADAPTATION) != 0, bloom = (settings.scene_flags & OXC_SCENE_HAS_BLOOM) != 0;
   if ((adapt && !d_post_) || (bloom && !bloomed_)) return OXC_E_STATE; // no record before an eye_adaptation, no image before a bloom
   const size_t px = (size_t)width_ * height_;
@@ -545,8 +545,21 @@ auto RendererInstance::tonemap(const OxcTonemapSettings& settings, float* rgba_h
   const OxcExposure* record = adapt ? reinterpret_cast<const OxcExposure*>(d_post_ + OXC_HISTOGRAM_BIN_COUNT) : nullptr;
   const float* image = bloom ? d_bloom_ + oxc_bloom_chain_texels(width_, height_) * 4 : nullptr; // upsampled level 0
   int rc;
-  if ((rc = oxc_tonemap(ctx_, d_pbr_, width_, height_, &settings, record, image, d_tonemap_, stream_)) != OXC_OK) return fail(rc);
+  if ((rc = oxc_tonemap(ctx_, post_source_, width_, height_, &settings, record, image, d_tonemap_, stream_)) != OXC_OK) return fail(rc);
   return copy_to_host({{rgba_host, d_tonemap_, px * 16}});
+}
+
+// FXAA on stream_, synchronous: the output plane is allocated at the first call and becomes the post chain's source
+auto RendererInstance::fxaa(float* rgba_host) -> int {
+  if (!ctx_ || !error_.empty()) return OXC_E_STATE;
+  if (!post_source_) return OXC_E_INVALID; // no lit plane yet
+  const size_t px = (size_t)width_ * height_;
+  if (optional_plane(&d_fxaa_, px * 16) != OXC_OK) return OXC_E_CAPACITY;
+  int rc;
+  if ((rc = oxc_fxaa(ctx_, d_pbr_, width_, height_, d_fxaa_, stream_)) != OXC_OK) return fail(rc);
+  if ((rc = copy_to_host({{rgba_host, d_fxaa_, px * 16}})) != OXC_OK) return rc;
+  post_source_ = d_fxaa_;
+  return OXC_OK;
 }
 
 // the contact_shadows pass (RendererInstance.cpp:990-1020) on stream_, synchronous: the last frame's depth, the pass into the renderer's
@@ -1171,6 +1184,11 @@ int oxr_bloom(OxrRenderer* r, const OxcBloomSettings* settings, float* bloom_hos
 int oxr_tonemap(OxrRenderer* r, const OxcTonemapSettings* settings, float* rgba_host) {
   if (!r || !settings) return OXC_E_INVALID;
   return r->impl.tonemap(*settings, rgba_host);
+}
+
+int oxr_fxaa(OxrRenderer* r, float* rgba_host) {
+  if (!r) return OXC_E_INVALID;
+  return r->impl.fxaa(rgba_host);
 }
 
 int oxr_contact_shadows(OxrRenderer* r, const OxcContactShadowCamera* contact_camera, const OxcContactShadowSettings* settings,

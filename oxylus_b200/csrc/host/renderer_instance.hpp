@@ -105,15 +105,18 @@ public:
   // sun_ambient_strength 0.15 and frame_index = the number of earlier calls; the cube (binary16 RGBA, 48 KiB) to the host when non-null
   auto atmosphere_sky_ibl(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3], float sun_intensity,
                           uint16_t* cube_host) -> int;
-  // eye adaptation (PostProcess.cpp:7-77) on the lit plane of the last successful apply_pbr, into the renderer's persistent exposure
+  // eye adaptation (PostProcess.cpp:7-77) on the post chain's source (post_source_), into the renderer's persistent exposure
   // record ((1, 1) at allocation, as the reference's vuk::fill); the record to the host when non-null
   auto eye_adaptation(const OxcEyeAdaptationSettings& settings, float delta_time, OxcExposure* exposure_host) -> int;
-  // bloom (PostProcess.cpp:79-203) of the same plane into the renderer's two chains, reading the record under HasEyeAdaptation;
+  // bloom (PostProcess.cpp:79-203) of the post chain's source into the renderer's two chains, reading the record under HasEyeAdaptation;
   // upsampled level 0 ((width / 2) x (height / 2) float4) to the host when non-null
   auto bloom(const OxcBloomSettings& settings, float* bloom_host) -> int;
-  // the tonemap (PostProcess.cpp:205-247) of the same plane into the renderer's tonemap plane, reading the record under
+  // the tonemap (PostProcess.cpp:205-247) of the post chain's source into the renderer's tonemap plane, reading the record under
   // HasEyeAdaptation and upsampled level 0 of the bloom chain under HasBloom; width x height float4 to the host when non-null
   auto tonemap(const OxcTonemapSettings& settings, float* rgba_host) -> int;
+  // FXAA (RendererInstance.cpp:1225-1255) of the lit plane of the last successful apply_pbr into the renderer's FXAA plane, which
+  // becomes the post chain's source; width x height float4 to the host when non-null
+  auto fxaa(float* rgba_host) -> int;
 
   // RendererInstance::render geometry section: run_geometry_pass(false) -> generate_hiz -> run_geometry_pass(true)
   auto render(const OxcCullCamera& camera, const float* occluder_depth_host, uint32_t* vis32_host, float* depth_host,
@@ -209,11 +212,14 @@ private:
   int atmosphere_luts_device(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3], float sun_intensity);
   uint16_t* d_sky_ibl_cube_ = nullptr; // the sky IBL cube, allocated and zeroed by the first atmosphere_sky_ibl
   uint32_t sky_ibl_calls_ = 0;         // atmosphere_sky_ibl calls so far: the frame_index of the next one
-  bool pbr_lit_ = false;               // d_pbr_ holds the output of a successful apply_pbr
+  // the plane eye_adaptation, bloom and tonemap read: d_pbr_ after a successful apply_pbr, d_fxaa_ after a successful fxaa (the
+  // reference's final_attachment); null before the first successful apply_pbr
+  const float* post_source_ = nullptr;
   uint32_t* d_post_ = nullptr;         // the eye-adaptation histogram (256 u32), then the exposure record, from the first eye_adaptation
   float* d_bloom_ = nullptr;           // bloom's downsampled chain, then its upsampled chain, from the first bloom
   bool bloomed_ = false;               // d_bloom_ holds the chains of a successful bloom
   float* d_tonemap_ = nullptr;         // the tonemap's output plane (float4 per pixel), from the first tonemap
+  float* d_fxaa_ = nullptr;            // FXAA's output plane (float4 per pixel), from the first fxaa
   int sky_ibl_device(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3], float sun_intensity);
   OxcLight* d_lights_ = nullptr;    // apply_pbr's lights buffer (OXC_MAX_LIGHTS records), allocated with d_pbr_
   bool has_external_depth_ = false;

@@ -1,6 +1,6 @@
 // oxc_shader_math.cuh — the HLSL-semantics primitives the screen-space passes' per-pixel headers share: max / min / saturate / sign /
-// frac with the shaders' NaN rules, the saturating float -> integer conversions and the index clamp of the software taps, the binary16
-// conversions of the planes the passes store, pi, and one 3-vector with the canonical operation order.  Each states its NaN and
+// frac with the shaders' NaN rules, the saturating float -> integer conversions, the address modes and the four-channel bilinear tap of
+// the software taps, the binary16 conversions of the planes the passes store, pi, and one 3-vector with the canonical operation order.  Each states its NaN and
 // rounding rule once, so every pass that calls it gives the same bits.
 // No warp intrinsics, no shared memory: tests compile this source for the host.
 #pragma once
@@ -30,6 +30,41 @@ OXC_DI int wrap_index(long long i, int n) {
   if (i >= 0 && i < n) return (int)i;
   const long long r = i % n;
   return (int)(r < 0 ? r + n : r);
+}
+
+// the texel index rule of a sampler's address mode: ClampToEdge (clamp_index) or Repeat (wrap_index)
+enum AddressMode { CLAMP_TO_EDGE, REPEAT };
+template <AddressMode MODE>
+OXC_DI int address_index(long long i, int n) { return MODE == REPEAT ? wrap_index(i, n) : clamp_index(i, n); }
+
+// the four-channel bilinear tap of a W x H float4 plane at the unnormalised, half-texel-shifted coordinate (x, y): oxc_bloom item 1's
+// rule, x0 = floor(x), wx = x - x0, texels x0, x0 + 1 / y0, y0 + 1 through the address mode, top = a00 + wx * (a10 - a00), bottom
+// likewise, top + wy * (bottom - top).  NaN-safe: the floor goes through sat_i32 and a NaN coordinate gives NaN weights.
+template <AddressMode MODE>
+OXC_DI float4 bilinear_at(const float4* src, int W, int H, float x, float y) {
+  const float x0 = floorf(x), y0 = floorf(y);
+  const float wx = fs(x, x0), wy = fs(y, y0);
+  const long long ix = sat_i32(x0), iy = sat_i32(y0);
+  const int c0 = address_index<MODE>(ix, W), c1 = address_index<MODE>(ix + 1, W);
+  const size_t r0 = (size_t)address_index<MODE>(iy, H) * W, r1 = (size_t)address_index<MODE>(iy + 1, H) * W;
+  const float4 a00 = src[r0 + c0], a10 = src[r0 + c1], a01 = src[r1 + c0], a11 = src[r1 + c1];
+  const float4 top = make_float4(fa(a00.x, fm(wx, fs(a10.x, a00.x))), fa(a00.y, fm(wx, fs(a10.y, a00.y))), fa(a00.z, fm(wx, fs(a10.z, a00.z))),
+                                 fa(a00.w, fm(wx, fs(a10.w, a00.w))));
+  const float4 bot = make_float4(fa(a01.x, fm(wx, fs(a11.x, a01.x))), fa(a01.y, fm(wx, fs(a11.y, a01.y))), fa(a01.z, fm(wx, fs(a11.z, a01.z))),
+                                 fa(a01.w, fm(wx, fs(a11.w, a01.w))));
+  return make_float4(fa(top.x, fm(wy, fs(bot.x, top.x))), fa(top.y, fm(wy, fs(bot.y, top.y))), fa(top.z, fm(wy, fs(bot.z, top.z))),
+                     fa(top.w, fm(wy, fs(bot.w, top.w))));
+}
+// Sample / SampleLevel(uv) at level 0: x = u * W - 0.5 (y likewise)
+template <AddressMode MODE>
+OXC_DI float4 bilinear_tap(const float4* src, int W, int H, float u, float v) {
+  return bilinear_at<MODE>(src, W, H, fs(fm(u, (float)W), 0.5f), fs(fm(v, (float)H), 0.5f));
+}
+// Sample(uv, int2(dx, dy)): the constant texel offset joins the unnormalised coordinate before the half-texel shift (Vulkan's
+// order), x = (u * W + dx) - 0.5
+template <AddressMode MODE>
+OXC_DI float4 bilinear_tap(const float4* src, int W, int H, float u, float v, int dx, int dy) {
+  return bilinear_at<MODE>(src, W, H, fs(fa(fm(u, (float)W), (float)dx), 0.5f), fs(fa(fm(v, (float)H), (float)dy), 0.5f));
 }
 
 // the blend of two mip levels' values: (1 - f) * lo + f * hi

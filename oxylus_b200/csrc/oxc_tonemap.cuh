@@ -96,23 +96,6 @@ inline TonemapParams tonemap_make_params(const float* frame, uint32_t width, uin
   return p;
 }
 
-// item 1: SampleLevel of a W x H float4 plane with linear filtering and the Repeat address mode
-OXC_DI float4 tonemap_tap(const float4* src, int W, int H, float u, float v) {
-  const float x = fs(fm(u, (float)W), 0.5f), y = fs(fm(v, (float)H), 0.5f);
-  const float x0 = floorf(x), y0 = floorf(y);
-  const float wx = fs(x, x0), wy = fs(y, y0);
-  const long long ix = sat_i32(x0), iy = sat_i32(y0);
-  const int c0 = wrap_index(ix, W), c1 = wrap_index(ix + 1, W);
-  const size_t r0 = (size_t)wrap_index(iy, H) * W, r1 = (size_t)wrap_index(iy + 1, H) * W;
-  const float4 a00 = src[r0 + c0], a10 = src[r0 + c1], a01 = src[r1 + c0], a11 = src[r1 + c1];
-  const float4 top = make_float4(fa(a00.x, fm(wx, fs(a10.x, a00.x))), fa(a00.y, fm(wx, fs(a10.y, a00.y))), fa(a00.z, fm(wx, fs(a10.z, a00.z))),
-                                 fa(a00.w, fm(wx, fs(a10.w, a00.w))));
-  const float4 bot = make_float4(fa(a01.x, fm(wx, fs(a11.x, a01.x))), fa(a01.y, fm(wx, fs(a11.y, a01.y))), fa(a01.z, fm(wx, fs(a11.z, a01.z))),
-                                 fa(a01.w, fm(wx, fs(a11.w, a01.w))));
-  return make_float4(fa(top.x, fm(wy, fs(bot.x, top.x))), fa(top.y, fm(wy, fs(bot.y, top.y))), fa(top.z, fm(wy, fs(bot.z, top.z))),
-                     fa(top.w, fm(wy, fs(bot.w, top.w))));
-}
-
 // mul(M, v) of a row-major 3 x 3: row . v
 OXC_DI Vec3 mat_vec(const float* m, Vec3 c) { return vec3(vdot(vec3(m[0], m[1], m[2]), c), vdot(vec3(m[3], m[4], m[5]), c), vdot(vec3(m[6], m[7], m[8]), c)); }
 OXC_DI float clamp01(float x) { return vmin(vmax(x, 0.0f), 1.0f); }
@@ -258,18 +241,18 @@ OXC_DI void tonemap_film_grain(const TonemapParams& p, int x, int y, Vec3& c) {
 template <uint32_t TYPE>
 OXC_DI float4 tonemap_pixel(const TonemapParams& p, int x, int y) {
   const float u = fd(fa((float)x, 0.5f), (float)p.width), v = fd(fa((float)y, 0.5f), (float)p.height);
-  const float4 src = tonemap_tap(p.frame, p.width, p.height, u, v);
+  const float4 src = bilinear_tap<REPEAT>(p.frame, p.width, p.height, u, v);
   Vec3 c;
   if (p.flags & OXC_SCENE_HAS_CHROMATIC_ABERRATION) {
     // item 4: the colour is replaced, so exposure, bloom and curve are not computed
     const float dx = (float)(x - p.cx), dy = (float)(y - p.cy), cx = (float)p.cx, cy = (float)p.cy;
-    c.x = tonemap_tap(p.frame, p.width, p.height, fm(fa(fa(fm(dx, p.red_mag), cx), 0.5f), p.rcp_x), fm(fa(fa(fm(dy, p.red_mag), cy), 0.5f), p.rcp_y)).x;
-    c.y = tonemap_tap(p.frame, p.width, p.height, fm(fa(fa(fm(dx, p.green_mag), cx), 0.5f), p.rcp_x), fm(fa(fa(fm(dy, p.green_mag), cy), 0.5f), p.rcp_y)).y;
-    c.z = tonemap_tap(p.frame, p.width, p.height, fm((float)x, p.rcp_x), fm((float)y, p.rcp_y)).z;
+    c.x = bilinear_tap<REPEAT>(p.frame, p.width, p.height, fm(fa(fa(fm(dx, p.red_mag), cx), 0.5f), p.rcp_x), fm(fa(fa(fm(dy, p.red_mag), cy), 0.5f), p.rcp_y)).x;
+    c.y = bilinear_tap<REPEAT>(p.frame, p.width, p.height, fm(fa(fa(fm(dx, p.green_mag), cx), 0.5f), p.rcp_x), fm(fa(fa(fm(dy, p.green_mag), cy), 0.5f), p.rcp_y)).y;
+    c.z = bilinear_tap<REPEAT>(p.frame, p.width, p.height, fm((float)x, p.rcp_x), fm((float)y, p.rcp_y)).z;
   } else {
     c = vscale(vec3(src.x, src.y, src.z), p.record ? p.record->exposure : p.exposure);
     if (p.bloom) {
-      const float4 b = tonemap_tap(p.bloom, p.bloom_w, p.bloom_h, u, v);
+      const float4 b = bilinear_tap<REPEAT>(p.bloom, p.bloom_w, p.bloom_h, u, v);
       c = vadd(c, vscale(vec3(b.x, b.y, b.z), p.bloom_intensity));
     }
     c = tonemap_curve<TYPE>(p.k, c);

@@ -34,6 +34,7 @@
 #include "kernels_exposure.cuh"
 #include "kernels_bloom.cuh"
 #include "kernels_tonemap.cuh"
+#include "kernels_fxaa.cuh"
 
 using namespace oxc;
 
@@ -1757,6 +1758,20 @@ int oxc_tonemap(OxcContext* c, const float* frame_dev, uint32_t w, uint32_t h, c
   case OXC_TONEMAP_AGX: k_tonemap<OXC_TONEMAP_AGX><<<grid, TONEMAP_THREADS, 0, s>>>(p); break;
   default: k_tonemap<OXC_TONEMAP_GT7><<<grid, TONEMAP_THREADS, 0, s>>>(p); break;
   }
+  LAUNCHED();
+  return OXC_OK;
+}
+
+int oxc_fxaa(OxcContext* c, const float* frame_dev, uint32_t w, uint32_t h, float* out_dev, void* stream) {
+  if (!c || !frame_dev || !out_dev) return fail(OXC_E_INVALID, "null argument");
+  int rc;
+  if ((rc = check_extent(w, h)) != OXC_OK) return rc;
+  if (misaligned(16, frame_dev, out_dev)) return fail(OXC_E_INVALID, "frame_dev and out_dev must be 16-byte aligned");
+  const uint64_t bytes = (uint64_t)w * h * 16;
+  if (overlaps(out_dev, bytes, frame_dev, bytes)) return fail(OXC_E_INVALID, "out_dev overlaps frame_dev (the taps read other pixels)");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  k_fxaa<<<tiles(w, h, FXAA_TILE_X, FXAA_TILE_Y), FXAA_THREADS, 0, s>>>(fxaa_make_params(frame_dev, w, h, out_dev));
   LAUNCHED();
   return OXC_OK;
 }
