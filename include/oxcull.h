@@ -524,6 +524,73 @@ int oxc_cull_terrain(OxcContext* ctx, const OxcTerrainData* terrain, const float
                      const OxcCullCamera* camera, uint32_t cull_flags, uint32_t* visible_patches_dev,
                      uint32_t* patch_visibility_mask_dev, OxcDrawIndirectCommand* draw_cmd_dev, void* stream);
 
+/* Terrain draw into the vis buffer: passes/terrain_visbuffer.slang (vs_main, hs_constants, ds_main, fs_main) via
+ * RendererInstance::draw_terrain_for_visbuffer (Passes/Terrain.cpp:218-277), the consumer of oxc_cull_terrain's visible_patches and
+ * draw_cmd.  The hardware tessellator leaves points open; each item states what this library commits to.  Binary32, IEEE RN, no
+ * contraction, the canonical operation order (oracle/oxc_oracle_terrain_draw.c computes it; oxylus_b200/csrc/oxc_terrain.cuh is the
+ * device source).
+ *   1. Corners and factors.  Patch i of visible_patches is (i % patch_count.x, i / patch_count.x); corner (dx, dz) is patch_corner =
+ *      world_min + (f32(patch + corner) / f32(patch_count)) * world_size, as oxc_cull_terrain forms it; p0 = (0, 0), p1 = (1, 0),
+ *      p2 = (1, 1), p3 = (0, 1); its height is sampled like a domain point (item 4).  Edges as hs_constants writes them:
+ *      u0 = (p0, p3), v0 = (p0, p1), u1 = (p1, p2), v1 = (p3, p2); inner[0] = max(v0, v1) (along u), inner[1] = max(u0, u1) (along v).
+ *      edge_tessellation(a, b): centre = (a + b) * 0.5; radius = length(a - b) * 0.5; view_distance = max(length(centre - camera.
+ *      position) - radius, camera.near_clip); projected = ((2 * radius) * projection_scale) / view_distance; factor = clamp(projected /
+ *      target_edge_pixels, 1, max_tessellation), with HLSL max / min (a NaN quotient gives 1).  length(v) = sqrt((x*x + y*y) + z*z).
+ *      projection_scale = (camera.resolution.y * 0.5) / (s / c), (s, c) = the library's canonical sin and cos (oxc_exact.cuh
+ *      canonical_sincos) of (fov * 0x3C8EFA35) * 0.5 — fov in degrees (Camera::fov), 0x3C8EFA35 = pi / 180 in binary32 — formed
+ *      once per call.
+ *   2. Rounding (fractional_odd).  Each of the six factors is pinned to [1, 63] (Vulkan's maxTessellationGenerationLevel of 64, minus
+ *      one for odd spacing; NaN -> 1) and rounded up to the next odd integer n = 2 * ceil((f - 1) / 2) + 1.  When all six n are 1 the
+ *      patch is the two-triangle quad.  Otherwise an inner factor of 1 counts as 1 + 2^-23 and becomes 3 (Vulkan: an inner level of 1
+ *      with odd spacing is rounded as if it were slightly above 1).
+ *   3. Domain points and triangulation.  An edge of pinned factor f rounded to n has the points t_0 = 0 < t_1 < ... < t_n = 1: n - 2
+ *      equal segments L = 1 / f and two equal shorter ones s = (f - (n - 2)) / (2 f) at its two ends (symmetric, and 0 < s <= L since
+ *      n - 2 < f <= n: the fractional_odd rule of equal full segments and two symmetric fractional ones).  For 1 <= k < n / 2:
+ *      t_k = s + f32(k - 1) * L; past the middle t_k = 1 - t_{n - k}, so the points are mirror images bit for bit; n = 1 gives {0, 1}.
+ *      The domain (u, v) has u along p0 -> p1 and v along p0 -> p3.  The inner grid is (a_i, b_j), i = 1..N_u - 1, j = 1..N_v - 1,
+ *      with a, b the points of the inner factors; its (N_u - 2)(N_v - 2) cells are split along the (a_i, b_j) - (a_i+1, b_j+1)
+ *      diagonal.  Each outer edge is stitched to the inner row beside it by a merge walk over the two rows by coordinate along the edge,
+ *      ties going to the outer row: from (O_0, I_0) each step adds the triangle of the next outer point when the inner row is finished
+ *      or that point's coordinate is <= the next inner point's, else of the next inner point.  The four stitch strips meet on the
+ *      corner diagonals (corner, inner corner), so strips and cells tile the unit square exactly: no gap, no overlap, one winding.  A
+ *      patch has 2 triangles, or sum(n_edge) + 2 (N_u - 2 + N_v - 2) + 2 (N_u - 2)(N_v - 2) (7,938 at 63 everywhere).
+ *   4. Heights.  sample_height(x, z) = base_height + tap * height_scale, tap = the bilinear R16Unorm tap (texel / 65535 in binary32) of
+ *      the res_x x res_y heightmap at uv = ((x, z) - world_min) * inv_world_size: level 0, ClampToEdge, Vulkan's texel centres
+ *      (x = u * res_x - 0.5, x0 = floor(x), weights x - x0, a + w * (b - a) per axis).  ds_main's point: e0 = lerp(p0, p1, u),
+ *      e1 = lerp(p3, p2, u), (x, z) = lerp(e0, e1, v), with lerp(a, b, t) = a * (1 - t) + b * t.  That form gives b exactly at t = 1
+ *      (and a at t = 0), so two neighbouring patches place bit-identical vertices along their shared edge (same factor: the same two
+ *      corners in the same order; same points) and the terrain is watertight; a + (b - a) * t does not return b at t = 1.
+ *   5. Raster.  clip = projection_view x (x, h, z, 1) in the meshlet raster's order (((m0 x + m4 h) + m8 z) + m12 per row), then the
+ *      raster specification of oxc_raster_visbuffer (oracle/oxc_oracle.c raster_triangle): 24.8 snapping, set-up, top-left rule,
+ *      depth, and the clip path for triangles across the near or side planes.  Data word TERRAIN_INSTANCE_ID << prim_bits with the
+ *      id = the packing's all-ones id minus one (visbuffer.slang:16-20): 0xFFFFFE00, or 0xFFFFFF80 under OxcCreateInfo::wide_ids.
+ *      Packed 64-bit max into the caller's vis buffer.  At equal depth the terrain's word beats every meshlet word (ids below the
+ *      sentinel), as in the reference, where the terrain draws after the meshlets under GreaterOrEqual.
+ *   6. Winding.  triangle_ccw with cullMode Back keeps the face seen from +y.  The raster draws one winding: area2 < 0 in its
+ *      snapped screen coordinates (y down).  A camera above the terrain looking down with the reference's projection (P[1][1]
+ *      negated) maps world x to screen x and world z to screen y with positive scales, so (u, v) = (x, z) keeps its orientation on
+ *      screen and a triangle must be clockwise in (u, v) to be drawn.  Every triangle of item 3 is therefore handed to the raster
+ *      clockwise in (u, v): a flat terrain seen from above is fully drawn, seen from below nothing is.
+ *   7. Instances.  draw_cmd->instance_count and visible_patches are read on the device (no read-back: graph-capturable from the first
+ *      call); the count is clamped to patch_count.x * patch_count.y, and a slot holding a patch index past that total draws nothing.
+ * Triangles with large pixel boxes go through the context's chunk queue of oxc_raster_visbuffer (k_raster_big), so a terrain draw and
+ * a meshlet raster of one context must run in stream order, not concurrently on two streams.
+ * visible_patches_dev must hold patch_count.x * patch_count.y entries (oxc_cull_terrain's list).  OXC_E_INVALID before any launch
+ * for NULL arguments, a zero or > 32768 extent, a zero or > 65536 heightmap side, an empty or > 2^32 - 1 patch grid, misaligned
+ * pointers (heightmap 2, visible_patches and draw_cmd 4, vis 8 bytes), and a target_edge_pixels or max_tessellation that is not
+ * finite or below 1. */
+typedef struct OxcTerrainDrawSettings { /* TerrainData's fields the draw reads (scene.slang:634-647) and Camera::fov */
+  OxcTerrainData terrain;
+  float inv_world_size[2];   /* 1 / world_size (Passes/Terrain.cpp:20) */
+  float target_edge_pixels;  /* default 16 */
+  float max_tessellation;    /* default 64 */
+  float fov;                 /* vertical field of view, degrees */
+} OxcTerrainDrawSettings;
+OXC_STATIC_ASSERT(sizeof(OxcTerrainDrawSettings) == 52, "TerrainDrawSettings");
+int oxc_draw_terrain(OxcContext* ctx, const uint16_t* heightmap_dev, uint32_t res_x, uint32_t res_y, const OxcTerrainDrawSettings* settings,
+                     const uint32_t* visible_patches_dev, const OxcDrawIndirectCommand* draw_cmd_dev, const OxcCullCamera* camera,
+                     uint32_t width, uint32_t height, uint64_t* vis_dev, void* stream);
+
 /* Vis-buffer decode, geometry part (SURVEY §8f.1): passes/visbuffer_decode.slang:42-183 via RendererInstance's
  * "vis decode" pass.  Per pixel: texel -> (meshlet instance, triangle) (visbuffer.slang:31-36), triangle re-fetch
  * (scene.slang:363-399), world positions, compute_partial_derivatives (:42-92: analytic perspective-correct
@@ -1459,6 +1526,16 @@ int oxr_update_transforms(OxrRenderer* r, const OxcTransformWorld* transforms, u
 /* Depth laid down by passes outside this path (terrain, RendererInstance.cpp:862-873): a width x height D32F HOST
  * image copied to the device once and merged into every following frame; NULL removes it. */
 int oxr_set_external_depth(OxrRenderer* r, const float* depth_host);
+/* The terrain of RendererInstance::render (Passes/Terrain.cpp:159-277, RendererInstance.cpp:864-880): copies the res_x x res_y R16
+ * heightmap and the patch min / max (float2 per patch, row-major) from HOST memory with the settings of oxc_draw_terrain, and allocates
+ * the visible-patch list, the draw command and the persistent patch visibility mask (zeroed).  With a terrain set, each geometry pass
+ * of oxr_render / oxr_submit runs oxc_cull_terrain (TestFrustum | TestOcclusion, | LatePass in the late pass) and oxc_draw_terrain
+ * right after its meshlet raster, before generate_hiz in the early pass.  Those two take the camera by value, so oxr_submit enqueues a
+ * frame with a terrain without its CUDA graphs.  heightmap_host == NULL removes the terrain (the frame is the terrain-less one again).
+ * Either call drops the captured frame graphs.  OXC_E_INVALID for a missing min / max or settings, a zero or > 65536 side, an empty or
+ * > 2^32 - 1 patch grid, or a target_edge_pixels / max_tessellation that is not finite or below 1; the terrain is removed then. */
+int oxr_set_terrain(OxrRenderer* r, const uint16_t* heightmap_host, uint32_t res_x, uint32_t res_y, const float* patch_minmax_host,
+                    const OxcTerrainDrawSettings* settings);
 /* MainGeometryContext::draw_overdraw (RendererInstance.cpp:771-776): the encode pass's fragment counter (oxc_raster_overdraw, both
  * passes) of the frame that oxr_render / oxr_wait completed last, for the camera it was rendered with; width x height u32 to the
  * host.  Synchronous; the frame's own outputs are not touched. */

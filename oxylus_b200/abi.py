@@ -91,6 +91,22 @@ DRAW_INDIRECT_DT = np.dtype([("vertex_count", "<u4"), ("instance_count", "<u4"),
 CLIPMAP_DT = np.dtype([("projection_view_mat", "<f4", (16,)), ("page_offset", "<i4", (2,)), ("z_near", "<f4")])
 assert CLIPMAP_DT.itemsize == 76
 assert TERRAIN_DT.itemsize == 32 and DRAW_INDIRECT_DT.itemsize == 16
+# OxcTerrainDrawSettings: TerrainData's fields the terrain draw reads and Camera::fov (degrees)
+TERRAIN_DRAW_SETTINGS_DT = np.dtype([("terrain", TERRAIN_DT), ("inv_world_size", "<f4", (2,)), ("target_edge_pixels", "<f4"),
+                                     ("max_tessellation", "<f4"), ("fov", "<f4")])
+assert TERRAIN_DRAW_SETTINGS_DT.itemsize == 52
+
+
+def terrain_draw_settings(terrain, target_edge_pixels=16.0, max_tessellation=64.0, fov=60.0):
+    """OxcTerrainDrawSettings of a TERRAIN_DT record with the reference's defaults (Terrain.hpp: 16 px, 64; Camera fov 60 degrees);
+    inv_world_size = 1 / world_size in binary32, as Passes/Terrain.cpp:20 forms it"""
+    s = np.zeros(1, dtype=TERRAIN_DRAW_SETTINGS_DT)
+    s["terrain"] = np.asarray(terrain, dtype=TERRAIN_DT).reshape(1)
+    size = s["terrain"]["world_size"][0].astype(np.float32)
+    with np.errstate(divide="ignore"):
+        s["inv_world_size"][0] = np.float32(1.0) / size
+    s["target_edge_pixels"], s["max_tessellation"], s["fov"] = target_edge_pixels, max_tessellation, fov
+    return s
 assert TRANSFORM_DT.itemsize == 64
 assert MESHLET_BOUNDS_DT.itemsize == 16
 assert VISIBILITY_DT.itemsize == 12

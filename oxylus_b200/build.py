@@ -16,7 +16,7 @@ SOURCES = [os.path.join(CSRC, "oxcull.cu"), os.path.join(CSRC, "host", "renderer
            os.path.join(CSRC, "host", "mesh_builder.cpp"), os.path.join(CSRC, "host", "mesh_simplifier.cpp")]
 DEPS = SOURCES + [
     os.path.join(CSRC, f)
-    for f in ("oxc_types.cuh", "oxc_exact.cuh", "oxc_shader_math.cuh", "oxc_filtered.cuh", "oxc_raster_core.cuh", "kernels_cull.cuh", "kernels_decode.cuh", "kernels_hiz.cuh", "kernels_mgpu.cuh", "kernels_tri.cuh", "kernels_alpha.cuh", "kernels_vsm.cuh", "kernels_vsm_draw.cuh", "kernels_vsm_resolve.cuh", "kernels_gtao.cuh", "kernels_pbr.cuh", "kernels_contact_shadows.cuh", "kernels_atmosphere.cuh", "kernels_sky_ibl.cuh", "kernels_pbr_atmosphere.cuh", "kernels_exposure.cuh", "kernels_bloom.cuh", "kernels_tonemap.cuh", "kernels_fxaa.cuh", "oxc_alpha.cuh", "oxc_gbuffer.cuh", "oxc_vsm_resolve.cuh", "oxc_gtao.cuh", "oxc_pbr.cuh", "oxc_contact_shadows.cuh", "oxc_atmosphere.cuh", "oxc_sky_ibl.cuh", "oxc_pbr_atmosphere.cuh", "oxc_exposure.cuh", "oxc_bloom.cuh", "oxc_tonemap.cuh", "oxc_fxaa.cuh")
+    for f in ("oxc_types.cuh", "oxc_exact.cuh", "oxc_shader_math.cuh", "oxc_filtered.cuh", "oxc_raster_core.cuh", "kernels_cull.cuh", "kernels_decode.cuh", "kernels_hiz.cuh", "kernels_mgpu.cuh", "kernels_tri.cuh", "kernels_alpha.cuh", "kernels_vsm.cuh", "kernels_vsm_draw.cuh", "kernels_vsm_resolve.cuh", "kernels_gtao.cuh", "kernels_pbr.cuh", "kernels_contact_shadows.cuh", "kernels_atmosphere.cuh", "kernels_sky_ibl.cuh", "kernels_pbr_atmosphere.cuh", "kernels_exposure.cuh", "kernels_bloom.cuh", "kernels_tonemap.cuh", "kernels_fxaa.cuh", "kernels_terrain.cuh", "oxc_alpha.cuh", "oxc_gbuffer.cuh", "oxc_vsm_resolve.cuh", "oxc_gtao.cuh", "oxc_pbr.cuh", "oxc_contact_shadows.cuh", "oxc_atmosphere.cuh", "oxc_sky_ibl.cuh", "oxc_pbr_atmosphere.cuh", "oxc_exposure.cuh", "oxc_bloom.cuh", "oxc_tonemap.cuh", "oxc_fxaa.cuh", "oxc_terrain.cuh")
 ] + [os.path.join(CSRC, "host", "renderer_instance.hpp"), os.path.join(CSRC, "host", "mesh_simplifier.hpp"), os.path.join(os.path.dirname(HERE), "include", "oxcull.h")]
 
 NVCC_FLAGS = [

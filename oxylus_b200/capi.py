@@ -18,7 +18,7 @@ SYMBOLS = [
     "oxc_last_error", "oxc_kernel_launch_count", "oxc_version", "oxc_create", "oxc_destroy", "oxc_set_scene",
     "oxc_update_transforms", "oxc_reset_visibility_mask", "oxc_clear_hiz", "oxc_set_shard", "oxc_set_shard_auto", "oxc_cull_meshes",
     "oxc_cull_meshlets", "oxc_build_hiz", "oxc_build_hiz_packed", "oxc_build_hiz_mip0_packed", "oxc_build_hiz_from_mip0", "oxc_cull_triangles", "oxc_cull_triangles_small_primitive", "oxc_clear_visbuffer",
-    "oxc_raster_visbuffer", "oxc_raster_visbuffer_clip_pass", "oxc_set_materials", "oxc_raster_overdraw", "oxc_clear_overdraw", "oxc_resolve_visbuffer", "oxc_merge_depth", "oxc_clear_visbuffer_with_depth", "oxc_cull_meshlets_multiview", "oxc_cull_meshlets_hpb", "oxc_cull_terrain",
+    "oxc_raster_visbuffer", "oxc_raster_visbuffer_clip_pass", "oxc_set_materials", "oxc_raster_overdraw", "oxc_clear_overdraw", "oxc_resolve_visbuffer", "oxc_merge_depth", "oxc_clear_visbuffer_with_depth", "oxc_cull_meshlets_multiview", "oxc_cull_meshlets_hpb", "oxc_cull_terrain", "oxc_draw_terrain",
     "oxc_decode_visbuffer", "oxc_decode_gbuffer", "oxc_build_hpb", "oxc_mark_visible_pages",
     "oxc_vsm_begin_frame", "oxc_vsm_invalidate_pages", "oxc_vsm_allocate_pages", "oxc_vsm_clear_dirty_pages", "oxc_cull_meshlets_hpb_dirty_dev",
     "oxc_vsm_draw_pages", "oxc_vsm_draw_stats", "oxc_vsm_resolve_shadows", "oxc_generate_ambient_occlusion", "oxc_apply_pbr",
@@ -29,7 +29,7 @@ SYMBOLS = [
     "oxc_mgpu_get_unique_id", "oxc_mgpu_init", "oxc_mgpu_init_with_comm", "oxc_mgpu_shutdown", "oxc_mgpu_info", "oxc_mgpu_exchange_hiz",
     "oxc_mgpu_exchange_frame", "oxc_mgpu_stage_survivors", "oxc_mgpu_set_survivor_capacity", "oxc_copy", "oxc_sync", "oxc_device_alloc", "oxc_device_free", "oxc_debug_dequantize_half",
     "oxb_last_error", "oxb_build_mesh", "oxb_mesh_blob_size", "oxb_mesh_lod0_meshlet_count", "oxb_mesh_emit", "oxb_mesh_free", "oxb_simplify",
-    "oxr_create", "oxr_destroy", "oxr_context", "oxr_update", "oxr_update_transforms", "oxr_set_external_depth", "oxr_set_materials", "oxr_overdraw", "oxr_render", "oxr_submit", "oxr_wait",
+    "oxr_create", "oxr_destroy", "oxr_context", "oxr_update", "oxr_update_transforms", "oxr_set_external_depth", "oxr_set_terrain", "oxr_set_materials", "oxr_overdraw", "oxr_render", "oxr_submit", "oxr_wait",
     "oxr_vsm_update_pages", "oxr_vsm_pages", "oxr_vsm_draw_shadows", "oxr_vsm_resolve_shadows", "oxr_decode_gbuffer",
     "oxr_generate_ambient_occlusion", "oxr_apply_pbr", "oxr_contact_shadows", "oxr_apply_pbr_with_contact_shadows",
     "oxr_atmosphere_luts", "oxr_atmosphere_sky_ibl",
@@ -88,6 +88,7 @@ def load(build_if_missing=True):
     lib.oxc_cull_meshlets_multiview.argtypes = [vp, vp, u32, i32, vp]
     lib.oxc_cull_meshlets_hpb.argtypes = [vp, vp, vp, vp, u32, vp, u32, u32, vp]
     lib.oxc_cull_terrain.argtypes = [vp, vp, vp, vp, u32, vp, vp, vp, vp]
+    lib.oxc_draw_terrain.argtypes = [vp, vp, u32, u32, vp, vp, vp, vp, u32, u32, vp, vp]
     lib.oxc_decode_visbuffer.argtypes = [vp, vp, vp, vp, u32, u32, C.POINTER(abi.DecodeTargets), vp]
     lib.oxc_decode_gbuffer.argtypes = [vp, vp, vp, vp, u32, u32, C.POINTER(abi.GBufferTargets), vp]
     lib.oxc_build_hpb.argtypes = [vp, vp, u32, u32, vp, u32, vp]
@@ -142,6 +143,7 @@ def load(build_if_missing=True):
     lib.oxr_update_transforms.argtypes = [vp, vp, u32, u32]
     lib.oxr_set_external_depth.argtypes = [vp, vp]
     lib.oxr_set_materials.argtypes = [vp, C.POINTER(abi.MaterialTable)]
+    lib.oxr_set_terrain.argtypes = [vp, vp, u32, u32, vp, vp]
     lib.oxr_overdraw.argtypes = [vp, vp, vp]
     lib.oxr_submit.argtypes = [vp, vp, vp, vp, vp, u32, C.POINTER(C.c_int)]
     lib.oxr_wait.argtypes = [vp, i32, C.POINTER(abi.FrameResult)]
@@ -444,6 +446,13 @@ class Context:
         t = np.ascontiguousarray(terrain)
         _check(self.lib.oxc_cull_terrain(self.h, _ptr(t), _ptr(patch_minmax_dev), _ptr(cam), flags, _ptr(visible_patches_dev),
                                          _ptr(mask_dev), _ptr(draw_cmd_dev), self.stream), "oxc_cull_terrain")
+
+    def draw_terrain(self, heightmap_dev, res_x, res_y, settings, visible_patches_dev, draw_cmd_dev, cam, w, h, vis_dev):
+        """oxc_draw_terrain: tessellates the visible patches of oxc_cull_terrain over the R16 heightmap (res_x x res_y uint16 on the
+        device) and rasterises them into the packed vis buffer; settings is an abi.TERRAIN_DRAW_SETTINGS_DT record"""
+        st = np.ascontiguousarray(settings)
+        _check(self.lib.oxc_draw_terrain(self.h, _ptr(heightmap_dev), res_x, res_y, _ptr(st), _ptr(visible_patches_dev), _ptr(draw_cmd_dev),
+                                         _ptr(cam), w, h, _ptr(vis_dev), self.stream), "oxc_draw_terrain")
 
     def decode_visbuffer(self, cam, w, h, targets, vis64_dev=None, vis32_dev=None):
         """targets: dict with any of lambda_, ddx, ddy, uv_normal, uv_grad -> device pointers (float4 planes)."""
@@ -768,6 +777,17 @@ class Renderer:
         out = np.zeros((self.scene.height, self.scene.width), dtype=np.uint32)
         _check(self.lib.oxr_overdraw(self.h, _ptr(cam), _ptr(out)), "oxr_overdraw")
         return out
+
+    def set_terrain(self, heightmap, patch_minmax=None, settings=None):
+        """oxr_set_terrain: heightmap uint16 [res_y, res_x], patch_minmax float32 [patches, 2], settings an abi.TERRAIN_DRAW_SETTINGS_DT
+        record; heightmap None removes the terrain"""
+        if heightmap is None:
+            _check(self.lib.oxr_set_terrain(self.h, None, 0, 0, None, None), "oxr_set_terrain")
+            return
+        hm = np.ascontiguousarray(heightmap, dtype=np.uint16)
+        mm = np.ascontiguousarray(patch_minmax, dtype=np.float32)
+        st = np.ascontiguousarray(settings)
+        _check(self.lib.oxr_set_terrain(self.h, _ptr(hm), hm.shape[1], hm.shape[0], _ptr(mm), _ptr(st)), "oxr_set_terrain")
 
     def set_external_depth(self, depth):
         d = None if depth is None else np.ascontiguousarray(depth, dtype=np.float32)

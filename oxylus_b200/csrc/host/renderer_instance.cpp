@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -146,6 +147,7 @@ RendererInstance::~RendererInstance() {
   cudaFree(d_vis64_); cudaFree(d_vis32_); cudaFree(d_depth_); cudaFree(d_occluder_); cudaFree(d_overdraw_); cudaFree(d_gbuffer_);
   cudaFree(d_uv_normal_); cudaFree(d_gtao_); cudaFree(d_pbr_); cudaFree(d_lights_); cudaFree(d_contact_); cudaFree(d_atmosphere_); cudaFree(d_sky_ibl_cube_);
   cudaFree(d_post_); cudaFree(d_bloom_); cudaFree(d_tonemap_); cudaFree(d_fxaa_);
+  terrain_release();
   if (h_pinned_) cudaFreeHost(h_pinned_);
   if (copy_stream_) cudaStreamSynchronize(static_cast<cudaStream_t>(copy_stream_));
   for (auto& sl : slots_) {
@@ -699,6 +701,54 @@ auto RendererInstance::set_external_depth(const float* depth_host) -> int {
   return OXC_OK;
 }
 
+void RendererInstance::terrain_release() {
+  cudaFree(terrain_.d_heightmap); cudaFree(terrain_.d_minmax); cudaFree(terrain_.d_visible); cudaFree(terrain_.d_mask); cudaFree(terrain_.d_cmd);
+  terrain_ = Terrain();
+}
+
+auto RendererInstance::set_terrain(const uint16_t* heightmap_host, uint32_t res_x, uint32_t res_y, const float* patch_minmax_host,
+                                   const OxcTerrainDrawSettings* settings) -> int {
+  if (!ctx_) return OXC_E_STATE;
+  cudaStream_t s = static_cast<cudaStream_t>(stream_);
+  if (cudaStreamSynchronize(s) != cudaSuccess) return fail(OXC_E_CUDA); // no frame in flight reads the buffers released below
+  drop_graphs(); // a captured frame holds the old terrain's launches (or none)
+  terrain_release();
+  if (!heightmap_host) return OXC_OK;
+  if (!patch_minmax_host || !settings || res_x == 0 || res_y == 0 || res_x > 65536 || res_y > 65536) return OXC_E_INVALID;
+  const uint64_t total = (uint64_t)settings->terrain.patch_count[0] * settings->terrain.patch_count[1];
+  if (total == 0 || total > 0xFFFFFFFFull) return OXC_E_INVALID;
+  if (!std::isfinite(settings->target_edge_pixels) || !(settings->target_edge_pixels >= 1.0f) || !std::isfinite(settings->max_tessellation) ||
+      !(settings->max_tessellation >= 1.0f))
+    return OXC_E_INVALID;
+  const size_t texels = (size_t)res_x * res_y, words = (size_t)((total + 31) / 32);
+  Terrain t;
+  t.res_x = res_x; t.res_y = res_y; t.settings = *settings;
+  if (cudaMalloc(&t.d_heightmap, texels * 2) != cudaSuccess || cudaMalloc(&t.d_minmax, (size_t)total * 8) != cudaSuccess ||
+      cudaMalloc(&t.d_visible, (size_t)total * 4) != cudaSuccess || cudaMalloc(&t.d_mask, words * 4) != cudaSuccess ||
+      cudaMalloc(&t.d_cmd, sizeof(OxcDrawIndirectCommand)) != cudaSuccess) {
+    cudaGetLastError();
+    terrain_ = t;
+    terrain_release();
+    return OXC_E_CAPACITY;
+  }
+  t.set = true;
+  terrain_ = t;
+  if (cudaMemcpyAsync(t.d_heightmap, heightmap_host, texels * 2, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+      cudaMemcpyAsync(t.d_minmax, patch_minmax_host, (size_t)total * 8, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+      cudaMemsetAsync(t.d_mask, 0, words * 4, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
+    return fail(OXC_E_CUDA);
+  return OXC_OK;
+}
+
+int RendererInstance::terrain_pass(const OxcCullCamera& camera, bool late) {
+  const uint32_t flags = OXC_CULL_TEST_FRUSTUM | OXC_CULL_TEST_OCCLUSION | (late ? OXC_CULL_LATE_PASS : 0u);
+  int rc = oxc_cull_terrain(ctx_, &terrain_.settings.terrain, terrain_.d_minmax, &camera, flags, terrain_.d_visible, terrain_.d_mask,
+                            terrain_.d_cmd, stream_);
+  if (rc != OXC_OK) return rc;
+  return oxc_draw_terrain(ctx_, terrain_.d_heightmap, terrain_.res_x, terrain_.res_y, &terrain_.settings, terrain_.d_visible, terrain_.d_cmd,
+                          &camera, width_, height_, d_vis64_, stream_);
+}
+
 // CullGeometry.cpp:61-404
 auto RendererInstance::cull_geometry(CullGeometryContext& context) -> int {
   int rc;
@@ -781,6 +831,7 @@ int RendererInstance::frame_tail(const OxcCullCamera& camera, void* readback) {
   if (materialize && cudaMemcpyAsync(&rb->draw_index_count[0], &out.draw_cmd->index_count, 4, cudaMemcpyDefault, s) != cudaSuccess) return OXC_E_CUDA;
   main_geometry_context.cull_flags = OXC_CULL_TEST_ALL;
   if ((rc = draw_for_visbuffer(main_geometry_context)) != OXC_OK) return rc;
+  if (terrain_.set && (rc = terrain_pass(camera, false)) != OXC_OK) return rc; // :864-880, after the meshlets
   g_trace.mark(s);
   if ((rc = generate_hiz(main_geometry_context)) != OXC_OK) return rc; // :883
   g_trace.mark(s);
@@ -796,6 +847,7 @@ int RendererInstance::frame_tail(const OxcCullCamera& camera, void* readback) {
   if (materialize && cudaMemcpyAsync(&rb->draw_index_count[1], &out.draw_cmd->index_count, 4, cudaMemcpyDefault, s) != cudaSuccess) return OXC_E_CUDA;
   main_geometry_context.cull_flags = cull_geometry_context.cull_flags;
   if ((rc = draw_for_visbuffer(main_geometry_context)) != OXC_OK) return rc;
+  if (terrain_.set && (rc = terrain_pass(camera, true)) != OXC_OK) return rc;
   g_trace.mark(s);
   return OXC_OK;
 }
@@ -927,7 +979,9 @@ auto RendererInstance::submit(const OxcCullCamera& camera, uint32_t* vis32_host,
   // a device buffer (oxc_bind_camera_buffer) that the head graph fills from this slot's pinned copy, so a replay only needs the
   // new camera written there.  Everything else a graph bakes in is part of its key; a mismatch re-captures.
   bool done = false;
-  if (use_graphs_ && !g_trace.on && out.reordered_indices == nullptr && d_cam_[slot] && h_cam_[slot]) {
+  // The terrain cull and draw take the camera by value (they never read the bound device camera), so a frame with a terrain is
+  // enqueued eagerly: a replayed graph would draw the terrain from the camera it was captured with.
+  if (use_graphs_ && !g_trace.on && !terrain_.set && out.reordered_indices == nullptr && d_cam_[slot] && h_cam_[slot]) {
     FrameGraph& g = graphs_[slot];
     const uint32_t key = (has_external_depth_ ? 1u : 0u) | (want_vis32 ? 2u : 0u) | (want_depth ? 4u : 0u);
     *static_cast<OxcCullCamera*>(h_cam_[slot]) = camera;
@@ -1090,6 +1144,12 @@ int oxr_overdraw(OxrRenderer* r, const OxcCullCamera* camera, uint32_t* overdraw
 int oxr_set_materials(OxrRenderer* r, const OxcMaterialTable* table) {
   if (!r) return OXC_E_INVALID;
   return r->impl.set_materials(table);
+}
+
+int oxr_set_terrain(OxrRenderer* r, const uint16_t* heightmap_host, uint32_t res_x, uint32_t res_y, const float* patch_minmax_host,
+                    const OxcTerrainDrawSettings* settings) {
+  if (!r) return OXC_E_INVALID;
+  return r->impl.set_terrain(heightmap_host, res_x, res_y, patch_minmax_host, settings);
 }
 
 int oxr_set_external_depth(OxrRenderer* r, const float* depth_host) {

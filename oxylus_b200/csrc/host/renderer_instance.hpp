@@ -66,6 +66,11 @@ public:
   auto set_materials(const OxcMaterialTable* table) -> int; // nullptr: plain encode
   auto overdraw(const OxcCullCamera& camera, uint32_t* overdraw_host) -> int; // fragment counter of the last rendered frame
   auto set_external_depth(const float* depth_host) -> int;
+  // the terrain of RendererInstance::render (Passes/Terrain.cpp:159-277): uploads the R16 heightmap (res_x x res_y), the patch min / max
+  // (float2 per patch) and the settings, and owns the visible-patch list, the draw command and the persistent patch mask; with a
+  // terrain set, both geometry passes run the terrain cull and draw after the meshlet raster.  heightmap_host == nullptr removes it.
+  auto set_terrain(const uint16_t* heightmap_host, uint32_t res_x, uint32_t res_y, const float* patch_minmax_host,
+                   const OxcTerrainDrawSettings* settings) -> int;
   auto cull_geometry(CullGeometryContext& context) -> int;
   auto generate_hiz(MainGeometryContext& context) -> int;
   auto draw_for_visbuffer(MainGeometryContext& context) -> int;
@@ -223,6 +228,20 @@ private:
   int sky_ibl_device(const OxcAtmosphere& atmosphere, const OxcPbrCamera& camera, const float sun_direction[3], float sun_intensity);
   OxcLight* d_lights_ = nullptr;    // apply_pbr's lights buffer (OXC_MAX_LIGHTS records), allocated with d_pbr_
   bool has_external_depth_ = false;
+  // the terrain of set_terrain (device copies and the cull's buffers); the frame runs terrain_pass when `set`
+  struct Terrain {
+    bool set = false;
+    uint16_t* d_heightmap = nullptr;
+    uint32_t res_x = 0, res_y = 0;
+    float* d_minmax = nullptr;
+    uint32_t* d_visible = nullptr;
+    uint32_t* d_mask = nullptr;
+    OxcDrawIndirectCommand* d_cmd = nullptr;
+    OxcTerrainDrawSettings settings{};
+  } terrain_;
+  void terrain_release();
+  // run_geometry_pass's terrain half (RendererInstance.cpp:864-880): cull with TestFrustum | TestOcclusion (| LatePass), then draw
+  int terrain_pass(const OxcCullCamera& camera, bool late);
   // transforms as the host last uploaded them, and on the device the values before the upload that last changed each of them
   // (TransformPrevious::previous_world, RendererInstance.cpp:1600-1609)
   std::vector<OxcTransformWorld> transforms_;

@@ -56,7 +56,7 @@ OXC_DI uint32_t decode_geometry(const DecodeParams& p, uint32_t x, uint32_t y, f
   const uint32_t tri = texel & ((1u << p.prim_bits) - 1u);
   const uint32_t id_base = p.id_base ? __ldg(p.id_base) : 0u;
   const uint32_t mii = gid - id_base;
-  const bool discard = texel == 0xFFFFFFFFu || gid == (0xFFFFFFFEu >> p.prim_bits) /* terrain sentinel, visbuffer.slang:16-20 */ || gid < id_base ||
+  const bool discard = texel == 0xFFFFFFFFu || gid == (0xFFFFFFFFu >> p.prim_bits) - 1u /* terrain sentinel TERRAIN_INSTANCE_ID in either packing, visbuffer.slang:16-20 */ || gid < id_base ||
                        mii >= __ldg(&p.vis->total_visible_meshlet_instances); // :97-99 (+ range guard)
   if (discard) return 0u;
   const uint2 mi = __ldg(reinterpret_cast<const uint2*>(p.meshlet_instances) + mii); // :103
@@ -176,7 +176,7 @@ __global__ void __launch_bounds__(DECODE_TX* DECODE_TY) k_decode_visbuffer(const
   const uint32_t tri = texel & ((1u << p.prim_bits) - 1u);
   const uint32_t id_base = p.id_base ? __ldg(p.id_base) : 0u;
   const uint32_t mii = gid - id_base;
-  const bool discard = texel == 0xFFFFFFFFu || gid == (0xFFFFFFFEu >> p.prim_bits) /* terrain sentinel, visbuffer.slang:16-20 */ || gid < id_base ||
+  const bool discard = texel == 0xFFFFFFFFu || gid == (0xFFFFFFFFu >> p.prim_bits) - 1u /* terrain sentinel TERRAIN_INSTANCE_ID in either packing, visbuffer.slang:16-20 */ || gid < id_base ||
                        mii >= __ldg(&p.vis->total_visible_meshlet_instances); // :97-99 (+ range guard)
   if (!discard) {
     const uint2 mi = __ldg(reinterpret_cast<const uint2*>(p.meshlet_instances) + mii); // :103

@@ -1,5 +1,5 @@
 // oxc_shader_math.cuh — the HLSL-semantics primitives the screen-space passes' per-pixel headers share: max / min / saturate / sign /
-// frac with the shaders' NaN rules, the saturating float -> integer conversions, the address modes and the four-channel bilinear tap of
+// frac with the shaders' NaN rules, the saturating float -> integer conversions, the address modes and the bilinear taps (float4 and R16) of
 // the software taps, the binary16 conversions of the planes the passes store, pi, and one 3-vector with the canonical operation order.  Each states its NaN and
 // rounding rule once, so every pass that calls it gives the same bits.
 // No warp intrinsics, no shared memory: tests compile this source for the host.
@@ -37,23 +37,30 @@ enum AddressMode { CLAMP_TO_EDGE, REPEAT };
 template <AddressMode MODE>
 OXC_DI int address_index(long long i, int n) { return MODE == REPEAT ? wrap_index(i, n) : clamp_index(i, n); }
 
-// the four-channel bilinear tap of a W x H float4 plane at the unnormalised, half-texel-shifted coordinate (x, y): oxc_bloom item 1's
-// rule, x0 = floor(x), wx = x - x0, texels x0, x0 + 1 / y0, y0 + 1 through the address mode, top = a00 + wx * (a10 - a00), bottom
-// likewise, top + wy * (bottom - top).  NaN-safe: the floor goes through sat_i32 and a NaN coordinate gives NaN weights.
-template <AddressMode MODE>
-OXC_DI float4 bilinear_at(const float4* src, int W, int H, float x, float y) {
+// the bilinear blend a + w * (b - a) of one channel, and of four
+OXC_DI float tap_lerp(float a, float b, float w) { return fa(a, fm(w, fs(b, a))); }
+OXC_DI float4 tap_lerp(float4 a, float4 b, float w) {
+  return make_float4(tap_lerp(a.x, b.x, w), tap_lerp(a.y, b.y, w), tap_lerp(a.z, b.z, w), tap_lerp(a.w, b.w, w));
+}
+
+// the bilinear tap of a W x H plane at the unnormalised, half-texel-shifted coordinate (x, y): oxc_bloom item 1's rule, x0 = floor(x),
+// wx = x - x0, texels x0, x0 + 1 / y0, y0 + 1 through the address mode, top = a00 + wx * (a10 - a00), bottom likewise,
+// top + wy * (bottom - top).  NaN-safe: the floor goes through sat_i32 and a NaN coordinate gives NaN weights.  fetch(i) returns
+// texel i (row-major) as a float or a float4.
+template <AddressMode MODE, class Fetch>
+OXC_DI auto bilinear_fetch(Fetch fetch, int W, int H, float x, float y) -> decltype(fetch(size_t(0))) {
   const float x0 = floorf(x), y0 = floorf(y);
   const float wx = fs(x, x0), wy = fs(y, y0);
   const long long ix = sat_i32(x0), iy = sat_i32(y0);
   const int c0 = address_index<MODE>(ix, W), c1 = address_index<MODE>(ix + 1, W);
   const size_t r0 = (size_t)address_index<MODE>(iy, H) * W, r1 = (size_t)address_index<MODE>(iy + 1, H) * W;
-  const float4 a00 = src[r0 + c0], a10 = src[r0 + c1], a01 = src[r1 + c0], a11 = src[r1 + c1];
-  const float4 top = make_float4(fa(a00.x, fm(wx, fs(a10.x, a00.x))), fa(a00.y, fm(wx, fs(a10.y, a00.y))), fa(a00.z, fm(wx, fs(a10.z, a00.z))),
-                                 fa(a00.w, fm(wx, fs(a10.w, a00.w))));
-  const float4 bot = make_float4(fa(a01.x, fm(wx, fs(a11.x, a01.x))), fa(a01.y, fm(wx, fs(a11.y, a01.y))), fa(a01.z, fm(wx, fs(a11.z, a01.z))),
-                                 fa(a01.w, fm(wx, fs(a11.w, a01.w))));
-  return make_float4(fa(top.x, fm(wy, fs(bot.x, top.x))), fa(top.y, fm(wy, fs(bot.y, top.y))), fa(top.z, fm(wy, fs(bot.z, top.z))),
-                     fa(top.w, fm(wy, fs(bot.w, top.w))));
+  const auto a00 = fetch(r0 + c0), a10 = fetch(r0 + c1), a01 = fetch(r1 + c0), a11 = fetch(r1 + c1);
+  return tap_lerp(tap_lerp(a00, a10, wx), tap_lerp(a01, a11, wx), wy);
+}
+// the four-channel tap of a float4 plane
+template <AddressMode MODE>
+OXC_DI float4 bilinear_at(const float4* src, int W, int H, float x, float y) {
+  return bilinear_fetch<MODE>([src](size_t i) { return src[i]; }, W, H, x, y);
 }
 // Sample / SampleLevel(uv) at level 0: x = u * W - 0.5 (y likewise)
 template <AddressMode MODE>
@@ -65,6 +72,12 @@ OXC_DI float4 bilinear_tap(const float4* src, int W, int H, float u, float v) {
 template <AddressMode MODE>
 OXC_DI float4 bilinear_tap(const float4* src, int W, int H, float u, float v, int dx, int dy) {
   return bilinear_at<MODE>(src, W, H, fs(fa(fm(u, (float)W), (float)dx), 0.5f), fs(fa(fm(v, (float)H), (float)dy), 0.5f));
+}
+// the one-channel sibling of bilinear_tap for an R16Unorm plane: SampleLevel(uv, 0) with texel t read as t / 65535 in binary32
+template <AddressMode MODE>
+OXC_DI float bilinear_tap_r16(const uint16_t* src, int W, int H, float u, float v) {
+  return bilinear_fetch<MODE>([src](size_t i) { return fd((float)src[i], 65535.0f); }, W, H, fs(fm(u, (float)W), 0.5f),
+                              fs(fm(v, (float)H), 0.5f));
 }
 
 // the blend of two mip levels' values: (1 - f) * lo + f * hi

@@ -8,6 +8,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
+#include <cmath>
 #include <cstring>
 #include <new>
 #include <string>
@@ -35,6 +36,7 @@
 #include "kernels_bloom.cuh"
 #include "kernels_tonemap.cuh"
 #include "kernels_fxaa.cuh"
+#include "kernels_terrain.cuh"
 
 using namespace oxc;
 
@@ -1186,6 +1188,40 @@ int oxc_cull_terrain(OxcContext* c, const OxcTerrainData* terrain, const float* 
   LAUNCHED();
   const uint32_t n = terrain->patch_count[0] * terrain->patch_count[1];
   if (n) { k_cull_terrain<<<(n + 255) / 256, 256, 0, s>>>(p); LAUNCHED(); }
+  return OXC_OK;
+}
+
+int oxc_draw_terrain(OxcContext* c, const uint16_t* heightmap_dev, uint32_t res_x, uint32_t res_y, const OxcTerrainDrawSettings* settings,
+                     const uint32_t* visible_patches_dev, const OxcDrawIndirectCommand* draw_cmd_dev, const OxcCullCamera* cam,
+                     uint32_t w, uint32_t h, uint64_t* vis_dev, void* stream) {
+  if (!c || !heightmap_dev || !settings || !visible_patches_dev || !draw_cmd_dev || !cam || !vis_dev) return fail(OXC_E_INVALID, "null argument");
+  int rc;
+  if ((rc = check_extent(w, h)) != OXC_OK) return rc;
+  if (res_x == 0 || res_y == 0 || res_x > 65536 || res_y > 65536)
+    return fail(OXC_E_INVALID, "heightmap resolution %u x %u outside 1..65536", res_x, res_y);
+  const OxcTerrainData& t = settings->terrain;
+  const uint64_t total = (uint64_t)t.patch_count[0] * t.patch_count[1];
+  if (total == 0 || total > 0xFFFFFFFFull) return fail(OXC_E_INVALID, "patch grid %u x %u is empty or above 2^32 - 1 patches", t.patch_count[0], t.patch_count[1]);
+  if (misaligned(2, heightmap_dev)) return fail(OXC_E_INVALID, "heightmap_dev is not 2-byte aligned (R16 texels)");
+  if (misaligned(4, visible_patches_dev, draw_cmd_dev)) return fail(OXC_E_INVALID, "visible_patches_dev and draw_cmd_dev must be 4-byte aligned");
+  if (misaligned(8, vis_dev)) return fail(OXC_E_INVALID, "vis_dev is not 8-byte aligned");
+  if (!std::isfinite(settings->target_edge_pixels) || !(settings->target_edge_pixels >= 1.0f))
+    return fail(OXC_E_INVALID, "target_edge_pixels %g is not a finite value >= 1", (double)settings->target_edge_pixels);
+  if (!std::isfinite(settings->max_tessellation) || !(settings->max_tessellation >= 1.0f))
+    return fail(OXC_E_INVALID, "max_tessellation %g is not a finite value >= 1", (double)settings->max_tessellation);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CK(cudaSetDevice(c->device));
+  const TerrainDrawParams p = terrain_make_params(heightmap_dev, res_x, res_y, *settings, visible_patches_dev, draw_cmd_dev, *cam, w, h,
+                                                  vis_dev, c->prim_bits);
+  // CTAs stride over the patch slots; beyond a few per SM the block scheduler's balancing gains nothing
+  const uint32_t grid = (uint32_t)std::min<uint64_t>(total, (uint64_t)c->sm_count * 16u);
+  CK(cudaMemsetAsync(c->d_big_counters, 0, 8, s));
+  k_draw_terrain<<<grid, TERRAIN_THREADS, 0, s>>>(p, c->d_big_queue, c->d_big_counters, c->big_capacity);
+  LAUNCHED();
+  TriParams tp{};
+  raster_target(c, vis_dev, w, h, &tp);
+  k_raster_big<<<c->sm_count * 8, 256, 0, s>>>(tp); // the large triangles' chunks, one warp each
+  LAUNCHED();
   return OXC_OK;
 }
 
